@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — agent-events/sec of the calfkit hot path on B200 (BASELINE.json metric).
+"""bench.py — agent-events/sec of the calfkit hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...        # the reference's CPU path (oracle port) on the host cores
+    python bench.py ... --dump-outputs DIR      # + the last timed step's outputs as DIR/<name>.npy (seeded inputs)
 
 One "step" = one pass of the tool-node hot path (decode -> ToolNodeDef.run -> _publish_action ->
 encode -> route) over one batch of `--events` synthetic 1 KB-class agent events per GPU
@@ -12,7 +13,7 @@ encode -> route) over one batch of `--events` synthetic 1 KB-class agent events 
 `e2e`       : the same through the public BatchEngine API with pinned HOST buffers — H2D of the
               batch and D2H of every payload + the publish table inside the timed region.
 `roofline`  : dominant kernel, algorithmic bytes / its CUDA-event duration (events recorded on the
-              engine's own stream inside the timed region) vs the measured HBM peak.
+              engine's own stream inside the timed region) vs the HBM peak (MEASURED_PEAKS.json, else the data sheet).
 `cpu_baseline`: the oracle port (reference algorithm on pydantic-core) on all host cores, bounded sample.
 N > 1: records shard by Kafka partition (murmur2(correlation_id) % 8 -> GPU), weak scaling; a
 fraction (--cross, default 1/8) of each rank's records arrive on the "wrong" partition (the
@@ -100,7 +101,7 @@ def bench_config(args, world: int) -> dict:
             "partitions": NUM_PARTITIONS, "cross_partition_fraction": args.cross if world > 1 else 0.0,
             "sharding": "records by Kafka partition -> GPU" if world > 1 else "single GPU",
             "tool": "device template " + repr(TOOL_FMT),
-            "l2": "inputs and outputs per step (> 1 GB each at 1 M events) far exceed the 126 MB L2: every step streams from HBM",
+            "l2": "inputs and outputs per step (> 1 GB each at 1 M events) far exceed the 50 MB L2: every step streams from HBM",
             "broker_io": "excluded on both arms (FastStream/aiokafka are not installable offline)"}
 
 
@@ -139,7 +140,7 @@ def run_reference(args, rank: int, world: int) -> None:
 
 
 def hbm_peak_gbs():
-    """-> (GB/s, where it came from): the driver-written measurement if present and sane, else the profiling guide's fallback"""
+    """-> (GB/s, where it came from): the driver-written measurement if present and sane, else the data-sheet figure"""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         v = float(json.load(open(path))["hbm_gbs"])
@@ -147,7 +148,7 @@ def hbm_peak_gbs():
             return v, "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:  # noqa: BLE001  (absent / unreadable / other schema)
         pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s at 700 W; not measured)"
 
 
 # ------------------------------------------------------------------------------------------------ helpers
@@ -164,12 +165,16 @@ class ClockSampler(threading.Thread):
     def __init__(self, index: int):
         super().__init__(daemon=True)
         self.index, self.samples, self.reasons, self.stop_flag, self.max_mhz = index, [], set(), False, None
+        self.gpu = self.power_limit_w = None
         try:
             import pynvml
             pynvml.nvmlInit()
             self.nv = pynvml
             self.dev = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.dev, pynvml.NVML_CLOCK_SM)
+            self.gpu = pynvml.nvmlDeviceGetName(self.dev)
+            self.gpu = self.gpu.decode() if isinstance(self.gpu, bytes) else self.gpu
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.dev) / 1000
         except Exception:
             self.nv = None
 
@@ -195,8 +200,51 @@ class ClockSampler(threading.Thread):
 
     def summary(self):
         s = sorted(self.samples)
-        return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
-                "samples": len(s)}
+        return {"gpu": self.gpu, "power_limit_w": self.power_limit_w, "sm_mhz": s[len(s) // 2] if s else None,
+                "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(s)}
+
+
+def dump_outputs(eng, path: str) -> None:
+    """--dump-outputs: what the engine's last plan produced, as float .npy files under 64 MB in all, so that two builds
+    can be compared output for output: length and CRC-32 of every payload, the first 1 KB of a seeded sample of payloads
+    (chosen by index only; -1 pads), the publish table and per-record status / action.  A table longer than its cap is a
+    seeded sample of rows, listed in <name>_index.npy."""
+    import zlib
+    import numpy as np
+    from calfkit.engine._lib import COL
+    out, off, ln, pubs = eng._fetch()
+    cols = eng.columns()
+    rng = np.random.default_rng(0)
+    arrays = {}
+
+    def rows(name: str, m: int, cap: int) -> np.ndarray:
+        if m <= cap:
+            return np.arange(m)
+        idx = np.sort(rng.choice(m, size=cap, replace=False))
+        arrays[name + "_index"] = idx.astype(np.float64)
+        return idx
+
+    mv = memoryview(out)
+    pr = rows("payload", len(ln), 1 << 20)
+    arrays["payload_len"] = ln[pr].astype(np.float32)
+    arrays["payload_crc32"] = np.array([zlib.crc32(mv[off[i]:off[i] + ln[i]]) for i in pr], dtype=np.float64)
+    take = np.sort(rng.choice(len(ln), size=min(len(ln), 4096), replace=False))
+    head = np.full((len(take), 1024), -1.0, dtype=np.float32)
+    for j, i in enumerate(take):
+        k = min(int(ln[i]), 1024)
+        head[j, :k] = out[off[i]:off[i] + k]
+    arrays["payload_sample_index"], arrays["payload_sample_head"] = take.astype(np.float64), head
+    fields = ("payload", "topic_id", "topic_off", "topic_len", "record", "has_key", "partition")
+    pi = rows("publishes", len(pubs), 1 << 17)
+    arrays["publishes"] = np.stack([pubs[f][pi].astype(np.float64) for f in fields], axis=1) if len(pi) \
+        else np.zeros((0, len(fields)), np.float64)
+    ri = rows("record", cols.shape[1], 1 << 20)
+    arrays["record_status"], arrays["record_action"] = (cols[COL[c]][ri].astype(np.float32) for c in ("STATUS", "ACTION"))
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, total
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 class CudaArray:
@@ -314,6 +362,8 @@ def run_fanout(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) -
     eng.profile(False)
     out_bytes, npay, npub = eng.out_size()
     value = world * n / (ms_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     # end to end: pinned host in -> device -> pinned host out
     h_in = torch.from_numpy(batch.data.copy()).pin_memory()
     h_off = torch.from_numpy(batch.offsets.copy()).pin_memory()
@@ -328,7 +378,7 @@ def run_fanout(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) -
         o, of, ln, pb = eng._fetch(out_buf=h_out.numpy(), off_buf=h_o, len_buf=h_l, pubs_buf=h_p)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    e2e_steps = 3
+    e2e_steps = args.steps
     for k in range(e2e_steps):
         eng.submit(h_in.numpy(), h_off.numpy()); eng.fanout_plan(ms0, 1, max_fanout=256)
         o, of, ln, pb = eng._fetch(out_buf=h_out.numpy(), off_buf=h_o, len_buf=h_l, pubs_buf=h_p)
@@ -462,13 +512,15 @@ def run_reply(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) ->
     eng.profile(False)
     out_bytes, npay, _npub = eng.out_size()
     value = world * n / (ms_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     h_in = torch.from_numpy(batch.data.copy()).pin_memory()
     h_off = torch.from_numpy(batch.offsets.copy()).pin_memory()
     h_out = torch.empty(out_bytes + (1 << 20), dtype=torch.uint8).pin_memory()
     h_o = torch.empty(npay + 1, dtype=torch.int64).pin_memory().numpy()
     h_l = torch.empty(npay, dtype=torch.int32).pin_memory().numpy().view(np.uint32)
     d2h = 0
-    e2e_steps = 4
+    e2e_steps = args.steps
     for k in range(2 + e2e_steps):
         if k == 2:
             torch.cuda.synchronize()
@@ -582,6 +634,8 @@ def run_mixed(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) ->
     eng.profile(False)
     out_bytes, npay, npub = eng.out_size()
     value = world * n / (ms_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     from calfkit.engine.lane import Arena, LanePipeline
     pipe = LanePipeline(local_rank, lambda e_: (e_.register_topics(topics, num_partitions=NUM_PARTITIONS),
                                                 e_.set_tool_node("tool.get_weather.output", ToolTemplate.from_format(TOOL_FMT)), e_.set_bucketing(True)),
@@ -589,7 +643,7 @@ def run_mixed(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) ->
     h_in = torch.from_numpy(batch.data.copy()).pin_memory()
     h_off = torch.from_numpy(batch.offsets.copy()).pin_memory()
     arena = Arena(h_in.numpy(), h_off.numpy())
-    d2h, e2e_steps = 0, 8
+    d2h, e2e_steps = 0, args.steps
     for k in range(3 + e2e_steps):
         if k == 3:
             for pb in pipe.drain():
@@ -661,7 +715,7 @@ def run_mixed(args, rank, world, local_rank, dev, real_stdout, all_cpus=None) ->
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps of every leg (device-resident and end to end)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--events", type=int, default=1_000_000, help="events per GPU per step (config 2: 1M)")
@@ -670,7 +724,11 @@ def main() -> None:
     ap.add_argument("--workload", default="tool_event_1k", choices=["tool_event_1k", "fanout", "reply", "mixed"],
                     help="tool_event_1k = BASELINE.json configs[1] (the headline); fanout = configs[2]: 1 Agent -> 64 tools")
     ap.add_argument("--fanout", type=int, default=64)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     if args.impl == "reference":
@@ -878,6 +936,8 @@ def main() -> None:
     ms_total = float(t.item())
     ms_step = ms_total / args.steps
     value = world * n / (ms_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(lanes[(args.steps - 1) % len(lanes)].eng, args.dump_outputs)
 
     # ---- end to end (host buffers), pipelined over several engines (3 at N = 1, 2 at N > 1) -----------------
     # step k: lane k%2 takes the batch from pinned host memory (H2D + all kernels, asynchronous) while the
@@ -886,7 +946,7 @@ def main() -> None:
     if world == 1:
         lanes = [lane, Lane(), Lane()]          # triple buffering: the D2H of step k-2 never waits for kernels
     h_in_np, h_off_np = h_in.numpy(), h_off.numpy()
-    e2e_steps = max(4, min(args.steps, 8))
+    e2e_steps = args.steps
 
     def run_e2e(k_steps):
         if world == 1:
@@ -1001,7 +1061,7 @@ def main() -> None:
     for _ in range(3):
         w_client.broker.produce_arena("tool.get_weather.input", w_arena)
     asyncio.run(worker.run(until_idle=True))
-    w_steps = max(8, min(2 * args.steps, 16))
+    w_steps = args.steps
     w_cnt["pubs"] = 0
     for _ in range(w_steps):
         w_client.broker.produce_arena("tool.get_weather.input", w_arena)

@@ -1,8 +1,8 @@
-"""calfkit-b200: Blackwell-native drop-in for the data-parallel hot path of calf-ai/calfkit-sdk.
+"""calfkit-b200: H100-native drop-in for the data-parallel hot path of calf-ai/calfkit-sdk.
 
 Keeps the reference's public surface for that path (reference calfkit/__init__.py:10-30):
 Client, Worker, Agent, agent_tool, ToolContext ... and puts a ctypes C-ABI over hand-written
-sm_100a CUDA kernels underneath (see DESIGN.md)."""
+sm_90a CUDA kernels underneath (see DESIGN.md)."""
 __version__ = "0.1.0"
 
 _LAZY = {

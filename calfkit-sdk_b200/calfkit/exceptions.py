@@ -4,7 +4,7 @@ class DeserializationError(Exception):
 
 
 class EngineError(RuntimeError):
-    """The B200 batch engine reported a failure (missing CUDA library, CUDA error, ...).
+    """The GPU batch engine reported a failure (missing CUDA library, CUDA error, ...).
     There is no CPU fallback: the engine fails loudly instead."""
 
 

@@ -40,7 +40,7 @@ class BaseNodeDef(BaseNodeSchema):
     # ---- batch path (what Worker.run drives) -----------------------------------------------------
     def configure_engine(self, engine) -> None:
         """load this node's routing/tool configuration into a BatchEngine"""
-        raise NotImplementedError(f"{type(self).__name__} has no batch plan: the B200 worker accelerates the node kinds "
+        raise NotImplementedError(f"{type(self).__name__} has no batch plan: the GPU worker accelerates the node kinds "
                                   "the reference ships (@agent_tool nodes, Agent); custom run() bodies are out of scope")
 
     def process_batch(self, engine, records: list[Record]) -> list[Record]:

@@ -18,6 +18,7 @@ static thread_local std::string g_create_error;
 
 struct ck_handle {
     int device = 0;
+    u32 num_sms = 0;                 // grid size of the grid-stride kernels: a fixed number of blocks per SM
     cudaStream_t stream = nullptr;
     cudaStream_t xstream = nullptr; cudaEvent_t x_ev0 = nullptr, x_ev1 = nullptr;   // high-priority side stream of the exchange
     std::string err;
@@ -114,7 +115,8 @@ extern "C" int ck_create(int device, uint64_t max_in_bytes, uint64_t max_out_byt
     if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return bail("cudaGetDeviceProperties", e);
-    if (prop.major != 10) { g_create_error = "ck_create: this library is built for sm_100a (B200) only"; ck_destroy(h); return 1; }
+    if (prop.major != 9 || prop.minor != 0) { g_create_error = "ck_create: this library is built for sm_90a (H100) only"; ck_destroy(h); return 1; }
+    h->num_sms = (u32)prop.multiProcessorCount;
     if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
     {   // the canonicaliser is (boundedly) recursive: give device threads room for its frames
         size_t cur = 0; cudaDeviceGetLimit(&cur, cudaLimitStackSize);
@@ -332,7 +334,7 @@ static int launch_decode(ck_handle* h) {
         // Both kernels exit at once when there are no such records.
         KTimer t(h, CK_K_WALK_LONG);
         CKL(h) ck_classify_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(v, n, h->d_cand);
-        u32 lblocks = (n + CK_LONG_WARPS - 1) / CK_LONG_WARPS; if (lblocks > 148 * CK_LONG_MINB) lblocks = 148 * CK_LONG_MINB;
+        u32 lblocks = (n + CK_LONG_WARPS - 1) / CK_LONG_WARPS; if (lblocks > h->num_sms * CK_LONG_MINB) lblocks = h->num_sms * CK_LONG_MINB;
         CKL(h) ck_walk_long_kernel<<<lblocks, 32 * CK_LONG_WARPS, CK_LONG_WARPS * sizeof(ck_long_index), h->stream>>>(v, h->d_cols, n, h->d_cand, h->d_hist_skip);
         CUDA_TRY(h, cudaGetLastError());
     }
@@ -346,14 +348,14 @@ static int launch_decode(ck_handle* h) {
         // the history messages listed by the pre-scan or deferred by the long walker, one thread each (exits at once when
         // there are none)
         KTimer t(h, CK_K_WALK_ELEMS);
-        CKL(h) ck_walk_elems_kernel<<<148 * CK_WALK_MINB, CK_WALK_THREADS, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, h->d_cols, n);
+        CKL(h) ck_walk_elems_kernel<<<h->num_sms * CK_WALK_MINB, CK_WALK_THREADS, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, h->d_cols, n);
         CUDA_TRY(h, cudaGetLastError());
     }
     {
         // the records the walker listed (usually none: both kernels exit at once) are re-emitted canonically into the
         // overlay and walked again in that spelling
         KTimer t(h, CK_K_CANON);
-        u32 blocks = (n + 63) / 64; if (blocks > 148 * 8) blocks = 148 * 8;
+        u32 blocks = (n + 63) / 64; if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
         CKL(h) ck_canon_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols, n, h->d_ovl, (long long)h->max_ovl, h->d_ovl_off, h->d_ovl_len);
         CKL(h) ck_rewalk_list_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols, n);
         CUDA_TRY(h, cudaGetLastError());
@@ -952,7 +954,7 @@ static int exchange_send_on_stream(ck_handle* h, uint64_t step) {
         KTimer t(h, CK_K_EMIT);
         // barrier 1: every peer has consumed what it received last time (its own stream order puts that before this point)
         CKL(h) ck_xbarrier_kernel<<<1, 32, 0, h->stream>>>(h->peers, rank, world, flags_off, 0, step, h->d_x_overflow + CK_X_MAXWORLD);
-        if (npubs) CKL(h) ck_xsend_kernel<<<148 * 4, 256, 0, h->stream>>>(h->d_pubs, h->d_x_pub, h->d_x_src_off, h->d_x_len32, h->d_x_dst_off, h->d_x_base, nb,
+        if (npubs) CKL(h) ck_xsend_kernel<<<h->num_sms * 4, 256, 0, h->stream>>>(h->d_pubs, h->d_x_pub, h->d_x_src_off, h->d_x_len32, h->d_x_dst_off, h->d_x_base, nb,
             h->d_x_grand, h->d_out, h->peers, rank, world, h->region_stride, h->max_fwd, h->region_data_cap, h->d_x_overflow);
         CKL(h) ck_xhdr_kernel<<<1, 32, 0, h->stream>>>(h->d_x_dst_off, h->d_x_base, nb, h->d_x_grand, h->peers, rank, world, h->region_stride, step, h->d_x_overflow);
         // barrier 2: everybody's stores (to everybody) have landed

@@ -3,14 +3,14 @@
 // Reference: Agent.run's list[Call] branch (calfkit/nodes/agent.py:177-211) + _publish_action (nodes/base.py:73-88).
 // Round 1 ran one thread per record: with 64 pending calls per 20 KB record that thread walked tool_calls once per pass,
 // looked every key up in tool_results by walking that dict again (O(F^2) bytes) and searched the tool registry linearly
-// per call — 2 x 3.5 ms for 4096 records, 60 % of the config-3 step, on 128 warps.  Here a warp owns a record: lane 0
+// per call — most of the config-3 step, on only 128 warps.  Here a warp owns a record: lane 0
 // indexes the two dicts once into shared memory (key span, value span, 32-bit key hash), then the lanes take one tool
 // call each: pending test against the hashed tool_results keys, registry lookup by name hash, and the splice descriptor
 // of their own Call envelope (same SegWriter, same bytes as before).
 // The index itself is built by the whole warp too: the structural pre-scan of ck_walk_long.cuh proposes the entry
 // boundaries of both dicts, every lane parses its own entry and checks that it ends exactly where the next one starts and
 // that the dict closes where the walker's column says; only if that chain does not hold does lane 0 index sequentially
-// (a 20 KB record: 1.9 ms per kernel that way, measured).
+// (milliseconds for a 20 KB record).
 #ifndef CK_FANOUT2_CUH
 #define CK_FANOUT2_CUH
 

@@ -39,7 +39,8 @@ struct ck_key_pub {
 struct ck_key_len {
     ck_view v;
     // longest first: the walk's blocks start in this order, so the records that take longest start first and the short ones
-    // fill in behind them (a 16 KB record alone takes a thread ~0.5 ms; started last it would be the kernel's tail)
+    // fill in behind them (a 16 KB record alone keeps a thread busy far longer than a short one; started last it would be
+    // the kernel's tail)
     __device__ __forceinline__ u32 operator()(u32 i) const { u32 len; ck_rec_in(v, i, len); u32 k = len >> 5; return CK_G_KEYS - 1 - (k < CK_G_KEYS - 1 ? k : CK_G_KEYS - 1); }
 };
 

@@ -1,4 +1,4 @@
-// sm_100a kernels of the calfkit-b200 hot path.  No tensor cores: the path has no dense
+// sm_90a (H100) kernels of the calfkit-b200 hot path.  No tensor cores: the path has no dense
 // contraction; everything here is HBM-bound byte/integer work (DESIGN.md §kernels).
 //
 //   ck_walk_kernel        decode: prove each record is a canonical Envelope + extract spans   (a2,a3,a4)
@@ -27,7 +27,7 @@ extern __shared__ uint4 ck_win_smem[];   // nvcc's host pass parses the device c
 #define CK_HIST_MIN 2048u        // records at least this long get the message_history pre-scan (ck_walk_long.cuh)
 #endif
 #ifndef CK_LONG_MIN
-#define CK_LONG_MIN 16384u       // records at least this long are walked one per warp (ck_walk_long.cuh); measured: §7 of DESIGN.md
+#define CK_LONG_MIN 16384u       // records at least this long are walked one per warp (ck_walk_long.cuh)
 #endif
 // per-batch counters (zeroed by launch_decode): overlay bytes handed out; records listed for the canonicaliser; list elements
 // deferred to ck_walk_elems_kernel (may exceed the capacity: clamp); records listed for the warp-per-record pass / handed out

@@ -1,11 +1,10 @@
 // Tool-node plan, staged through shared memory (replaces the thread-per-record ck_plan_tool_kernel for modes 1 / 2
 // and the separate ck_route_kernel launch behind it).
 //
-// Why (ncu, profiles/r01_plan_tool.txt): the first version issued ~150 dependent, lane-divergent global loads per
-// warp (byte / 8-byte reads of ten far-apart spots of each record) and 80 lane-divergent store instructions
-// (28 sectors per request: the 144 B descriptor, the 512 B-stride glue slot and the two 32 B publishes written
-// array-of-structs by one thread each) — latency bound at 17 % issue utilisation with 6.3x the algorithmic DRAM
-// traffic.  Here
+// Why: the first version issued ~150 dependent, lane-divergent global loads per warp (byte / 8-byte reads of ten
+// far-apart spots of each record) and 80 lane-divergent store instructions (the 144 B descriptor, the 512 B-stride
+// glue slot and the two 32 B publishes written array-of-structs by one thread each, so most sectors of every store
+// request were partial) — latency bound, moving several times the algorithmic DRAM traffic.  Here
 //   * every record read goes through a 64-byte per-thread window in shared memory filled by 16-byte cp.async copies
 //     (no data registers; one memory round trip per 48 fresh bytes instead of one per 8),
 //   * glue text, descriptor and the two publishes are assembled in shared memory and written to HBM by the whole

@@ -187,8 +187,8 @@ struct URd : GRd {
 // Window reader (the walker's): each thread stages CK_WIN_BYTES of its record in shared memory with
 // 16-byte asynchronous copies (cp.async, no data registers, all chunks of a refill in flight at once)
 // and reads bytes / unaligned words from there.  Thirty-two lanes walking thirty-two different records
-// cost one L1 tag lookup per lane per *load instruction* through global memory (the measured bound of the
-// GRd walker, DESIGN.md section 7); through shared memory a warp-wide access is one wavefront unless banks
+// cost one L1 tag lookup per lane per *load instruction* through global memory (what bounds the GRd
+// walker); through shared memory a warp-wide access is one wavefront unless banks
 // collide, and the global side shrinks to len/16 chunk copies per record.  Every access checks the
 // window and refills on demand (re-centred CK_WIN_BACK bytes behind the position), so correctness does not
 // depend on access order.  The window base is the reader's state; it travels through out-of-line
@@ -301,7 +301,7 @@ struct WRd {
 struct WRdT : WRd { static const bool kTrustFloats = true; };
 struct GRdT : GRd { static const bool kTrustFloats = true; };
 
-// Look-ahead prefetch of the record stream into L1 (experiment knob, DESIGN.md §7): every lane walks its
+// Look-ahead prefetch of the record stream into L1 (experiment knob, off by default): every lane walks its
 // own record, so almost every warp-level load has some lane missing L1; pulling the line CK_PF_DIST
 // bytes ahead turns those into hits.  CK_PF: 0 off, 1 once per 128 B line (entry lands in its first
 // 32 B), 2 unconditional, 4 = 1 with a dummy load instead of prefetch.global.L1.

@@ -1,8 +1,8 @@
 // Long records: one warp per record, intra-record parallelism (see the block comment in ck_walk.cuh above ck_long_index).
 //
 // Why: a schema walk is sequential per record, so one thread per record takes (record length) x (~100-200 cycles per byte)
-// no matter how idle the machine is — a 20 KB fan-out record 2.8 ms, a 64 KB history 5 ms (round 1: config 3 walk at 0.6 %
-// of the HBM roofline, config 5 at 1.8 %).  Long records are long because of LISTS (64 tool calls, 64 parts, dozens of
+// no matter how idle the machine is: milliseconds for a 20 KB fan-out record or a 64 KB history, a few percent of the HBM
+// roofline for configs 3 and 5.  Long records are long because of LISTS (64 tool calls, 64 parts, dozens of
 // messages): their elements are independent given the boundaries.
 //   ck_lx_build          warp-parallel structural pre-scan, 512 bytes per iteration (16 per lane): byte-class bit masks by
 //                        SIMD-in-word compares, escaped quotes from the backslash runs, string mask by prefix XOR (within
@@ -170,7 +170,7 @@ __device__ __forceinline__ void ck_lx_build(const u8* __restrict__ g, u32 n, ck_
 #define CK_ELEM_MAX 4096u           // longer messages stay with their record's warp (their parts are walked lane-parallel there)
 #endif
 #ifndef CK_LONG_MINB
-#define CK_LONG_MINB 6          // <= 80 registers: 24 warps per SM (measured on the mixed workload: 3.6 ms against 5.3 ms at 16 warps)
+#define CK_LONG_MINB 6          // <= 80 registers: 24 warps per SM (the warp walk is latency bound: more warps hide more of it than 16 do)
 #endif
 __global__ void __launch_bounds__(32 * CK_LONG_WARPS, CK_LONG_MINB)
 ck_walk_long_kernel(ck_view v, u32* __restrict__ cols, u32 stride, const u32* __restrict__ cand, uint2* __restrict__ hist_skip) {

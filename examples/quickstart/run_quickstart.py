@@ -1,5 +1,5 @@
 """BASELINE.json configs[0]: the reference's quickstart (examples/quickstart/{weather_tool,agent_service,
-invoke}.py) — weather_agent + get_weather tool, 100 events — on the B200 worker.
+invoke}.py) — weather_agent + get_weather tool, 100 events — on the GPU worker.
 
 Differences from the reference scripts, all outside the hot path: the three processes share one
 in-memory broker (no Kafka broker in the image) and the LLM is a deterministic function model

@@ -1,4 +1,4 @@
-/* calfkit_b200.h — C-ABI of libcalfkit_b200.so (sm_100a).
+/* calfkit_b200.h — C-ABI of libcalfkit_b200.so (sm_90a, H100).
  *
  * The reference (calf-ai/calfkit-sdk v0.2.5) has no FFI for this path: its per-record hot loop is
  *   FastStream decoder -> Envelope validation      calfkit/nodes/base.py:151, calfkit/models/envelope.py:9-17

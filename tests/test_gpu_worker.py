@@ -1,4 +1,4 @@
-"""Config 1 (BASELINE.json configs[0]) end to end on the B200 worker: quickstart weather agent +
+"""Config 1 (BASELINE.json configs[0]) end to end on the GPU worker: quickstart weather agent +
 get_weather tool, 100 events through Client -> Worker.run -> Agent/ToolNode batch plans -> reply."""
 import asyncio
 import importlib.util
