@@ -131,8 +131,11 @@ __device__ __forceinline__ void ck_walk_one(ck_view v, u32 n, u32* __restrict__ 
         v.canon_list[k] = i;
     }
 }
+// 6 blocks of 128 threads per SM: <= 80 registers (at 64 the walker spills about twice as much) and room for the
+// CK_WIN_BYTES = 224 windows.  Measured on H100 against 8 blocks with 160-byte windows: config-2 walk 1.30 -> 1.14 ms
+// (DESIGN.md §7)
 #ifndef CK_WALK_MINB
-#define CK_WALK_MINB 8
+#define CK_WALK_MINB 6
 #endif
 // records long enough for the history pre-scan (ck_hist_prescan_kernel), listed with one atomic per warp
 __global__ void __launch_bounds__(256)

@@ -194,8 +194,10 @@ struct URd : GRd {
 // depend on access order.  The window base is the reader's state; it travels through out-of-line
 // calls by value (cores return it next to their result).
 // -------------------------------------------------------------------------------------------------
+// 224 bytes: a 1.15 KB record takes about six refills, each a full round trip on the thread's critical path.  The 240-byte
+// slot (15 x 16 B) x 128 threads x CK_WALK_MINB (6) blocks is 180 KB of shared memory per SM
 #ifndef CK_WIN_BYTES
-#define CK_WIN_BYTES 160
+#define CK_WIN_BYTES 224
 #endif
 #define CK_WIN_BACK 16
 #ifndef CK_WIN_L2PF
@@ -1187,21 +1189,96 @@ struct WalkOut {
 
 #define SETSPAN(COL, a, b) do { o.set(COL, (a)); o.set(COL + 1, (b) - (a)); } while (0)
 
+// key `ko` (content offset) of the record equal to bytes [a, a + len): the closing quote, then the bytes (plain global
+// loads: two far-apart spans)
+CK_HD bool ck_key_is(const u8* g, u32 n, u32 ko, u32 a, u32 len) {
+    GRd gr, gq; gr.init(g, n); gq.init(g, n);
+    if (ko + len >= n || gr.at(ko + len) != '"') return false;
+    return ck_spans_equal(gr, ko, gq, a, len);
+}
+
+// keys of one id-keyed dict (tool_calls / tool_results): 32-bit hash (uniqueness check: the reference holds Python
+// dicts) + content offset, so that dict[input_args[0]] can be resolved at the end of the walk.  Up to CK_DICT_KEYS
+// entries.  A thread walking its record keeps the first CK_DICT_REG keys in registers (statically indexed: no local
+// memory) and finds the later ones again by re-scanning the dict from key CK_DICT_REG (values already validated:
+// ck_skip_value) — quadratic, but only dicts of more than CK_DICT_REG entries pay it.  A warp walking one record keeps
+// the whole table in shared memory (ck_long_index), where its lanes fill it in parallel.
+#ifndef CK_DICT_REG
+#define CK_DICT_REG 2
+#endif
+template <class R, bool kShared = R::kWarp>
+struct DictKeys {
+    u32 kh[CK_DICT_REG], koff[CK_DICT_REG];
+    u32 n;           // entries so far
+    u32 more;        // opening quote of key CK_DICT_REG
+    CK_HD void init(u32*, u32*) { n = 0; more = 0; }
+    // does key k (k >= CK_DICT_REG) hash to h?  Calls fn(k, content offset) for each such key until it returns true
+    template <class F>
+    CK_HD bool scan_more(R& r, u32 h, F fn) {
+        u32 p = more;
+        for (u32 k = CK_DICT_REG; k < n; k++) {
+            u32 q = p;
+            ck_skip_value(r, p);                               // the key string
+            if (ck_hash_span(r, q + 1, p - q - 2) == h && fn(q + 1)) return true;
+            p++;                                               // ':'
+            ck_skip_value(r, p);                               // the value
+            p++;                                               // ','
+        }
+        return false;
+    }
+    // record key `off` with hash h; false: a duplicate (or a hash collision) or too many entries
+    CK_HD bool add(R& r, u32 h, u32 off) {
+        bool dup = false;
+#pragma unroll
+        for (u32 k = 0; k < CK_DICT_REG; k++) dup |= (k < n) & (kh[k] == h);
+        if (dup || n >= CK_DICT_KEYS) return false;
+        if (n > CK_DICT_REG && scan_more(r, h, [](u32) { return true; })) return false;
+#pragma unroll
+        for (u32 k = 0; k < CK_DICT_REG; k++) if (k == n) { kh[k] = h; koff[k] = off; }
+        if (n == CK_DICT_REG) more = off - 1;
+        n++;
+        return true;
+    }
+    // index of the first key equal to bytes [a, a + len) (hash h), ~0u if none; ko = its content offset
+    CK_HD u32 find(R& r, u32 h, u32 a, u32 len, u32& ko) {
+#pragma unroll
+        for (u32 k = 0; k < CK_DICT_REG; k++)
+            if (k < n && kh[k] == h && ck_key_is(r.g, r.n, koff[k], a, len)) { ko = koff[k]; return k; }
+        u32 hit = ~0u;
+        if (n > CK_DICT_REG) scan_more(r, h, [&](u32 off) { if (!ck_key_is(r.g, r.n, off, a, len)) return false; ko = off; hit = CK_DICT_REG; return true; });
+        return hit;
+    }
+};
+template <class R>
+struct DictKeys<R, true> {
+    u32 *kh, *koff;
+    u32 n;
+    CK_HD void init(u32* h, u32* off) { kh = h; koff = off; n = 0; }
+    CK_HD bool add(R&, u32 h, u32 off) {
+        for (u32 k = 0; k < n; k++) if (kh[k] == h) return false;
+        if (n >= CK_DICT_KEYS) return false;
+        kh[n] = h; koff[n] = off; n++;
+        return true;
+    }
+    CK_HD u32 find(R& r, u32 h, u32 a, u32 len, u32& ko) {
+        for (u32 k = 0; k < n; k++)
+            if (kh[k] == h && ck_key_is(r.g, r.n, koff[k], a, len)) { ko = koff[k]; return k; }
+        return ~0u;
+    }
+};
+
 template <class R>
 CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     u32 pos = 0;
     Span t;
     stop = 0;
-    // keys of the two id-keyed dicts: 32-bit hash (uniqueness check: the reference holds Python dicts)
-    // + span, so that tool_calls[input_args[0]] / tool_results[...] can be resolved at the end of the
-    // walk without scanning the dicts again
-    u32 tc_kh_l[CK_DICT_KEYS], tc_koff_l[CK_DICT_KEYS], tc_n = 0;     // key length is re-derived from the closing quote
-    u32 tr_kh_l[CK_DICT_KEYS], tr_koff_l[CK_DICT_KEYS], tr_n = 0;
-    u32 *tc_kh = tc_kh_l, *tc_koff = tc_koff_l, *tr_kh = tr_kh_l, *tr_koff = tr_koff_l;
+    // keys of the two id-keyed dicts (DictKeys), so that tool_calls[input_args[0]] / tool_results[...] can be resolved
+    // at the end of the walk; the key length is re-derived from the closing quote
+    DictKeys<R> tck, trk;
     if constexpr (R::kWarp) {          // a warp on one record: the lanes share the key tables (shared memory)
         ck_long_index* lw = r.lxw();
-        tc_kh = lw->kh[0]; tc_koff = lw->koff[0]; tr_kh = lw->kh[1]; tr_koff = lw->koff[1];
-    }
+        tck.init(lw->kh[0], lw->koff[0]); trk.init(lw->kh[1], lw->koff[1]);
+    } else { tck.init(nullptr, nullptr); trk.init(nullptr, nullptr); }
     ToolCallSpans first_tc = {{0, 0}, {0, 0}, {0, 0}};
     u32 first_tc0 = 0, first_tc1 = 0, first_tr0 = 0, first_tr1 = 0;
 #define FAIL do { stop = pos; return false; } while (0)
@@ -1229,7 +1306,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
                         v0 = p;
                         ok = ok && ck_tool_call_part(lr, p, 5, cx, tc) == 1 && p == tend;
                         v1 = p;
-                        if (ok) { tc_kh[e] = ck_hash_span(lr, key.off, key.len); tc_koff[e] = key.off; }
+                        if (ok) { tck.kh[e] = ck_hash_span(lr, key.off, key.len); tck.koff[e] = key.off; }
                     }
                     good = ck_all(ok) && good;
                     if (base == 0) {       // entry 0 (lane 0 of the first round): the common single-call case needs no second look
@@ -1242,9 +1319,9 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
                 if (!good) FAIL;
                 ck_warp_sync();
                 bool dup = false;
-                for (u32 e = ck_lane(); e <= k; e += 32) for (u32 j = 0; j < e; j++) dup |= (tc_kh[j] == tc_kh[e]);
+                for (u32 e = ck_lane(); e <= k; e += 32) for (u32 j = 0; j < e; j++) dup |= (tck.kh[j] == tck.kh[e]);
                 if (!ck_all(!dup)) FAIL;
-                tc_n = k + 1; pos = q;
+                tck.n = k + 1; pos = q;
             }
         }
         if (!par) {
@@ -1252,15 +1329,12 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
         // 32-bit hashes of the raw key bytes, a (vanishingly rare) collision only costs the fast path
         for (;;) {
             if (!ck_string(r, pos, t)) FAIL;
-            u32 h = ck_hash_span(r, t.off, t.len);
-            for (u32 k = 0; k < tc_n; k++) if (tc_kh[k] == h) FAIL;
-            if (tc_n >= CK_DICT_KEYS) FAIL;
-            tc_kh[tc_n] = h; tc_koff[tc_n] = t.off; tc_n++;
+            if (!tck.add(r, ck_hash_span(r, t.off, t.len), t.off)) FAIL;
             ToolCallSpans tc;
             if (!M(":")) FAIL;
             u32 v0 = pos;
             if (ck_tool_call_part(r, pos, 5, cx, tc) != 1) FAIL;
-            if (tc_n == 1) { first_tc = tc; first_tc0 = v0; first_tc1 = pos; }      // the common single-call case needs no second look
+            if (tck.n == 1) { first_tc = tc; first_tc0 = v0; first_tc1 = pos; }      // the common single-call case needs no second look
             if (PEEK(',')) { pos++; continue; }
             break;
         }
@@ -1300,7 +1374,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
                         v0 = p;
                         ok = ok && ck_tool_result_value(lr, p, 5, cx) && p == tend;
                         v1 = p;
-                        if (ok) { tr_kh[e] = ck_hash_span(lr, key.off, key.len); tr_koff[e] = key.off; }
+                        if (ok) { trk.kh[e] = ck_hash_span(lr, key.off, key.len); trk.koff[e] = key.off; }
                     }
                     good = ck_all(ok) && good;
                     if (base == 0) { first_tr0 = ck_bcast(v0, 0); first_tr1 = ck_bcast(v1, 0); }
@@ -1308,22 +1382,19 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
                 if (!good) FAIL;
                 ck_warp_sync();
                 bool dup = false;
-                for (u32 e = ck_lane(); e <= k; e += 32) for (u32 j = 0; j < e; j++) dup |= (tr_kh[j] == tr_kh[e]);
+                for (u32 e = ck_lane(); e <= k; e += 32) for (u32 j = 0; j < e; j++) dup |= (trk.kh[j] == trk.kh[e]);
                 if (!ck_all(!dup)) FAIL;
-                tr_n = k + 1; pos = q;
+                trk.n = k + 1; pos = q;
             }
         }
         if (!par) {
         for (;;) {
             if (!ck_string(r, pos, t)) FAIL;
-            u32 h = ck_hash_span(r, t.off, t.len);
-            for (u32 k = 0; k < tr_n; k++) if (tr_kh[k] == h) FAIL;
-            if (tr_n >= CK_DICT_KEYS) FAIL;
-            tr_kh[tr_n] = h; tr_koff[tr_n] = t.off; tr_n++;
+            if (!trk.add(r, ck_hash_span(r, t.off, t.len), t.off)) FAIL;
             if (!M(":")) FAIL;
             u32 v0 = pos;
             if (!ck_tool_result_value(r, pos, 5, cx)) FAIL;
-            if (tr_n == 1) { first_tr0 = v0; first_tr1 = pos; }
+            if (trk.n == 1) { first_tr0 = v0; first_tr1 = pos; }
             if (PEEK(',')) { pos++; continue; }
             break;
         }
@@ -1547,32 +1618,24 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     Span tn = {0, 0}, ar = {0, 0};
     if (nframes > 0 && top_nargs == 2 && (top_kinds & 1u)) {
         u32 h = ck_hash_span(r, top_a0.off, top_a0.len);
-        GRd gr, gq; gr.init(r.g, r.n); gq.init(r.g, r.n);      // compares of two far-apart spans: plain global loads
-        // the hash covers the length, so a hit is (almost surely) the key: verify bytes + closing quote
-        for (u32 k = 0; k < tc_n; k++) {
-            if (tc_kh[k] != h) continue;
-            u32 ko = tc_koff[k];
-            if (ko + top_a0.len >= r.n || gr.at(ko + top_a0.len) != '"') continue;
-            if (!ck_spans_equal(gr, ko, gq, top_a0.off, top_a0.len)) continue;
-            if (k == 0) { call0 = first_tc0; call1 = first_tc1; tn = first_tc.tool_name; ar = first_tc.args; break; }
+        // the hash covers the length, so a hit is (almost surely) the key: find() verifies bytes + closing quote
+        u32 ko = 0;
+        u32 k = tck.find(r, h, top_a0.off, top_a0.len, ko);
+        if (k == 0) { call0 = first_tc0; call1 = first_tc1; tn = first_tc.tool_name; ar = first_tc.args; }
+        else if (k != ~0u) {
             u32 p2 = ko + top_a0.len + 2;
             call0 = p2;
             ToolCallSpans tcs;
             ck_tool_call_part(r, p2, 5, cx, tcs);
             call1 = p2; tn = tcs.tool_name; ar = tcs.args;
-            break;
         }
-        for (u32 k = 0; k < tr_n; k++) {
-            if (tr_kh[k] != h) continue;
-            u32 ko = tr_koff[k];
-            if (ko + top_a0.len >= r.n || gr.at(ko + top_a0.len) != '"') continue;
-            if (!ck_spans_equal(gr, ko, gq, top_a0.off, top_a0.len)) continue;
-            if (k == 0) { res0 = first_tr0; res1 = first_tr1; break; }
+        k = trk.find(r, h, top_a0.off, top_a0.len, ko);
+        if (k == 0) { res0 = first_tr0; res1 = first_tr1; }
+        else if (k != ~0u) {
             u32 p2 = ko + top_a0.len + 2;
             res0 = p2;
             ck_tool_result_value(r, p2, 5, cx);
             res1 = p2;
-            break;
         }
     }
     SETSPAN(CK_COL_CALL_VAL_OFF, call0, call1);
