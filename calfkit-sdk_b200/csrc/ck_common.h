@@ -78,7 +78,9 @@ enum {
 #define CK_NARGS_NULL 0xffffffffu
 
 // Output-record descriptor written by the plan kernels and consumed by emit/route.
-// An output payload is the concatenation of up to CK_MAX_SEGS segments.
+// An output payload is the concatenation of up to CK_MAX_SEGS segments.  A segment may start and end at
+// any byte of the payload, and may be empty; the payload itself starts 16-byte aligned in the output buffer.
+// Every source is readable up to 19 bytes past a segment's end (the emitter reads aligned words).
 #define CK_MAX_SEGS 16
 enum { CK_SRC_INPUT = 0, CK_SRC_LIT = 1, CK_SRC_AUX = 2, CK_SRC_GLUE = 3 };   // input record / literal pool / per-batch aux blob / per-payload glue slot
 #define CK_GLUE_STRIDE 512    // bytes of scratch per payload in which a plan thread assembles the new text of a splice

@@ -230,10 +230,11 @@ __device__ __forceinline__ Span ck_dict_find(Rd& r, u32 obj, u32 key_off, u32 ke
 }
 
 // ------------------------------------------------------------------------------------------------
-// Output layout planner.  A payload is described as <= CK_MAX_SEGS segments such that EVERY segment
-// starts at a 16-byte aligned offset of the output payload and every segment but the last is a
-// multiple of 16 bytes long — so each 16-byte output vector the emit kernel writes comes from exactly
-// one segment (no straddling, no per-segment head/tail handling; the kernel is instruction bound).
+// Output layout planner for the producers that generate text (uuid7 frame ids, merged values) and for the
+// global-memory tool plan.  The emit kernel accepts segments at any byte boundary (ck_out_desc); this writer
+// keeps the stricter aligned layout — every segment starts at a 16-byte aligned offset of the output payload
+// and every segment but the last is a multiple of 16 bytes long — so each output vector it describes comes
+// from exactly one segment and takes the emitter's single-gather path.
 // Pieces arrive in output order.  Long input / aux pieces become DIRECT segments (copied from where
 // they lie); everything short — the literals and ids of the inserted entry, and the <= 15 bytes on
 // either side of a splice point that do not fill a vector — is packed by this thread, 8 aligned bytes
@@ -830,16 +831,58 @@ ck_gather_spans_kernel(const u8* __restrict__ src, const long long* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
-// encode: one warp per payload.  Thanks to the aligned layout (SegWriter) the payload is a sequence of
-// 16-byte vectors each of which lies inside one segment: lane l of iteration k produces vector
-// 32k + l = unaligned 16-byte gather from its segment's source + one aligned 16-byte store.  Which
-// segment a vector belongs to is found without a search: the lanes holding the segment table mark the
-// vectors where a segment starts, one warp-wide OR gives the mask and a popcount gives the index.
+// encode: one warp per payload.  The payload is a sequence of aligned 16-byte output vectors; lane l of
+// iteration k produces vector 32k + l with one aligned 16-byte store.  Segments may start and end at any
+// byte (ck_out_desc), so a vector either lies inside one segment — one unaligned 16-byte gather from that
+// segment's source, the common case — or crosses segment boundaries and is assembled from the masked,
+// shifted bytes of every segment it overlaps.  The segment holding a vector's first byte is found by a
+// 4-step binary search over the prefix-summed segment starts (lanes 0..15 hold the table); the boundary
+// lanes, which diverge, read the table from shared memory instead.  Descriptors in the aligned layout
+// (SegWriter) take the single-gather path throughout (a warp-uniform choice per payload, below).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
+#define CK_EMIT_THREADS 256
+#define CK_EMIT_MINB 8         // 64 warps per SM: <= 32 registers, as the single-gather emitter used (no spills)
+// 16 bytes from an arbitrary address: 5 aligned words (may touch <= 19 bytes past the 16: all sources are padded)
+__device__ __forceinline__ uint4 ck_gather16(const u8* src) {
+    u32 sh = (u32)((uintptr_t)src & 3u) * 8u;
+    const u32* a = (const u32*)((uintptr_t)src & ~(uintptr_t)3);
+    u32 w0 = __ldg(a), w1 = __ldg(a + 1), w2 = __ldg(a + 2), w3 = __ldg(a + 3), w4 = __ldg(a + 4);
+    uint4 o;
+    o.x = __funnelshift_r(w0, w1, sh); o.y = __funnelshift_r(w1, w2, sh);
+    o.z = __funnelshift_r(w2, w3, sh); o.w = __funnelshift_r(w3, w4, sh);
+    return o;
+}
+struct ck_emit_segs { const u8* ptr[CK_MAX_SEGS]; u32 start[CK_MAX_SEGS]; u32 end[CK_MAX_SEGS]; };   // one per warp
+// ORs the bytes of x that land in output bytes [b0, b1) of the vector at pos into (lo, hi); x holds output bytes b0..b0+15
+__device__ __forceinline__ void ck_emit_part(uint4 x, u32 b0, u32 b1, u32 pos, unsigned long long& lo, unsigned long long& hi) {
+    unsigned long long xl = ((unsigned long long)x.y << 32) | x.x, xh = ((unsigned long long)x.w << 32) | x.z;
+    u32 nb = b1 - b0, sh = b0 - pos;                               // nb + sh <= 16
+    if (nb < 8) { xl &= (1ull << (8 * nb)) - 1ull; xh = 0; }
+    else if (nb < 16) xh &= (1ull << (8 * (nb - 8))) - 1ull;
+    if (sh >= 8) { xh = xl << (8 * (sh - 8)); xl = 0; }
+    else if (sh) { xh = (xh << (8 * sh)) | (xl >> (64 - 8 * sh)); xl <<= 8 * sh; }
+    lo |= xl; hi |= xh;
+}
+// output bytes [pos, lim) (lim - pos <= 16) of a vector that crosses segment boundaries: segment s holds bytes
+// [pos, s_end), already gathered in x0 (the same gather as the single-segment path); the later segments start inside the
+// vector and are gathered one after the other.  (Issuing two of them at a time needs 38 registers, i.e. 6 blocks per SM:
+// config-2 emit 1.22 ms against 1.05 ms for this loop at 8 blocks, H100 at 400 W.)
+__device__ __forceinline__ uint4 ck_emit_boundary(const ck_emit_segs* t, u32 s, u32 pos, u32 lim, uint4 x0, u32 s_end) {
+    unsigned long long lo = 0, hi = 0;
+    ck_emit_part(x0, pos, s_end, pos, lo, hi);
+    for (u32 k = s + 1; k < CK_MAX_SEGS; k++) {
+        u32 a1 = t->start[k];
+        if (a1 >= lim) break;
+        u32 e1 = t->end[k]; e1 = e1 < lim ? e1 : lim;
+        if (e1 > a1) ck_emit_part(ck_gather16(t->ptr[k]), a1, e1, pos, lo, hi);
+    }
+    return make_uint4((u32)lo, (u32)(lo >> 32), (u32)hi, (u32)(hi >> 32));
+}
+__global__ void __launch_bounds__(CK_EMIT_THREADS, CK_EMIT_MINB)
 ck_emit_kernel(ck_view vw, const u8* __restrict__ lit,
                const u8* __restrict__ aux, const u8* __restrict__ glue, const ck_out_desc* __restrict__ descs,
                const long long* __restrict__ out_off, u32 n, u8* __restrict__ out, long long out_cap) {
+    __shared__ ck_emit_segs s_tab[CK_EMIT_THREADS / 32];
     u32 warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= n) return;
     long long o0 = out_off[warp], o1 = out_off[warp + 1];
@@ -849,7 +892,8 @@ ck_emit_kernel(ck_view vw, const u8* __restrict__ lit,
     if (nseg == 0 || nseg > CK_MAX_SEGS) return;
     u32 total = d->total_len;
     u32 rec_len; const u8* rec = ck_rec(vw, d->record, rec_len);
-    // segment table: lane s holds segment s (source address, start vector, length)
+    // segment table: lane s holds segment s (source address, output start, length); lanes past nseg hold empty
+    // segments starting at the payload's end, so the search below never picks them
     u32 my_len = 0;
     const u8* my_ptr = rec;
     if (lane < nseg) {
@@ -859,33 +903,47 @@ ck_emit_kernel(ck_view vw, const u8* __restrict__ lit,
         my_ptr = (src == CK_SRC_INPUT) ? rec + so : (src == CK_SRC_LIT ? lit + so : (src == CK_SRC_AUX ? aux + so
                  : glue + (size_t)warp * CK_GLUE_STRIDE + so));
     }
-    u32 start = my_len;                      // exclusive prefix sum of the segment lengths = output offset
+    u32 start = my_len;                      // exclusive prefix sum of the segment lengths = output offset (lanes 0..15)
 #pragma unroll
     for (int k = 1; k < CK_MAX_SEGS; k <<= 1) { u32 y = __shfl_up_sync(0xffffffffu, start, k); if (lane >= k) start += y; }
     start -= my_len;
-    u32 start_vec = start >> 4;
+    u32 end = start + my_len;
     unsigned long long pbits = (unsigned long long)(uintptr_t)my_ptr;
     u32 plo = (u32)pbits, phi = (u32)(pbits >> 32);
     uint4* dst = (uint4*)(out + o0);
     u32 nvec = (total + 15u) >> 4;
-    u32 segs_before = 0;
+    // warp-uniform choice per payload: in the aligned layout (SegWriter: every segment starts on a vector, all but the
+    // last are whole vectors) no vector crosses a segment, and the segment of a vector is found without a search — the
+    // lanes holding the table mark the vectors where a segment starts, one warp-wide OR gives the mask, a popcount the index
+    bool aligned = __all_sync(0xffffffffu, lane >= nseg || ((start & 15u) == 0 && (lane + 1 == nseg || (my_len & 15u) == 0)));
+    ck_emit_segs* tab = &s_tab[threadIdx.x >> 5];
+    if (!aligned) {                          // the table for the boundary lanes
+        if (lane < CK_MAX_SEGS) { tab->ptr[lane] = my_ptr; tab->start[lane] = start; tab->end[lane] = end; }
+        __syncwarp();
+    }
+    u32 start_vec = start >> 4, segs_before = 0;
     for (u32 v0 = 0; v0 < nvec; v0 += 32) {
-        u32 bit = (lane < nseg && my_len && start_vec >= v0 && start_vec < v0 + 32) ? (1u << (start_vec - v0)) : 0u;
-        u32 mask = __reduce_or_sync(0xffffffffu, bit);
-        u32 seg = segs_before + __popc(mask & (0xffffffffu >> (31 - lane))) - 1;
-        segs_before += __popc(mask);
-        u32 s_start = __shfl_sync(0xffffffffu, start, seg & 31);
-        u32 s_lo = __shfl_sync(0xffffffffu, plo, seg & 31), s_hi = __shfl_sync(0xffffffffu, phi, seg & 31);
-        u32 v = v0 + lane;
+        u32 v = v0 + lane, pos = v << 4;
+        u32 seg = 0;                         // last segment starting at or before pos
+        if (aligned) {
+            u32 bit = (lane < nseg && my_len && start_vec >= v0 && start_vec < v0 + 32) ? (1u << (start_vec - v0)) : 0u;
+            u32 mask = __reduce_or_sync(0xffffffffu, bit);
+            seg = (segs_before + __popc(mask & (0xffffffffu >> (31 - lane))) - 1) & 31;
+            segs_before += __popc(mask);
+        } else {
+#pragma unroll
+            for (u32 step = CK_MAX_SEGS / 2; step; step >>= 1)
+                if (__shfl_sync(0xffffffffu, start, seg + step) <= pos) seg += step;
+        }
+        u32 s_start = __shfl_sync(0xffffffffu, start, seg);
+        u32 s_lo = __shfl_sync(0xffffffffu, plo, seg), s_hi = __shfl_sync(0xffffffffu, phi, seg);
+        u32 s_end = aligned ? 0u : __shfl_sync(0xffffffffu, end, seg);
         if (v < nvec) {
-            const u8* src = (const u8*)(uintptr_t)(((unsigned long long)s_hi << 32) | s_lo) + ((v << 4) - s_start);
-            u32 sh = (u32)((uintptr_t)src & 3u) * 8u;
-            const u32* a = (const u32*)((uintptr_t)src & ~(uintptr_t)3);
-            // 5 aligned words cover the 16 unaligned bytes (may touch <= 19 bytes past the span: all sources are padded)
-            u32 w0 = __ldg(a), w1 = __ldg(a + 1), w2 = __ldg(a + 2), w3 = __ldg(a + 3), w4 = __ldg(a + 4);
-            uint4 o;
-            o.x = __funnelshift_r(w0, w1, sh); o.y = __funnelshift_r(w1, w2, sh);
-            o.z = __funnelshift_r(w2, w3, sh); o.w = __funnelshift_r(w3, w4, sh);
+            uint4 o = ck_gather16((const u8*)(uintptr_t)(((unsigned long long)s_hi << 32) | s_lo) + (pos - s_start));
+            if (!aligned) {
+                u32 lim = total - pos < 16u ? total : pos + 16u;
+                if (s_end < lim) o = ck_emit_boundary(tab, seg, pos, lim, o, s_end);
+            }
             dst[v] = o;
         }
     }

@@ -5,23 +5,28 @@
 // far-apart spots of each record) and 80 lane-divergent store instructions (the 144 B descriptor, the 512 B-stride
 // glue slot and the two 32 B publishes written array-of-structs by one thread each, so most sectors of every store
 // request were partial) — latency bound, moving several times the algorithmic DRAM traffic.  Here
-//   * every record read goes through a 64-byte per-thread window in shared memory filled by 16-byte cp.async copies
-//     (no data registers; one memory round trip per 48 fresh bytes instead of one per 8),
-//   * glue text, descriptor and the two publishes are assembled in shared memory and written to HBM by the whole
-//     warp, 16 bytes per lane, two records per store instruction (full sectors),
-//   * the route step (topic table probe, murmur2 partition of the key, per-topic histogram) runs in the same thread,
-//     which already has the callback topic and — one window away — the correlation id.
-// Records whose splice needs more glue than the shared-memory slot holds fall back, record by record, to the
-// global-memory planner (ck_plan_tool_one) inside the same kernel: same bytes, no second launch.
+//   * the splice is written as it is: one segment per piece (input spans from the walker's columns, literals from the
+//     pool, a host result from the aux blob) at whatever byte it falls on — the emitter assembles the vectors that
+//     cross a piece boundary (ck_emit_kernel) — so no glue text is built and no record byte is read for the splice,
+//   * the record is read only where a decision needs it (the args object for the template, a non-string
+//     input_args[0], the callback topic, the correlation id), through a 64-byte per-thread window in shared memory
+//     filled by 16-byte cp.async copies (no data registers; one memory round trip per 48 fresh bytes),
+//   * the descriptor and the two publishes are assembled in shared memory and written to HBM by the whole warp,
+//     16 bytes per lane, two records per store instruction (full sectors),
+//   * the route step (topic table probe, murmur2 partition of the key, per-topic histogram) runs in the same thread.
+// Records whose splice needs more than CK_MAX_SEGS segments (a template of many parts plus frame overrides) fall back,
+// record by record, to the global-memory planner (ck_plan_tool_one, aligned glue) inside the same kernel: same bytes,
+// no second launch.
 #ifndef CK_PLAN2_CUH
 #define CK_PLAN2_CUH
 
 #define CK_P2_THREADS 128
 #define CK_P2_WIN 64u                 // window bytes per thread
 #define CK_P2_WSTRIDE 80u             // slot stride (the pad spreads the slots over the banks)
-#define CK_P2_GLUE 256u               // glue bytes per record assembled in shared memory (more: global-memory planner)
-#define CK_P2_GSTRIDE 272u
-#define CK_P2_SEGS 8u                 // segments per record staged in shared memory (more: global-memory planner)
+// 7 blocks per SM: 28,672 B of shared memory per block (windows + descriptors) and <= 72 registers both allow 7
+#ifndef CK_P2_MINB
+#define CK_P2_MINB 7
+#endif
 
 // out of line and by value: a member function taking `this` would pin the reader (and everything that points to it) in
 // local memory — the first version of this kernel made 307 local-memory loads per warp that way
@@ -64,68 +69,19 @@ struct PRd {
     __device__ __forceinline__ void load16(u32 pos, u64& x0, u64& x1) { x0 = load8(pos); x1 = load8(pos + 8); }
 };
 
-struct ck_p2_desc { u32 nseg, record, total_len, pad; u32 seg[CK_P2_SEGS][2]; };     // leading part of ck_out_desc
-struct ck_p2_stage {                   // one per warp
-    u8 glue[32][CK_P2_GSTRIDE];
-    ck_p2_desc desc[32];
-};
+struct ck_p2_stage { ck_out_desc desc[32]; };   // one per warp
 #define CK_P2_SMEM (CK_P2_THREADS * CK_P2_WSTRIDE + (CK_P2_THREADS / 32) * sizeof(ck_p2_stage))
 
-// SegWriter over shared-memory staging (same layout rules as SegWriter: every segment starts at a 16-byte aligned
-// output offset, all but the last are multiples of 16 bytes long)
+// the splice as a list of pieces, one segment each, at any byte boundary of the output (ck_out_desc)
 struct SegWriter2 {
-    ck_p2_desc* d; PRd* r; const u8* lit; const u8* aux; u8* slot;
-    u32 n, total; bool in_glue, overflow; u32 gfill, grun; unsigned long long acc; u32 cnt;
-    __device__ __forceinline__ void init(ck_p2_desc* dd, PRd* rr, const u8* l, const u8* a, u8* s) {
-        d = dd; r = rr; lit = l; aux = a; slot = s; n = 0; total = 0; in_glue = false; overflow = false; gfill = 0; grun = 0; acc = 0; cnt = 0;
-    }
-    __device__ __forceinline__ void seg(u32 src, u32 off, u32 len) {
-        if (n < CK_P2_SEGS) { *(uint2*)d->seg[n] = make_uint2(off, (len << 2) | src); n++; } else overflow = true;
-    }
-    __device__ __forceinline__ void put8(unsigned long long chunk, u32 nb) {
-        if (gfill + nb > CK_P2_GLUE) { overflow = true; return; }
-        if (nb < 8) chunk &= (~0ull >> (8 * (8 - nb)));
-        acc |= chunk << (8 * cnt);
-        u32 c2 = cnt + nb;
-        gfill += nb;
-        if (c2 >= 8) {
-            *(unsigned long long*)(slot + ((gfill - (c2 - 8)) - 8)) = acc;
-            acc = cnt ? (chunk >> (8 * (8 - cnt))) : 0ull;
-            c2 -= 8;
-        }
-        cnt = c2;
-    }
-    __device__ __forceinline__ unsigned long long fetch8(u32 src, u32 off) {
-        return src == CK_SRC_INPUT ? r->load8(off) : SegWriter::load8_g((src == CK_SRC_LIT ? lit : aux) + off);
-    }
-    __device__ __forceinline__ void close_run() {
-        if (cnt) { *(unsigned long long*)(slot + (gfill & ~7u)) = acc; acc = 0; cnt = 0; }
-        seg(CK_SRC_GLUE, grun, gfill - grun);
-        gfill = (gfill + 15u) & ~15u;
-        in_glue = false;
-    }
-    __device__ __forceinline__ void glue_bytes(u32 src, u32 off, u32 len) {
-        if (!in_glue) { in_glue = true; grun = gfill; }
-        for (u32 k = 0; k < len; k += 8) put8(fetch8(src, off + k), len - k < 8 ? len - k : 8);
-        total += len;
-    }
+    ck_out_desc* d; u32 n, total; bool overflow;
+    __device__ __forceinline__ void init(ck_out_desc* dd) { d = dd; n = 0; total = 0; overflow = false; }
     __device__ __forceinline__ void add(u32 src, u32 off, u32 len) {
         if (len == 0) return;
-        bool direct_ok = (src == CK_SRC_INPUT || src == CK_SRC_AUX) && len >= CK_DIRECT_MIN;
-        if (!direct_ok) { glue_bytes(src, off, len); return; }
-        if (in_glue || (total & 15u)) {
-            u32 need = (16u - (total & 15u)) & 15u;
-            glue_bytes(src, off, need);
-            off += need; len -= need;
-            close_run();
-        }
-        u32 body = len & ~15u;
-        seg(src, off, body);
-        total += body;
-        if (len - body) glue_bytes(src, off + body, len - body);
+        if (n < CK_MAX_SEGS) { *(uint2*)d->seg[n] = make_uint2(off, (len << 2) | src); n++; } else overflow = true;
+        total += len;
     }
     __device__ __forceinline__ bool finish(u32 record) {
-        if (in_glue) close_run();
         d->nseg = n; d->record = record; d->total_len = total; d->pad = 0;
         return !overflow;
     }
@@ -231,20 +187,20 @@ __device__ __forceinline__ void ck_route_one_global(ck_view vw, const u32* __res
     }
 }
 
-struct ck_p2_res { u32 action, nout, status, pay_len, glue_len, desc_len; };
+struct ck_p2_res { u32 action, nout, status, pay_len, desc_len; };
 
 // the plan proper: ToolNodeDef.run + handler dispatch + _publish_action(ReturnCall | Silent) + overrides rule
 // (nodes/tool.py:37-86, nodes/base.py:66-67,105-118,137-145,157-160), as ck_plan_tool_one, into shared memory
 __device__ __forceinline__ bool
 ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, const ck_tool_cfg& cfg, const u8* __restrict__ lit,
-                  const long long* __restrict__ aux_off, const u8* __restrict__ aux, int mode,
-                  ck_p2_desc* d, u8* gslot, ck_pub* pb /* [2] */, const ck_topic_table& tab, u32 num_partitions, ck_p2_res& out) {
+                  const long long* __restrict__ aux_off, int mode,
+                  ck_out_desc* d, ck_pub* pb /* [2] */, const ck_topic_table& tab, u32 num_partitions, ck_p2_res& out) {
 #define COL(k) cols[(size_t)(k) * stride + i]
     ck_pub none; none.payload = 0xffffffffu; none.topic_id = -1; none.topic_off = none.topic_len = 0; none.record = i;
     none.has_key = 0; none.partition = -1; none.pad = 0;
     pb[0] = none; pb[1] = none;
     d->nseg = 0; d->record = i; d->total_len = 0; d->pad = 0;
-    out.action = CK_ACT_NONE; out.nout = 0; out.pay_len = 0; out.glue_len = 0; out.desc_len = 16;
+    out.action = CK_ACT_NONE; out.nout = 0; out.pay_len = 0; out.desc_len = 16;
     u32 status = COL(CK_COL_STATUS);
     out.status = status;
     if (status != CK_OK) return true;
@@ -257,12 +213,10 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
     if (nframes > 0) {
         // the spots this thread will read, far apart in the record: start all of them towards L2 now so that the
         // window refills below find them there instead of queueing one DRAM miss behind the other
-        u32 tro = tr_off + tr_len;
-        ck_prefetch_l2(rec + (tro > 16 ? tro - 16 : 0)); ck_prefetch_l2(rec + id_off); ck_prefetch_l2(rec + COL(CK_COL_ARGS_OFF));
-        ck_prefetch_l2(rec + (top_off > 16 ? top_off - 16 : 0)); ck_prefetch_l2(rec + top_off + top_len); ck_prefetch_l2(rec + corr_off);
+        ck_prefetch_l2(rec + COL(CK_COL_ARGS_OFF)); ck_prefetch_l2(rec + cb_off); ck_prefetch_l2(rec + corr_off);
     }
     PRd r; r.init(rec, rlen);
-    SegWriter2 w; w.init(d, &r, lit, aux, gslot);
+    SegWriter2 w; w.init(d);
     // a canonical OverridesState is an object, never 4 bytes long: "null" <=> length 4 (no read needed)
     bool fov_set = nframes > 0 && fov_len != 4;
     u32 cur = 0;
@@ -278,7 +232,7 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
             // only the handler-return publish: the input envelope, unchanged (nodes/base.py:142, worker.py:52-53)
             w.add(CK_SRC_INPUT, 0, r.n);
             w.finish(i);
-            out.action = action; out.glue_len = w.gfill;
+            out.action = action;
             if (cfg.publish_topic_id >= 0) {
                 out.pay_len = r.n; out.nout = 1;
                 ck_pub p = none; p.payload = i; p.topic_id = cfg.publish_topic_id; pb[1] = p;
@@ -288,34 +242,9 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
         }
         Span args = {COL(CK_COL_ARGS_OFF), COL(CK_COL_ARGS_LEN)};
         Span existing = {COL(CK_COL_RES_OFF), COL(CK_COL_RES_LEN)};
-        u32 rv_src[CK_TPL_MAX_PARTS], rv_off[CK_TPL_MAX_PARTS], rv_len[CK_TPL_MAX_PARTS], rv_n = 0;
-        if (cfg.tpl_nparts == 0 || aux_off != nullptr) {         // host results, when supplied, win over the template
-            if (aux_off == nullptr) { out.action = CK_ACT_HOST_TOOL; return true; }
-            long long r0 = aux_off[i], r1 = aux_off[i + 1];
-            rv_src[0] = CK_SRC_AUX; rv_off[0] = (u32)r0; rv_len[0] = (u32)(r1 - r0); rv_n = 1;
-        } else {
-            bool ok = (r.at(args.off) == '{');
-            for (u32 k = 0; k < cfg.tpl_nparts && ok; k++) {
-                if (cfg.tpl_kind[k] == 0) { rv_src[rv_n] = CK_SRC_LIT; rv_off[rv_n] = cfg.tpl_off[k]; rv_len[rv_n] = cfg.tpl_len[k]; rv_n++; }
-                else {
-                    u32 p = args.off + 1; bool found = false;
-                    while (p < args.off + args.len && r.at(p) != '}') {
-                        Span k2; ck_string(r, p, k2); p++;
-                        u32 vv = p; ck_skip_value(r, p);
-                        bool eq = (k2.len == cfg.tpl_len[k]);
-                        for (u32 b = 0; eq && b < k2.len; b++) eq = (r.at(k2.off + b) == lit[cfg.tpl_off[k] + b]);
-                        if (eq) {
-                            if (r.at(vv) != '"') { ok = false; break; }          // non-string argument: host formats it
-                            rv_src[rv_n] = CK_SRC_INPUT; rv_off[rv_n] = vv + 1; rv_len[rv_n] = p - vv - 2; rv_n++;
-                            found = true; break;
-                        }
-                        if (p < r.n && r.at(p) == ',') p++;
-                    }
-                    if (!found) ok = false;
-                }
-            }
-            if (!ok) { out.action = CK_ACT_RAISES; out.status = CK_UNSUPPORTED; return true; }
-        }
+        bool host = cfg.tpl_nparts == 0 || aux_off != nullptr;   // host results, when supplied, win over the template
+        if (host && aux_off == nullptr) { out.action = CK_ACT_HOST_TOOL; return true; }
+        if (!host && r.at(args.off) != '{') { out.action = CK_ACT_RAISES; out.status = CK_UNSUPPORTED; return true; }
         if (existing.len == 0) {
             w.add(CK_SRC_INPUT, 0, tr_off + tr_len - 1);
             if (tr_len > 2) w.add(CK_SRC_LIT, cfg.lit_comma_q[0], cfg.lit_comma_q[1]); else w.add(CK_SRC_LIT, cfg.lit_q[0], cfg.lit_q[1]);
@@ -327,7 +256,30 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
             w.add(CK_SRC_LIT, cfg.lit_value_open[0], cfg.lit_value_open[1]);
             cur = existing.off + existing.len;
         }
-        for (u32 k = 0; k < rv_n; k++) w.add(rv_src[k], rv_off[k], rv_len[k]);
+        // the tool's return value as JSON: the host's result, or the template's literals and raw string arguments
+        if (host) {
+            long long r0 = aux_off[i], r1 = aux_off[i + 1];
+            w.add(CK_SRC_AUX, (u32)r0, (u32)(r1 - r0));
+        } else {
+            for (u32 k = 0; k < cfg.tpl_nparts; k++) {
+                if (cfg.tpl_kind[k] == 0) { w.add(CK_SRC_LIT, cfg.tpl_off[k], cfg.tpl_len[k]); continue; }
+                u32 p = args.off + 1; bool found = false;
+                while (p < args.off + args.len && r.at(p) != '}') {
+                    Span k2; ck_string(r, p, k2); p++;
+                    u32 vv = p; ck_skip_value(r, p);
+                    bool eq = (k2.len == cfg.tpl_len[k]);
+                    for (u32 b = 0; eq && b < k2.len; b++) eq = (r.at(k2.off + b) == lit[cfg.tpl_off[k] + b]);
+                    if (eq) {
+                        if (r.at(vv) != '"') break;                      // non-string argument: host formats it
+                        w.add(CK_SRC_INPUT, vv + 1, p - vv - 2);
+                        found = true; break;
+                    }
+                    if (p < r.n && r.at(p) == ',') p++;
+                }
+                // the segments written so far are not published: nseg stays 0 and only the header is written out
+                if (!found) { out.action = CK_ACT_RAISES; out.status = CK_UNSUPPORTED; return true; }
+            }
+        }
         w.add(CK_SRC_LIT, cfg.lit_mid[0], cfg.lit_mid[1]);
         w.add(CK_SRC_INPUT, id_off, id_len);
         w.add(CK_SRC_LIT, cfg.lit_close[0], cfg.lit_close[1]);
@@ -336,8 +288,8 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
     u32 cut0 = nframes > 1 ? top_off - 1 : top_off;
     w.add(CK_SRC_INPUT, cur, cut0 - cur);
     w.add(CK_SRC_INPUT, top_off + top_len, r.n - (top_off + top_len));
-    if (!w.finish(i)) return false;                     // needs more glue / segments than the staging slot holds
-    out.pay_len = w.total; out.glue_len = w.gfill; out.desc_len = 16 + 8 * w.n;
+    if (!w.finish(i)) return false;                     // more pieces than a descriptor holds
+    out.pay_len = w.total; out.desc_len = 16 + 8 * w.n;
     out.action = CK_ACT_RETURN;
     // publishes: callback (keyed by correlation id), then the handler return value to publish_topic; routed here
     ck_pub p = none; p.payload = i; p.topic_off = cb_off; p.topic_len = cb_len; p.has_key = 1;
@@ -350,7 +302,19 @@ ck_plan_tool2_one(ck_view v, u32 i, const u32* __restrict__ cols, u32 stride, co
 #undef COL
 }
 
-__global__ void __launch_bounds__(CK_P2_THREADS)
+// rare: more pieces than a descriptor holds -> the global-memory planner (aligned glue), then route its publishes.
+// Out of line, so that its registers do not count against the staged path's.
+__device__ __noinline__ void
+ck_plan_tool2_fallback(ck_view v, u32 i, u32* __restrict__ cols, u32 stride, const ck_tool_cfg* __restrict__ cfgp,
+                       const u8* __restrict__ lit, const long long* __restrict__ aux_off, const u8* __restrict__ aux,
+                       u8* __restrict__ glue, int mode, ck_out_desc* __restrict__ descs, u32* __restrict__ pay_len,
+                       ck_pub* __restrict__ pubs, const ck_topic_table& tab, u32 num_partitions) {
+    ck_plan_tool_one(v, i, cols, stride, cfgp, lit, aux_off, aux, glue, mode, descs, pay_len, pubs);
+    ck_route_one_global(v, cols, stride, pubs + 2 * i, tab, num_partitions);
+    ck_route_one_global(v, cols, stride, pubs + 2 * i + 1, tab, num_partitions);
+}
+
+__global__ void __launch_bounds__(CK_P2_THREADS, CK_P2_MINB)
 ck_plan_tool2_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride,
                      const ck_tool_cfg* __restrict__ cfgp, const u8* __restrict__ lit,
                      const long long* __restrict__ aux_off, const u8* __restrict__ aux, u8* __restrict__ glue,
@@ -360,19 +324,16 @@ ck_plan_tool2_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride,
     ck_p2_stage* st = (ck_p2_stage*)((u8*)ck_win_smem + CK_P2_THREADS * CK_P2_WSTRIDE) + warp;
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     u32 i0 = i - lane;                                   // first record of this warp
-    ck_p2_res res; res.action = CK_ACT_NONE; res.nout = 0; res.status = CK_OK; res.pay_len = 0; res.glue_len = 0; res.desc_len = 0;
+    ck_p2_res res; res.action = CK_ACT_NONE; res.nout = 0; res.status = CK_OK; res.pay_len = 0; res.desc_len = 0;
     bool live = i < n, staged = false;
     ck_pub pb[2];
     pb[0].payload = pb[1].payload = 0xffffffffu; pb[0].topic_id = pb[1].topic_id = -1;
     if (live) {
-        staged = ck_plan_tool2_one(v, i, cols, stride, *cfgp, lit, aux_off, aux, mode, &st->desc[lane], st->glue[lane], pb, tab, num_partitions, res);
+        staged = ck_plan_tool2_one(v, i, cols, stride, *cfgp, lit, aux_off, mode, &st->desc[lane], pb, tab, num_partitions, res);
         if (!staged) {
-            // rare: splice too large for the staging slot -> the global-memory planner, then route its two publishes
-            ck_plan_tool_one(v, i, cols, stride, cfgp, lit, aux_off, aux, glue, mode, descs, pay_len, pubs);
-            ck_route_one_global(v, cols, stride, pubs + 2 * i, tab, num_partitions);
-            ck_route_one_global(v, cols, stride, pubs + 2 * i + 1, tab, num_partitions);
+            ck_plan_tool2_fallback(v, i, cols, stride, cfgp, lit, aux_off, aux, glue, mode, descs, pay_len, pubs, tab, num_partitions);
             pb[0] = pubs[2 * i]; pb[1] = pubs[2 * i + 1];                                   // for the histogram below
-            res.glue_len = 0; res.desc_len = 0;
+            res.desc_len = 0;
         } else {
             pay_len[i] = res.pay_len;
             cols[(size_t)CK_COL_ACTION * stride + i] = res.action;
@@ -385,14 +346,13 @@ ck_plan_tool2_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride,
         }
     }
     __syncwarp();
-    // ---- coalesced write-out of descriptors and glue: two records per store instruction, 16 bytes per lane
+    // ---- coalesced write-out of the descriptors: two records per store instruction, 16 bytes per lane
     u32 half = lane >> 4, hl = lane & 15;
 #pragma unroll 1
     for (u32 it = 0; it < 16; it++) {
         u32 rr = 2 * it + half;
-        u32 dl = __shfl_sync(0xffffffffu, res.desc_len, rr), gl = __shfl_sync(0xffffffffu, res.glue_len, rr);
+        u32 dl = __shfl_sync(0xffffffffu, res.desc_len, rr);
         if (hl * 16 < dl) *(uint4*)((u8*)(descs + i0 + rr) + hl * 16) = *(const uint4*)((const u8*)&st->desc[rr] + hl * 16);
-        for (u32 k = hl * 16; k < gl; k += 256) *(uint4*)(glue + (size_t)(i0 + rr) * CK_GLUE_STRIDE + k) = *(const uint4*)(&st->glue[rr][k]);
     }
     // ---- per-topic histogram, aggregated inside the warp (one atomic per distinct topic)
 #pragma unroll
