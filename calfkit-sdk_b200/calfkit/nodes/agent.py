@@ -270,6 +270,10 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
             finally:
                 if saved_topics is not None:
                     self._restore_registry(engine, saved_topics)
+            for r in np.flatnonzero(out.cols[COL["STATUS"]] != CK_OK):
+                # e.g. more tool calls than the engine indexes per record (DESIGN.md §8): the conversation stops here
+                logger.error("record %d declined after the agent step: %s; nothing is published for it",
+                             items[r][0], STATUS_NAMES[int(out.cols[COL["STATUS"], r])])
             for p in publishes:
                 src = recs2[p.record]
                 corr = src.correlation_id or (p.key.decode() if p.key else None)

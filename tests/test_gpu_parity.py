@@ -145,9 +145,11 @@ def test_device_walker_equals_host_build_on_fuzz(engine):
     here the nvcc build must agree with it column for column on the same inputs."""
     from hostsim import walk                  # g++ build of the source the GPU kernel compiles (csrc/ck_walk.cuh)
     from calfkit import synth
+    from test_gpu_round_trip import oracle_tool_hop_inputs
     rng = random.Random(1)
+    calls = oracle_tool_hop_inputs()          # multi-call Call envelopes: the looked-up call at index 0, 1, 2, middle, last
     seeds = [as_bytes(c["input"]) for c in golden("codec.json")] + synth.tool_events(50, seed=2) + \
-        synth.mixed_events(40, seed=3, hi=20000)
+        synth.mixed_events(40, seed=3, hi=20000) + calls
     recs = list(seeds)
     for _ in range(6000):
         s = bytearray(rng.choice(seeds))
@@ -185,6 +187,19 @@ def test_device_walker_equals_host_build_on_fuzz(engine):
             assert ok
         assert cols[0, i] == 0, (i, r[:200])
         assert (cols[2:ncmp, i] == hc[2:ncmp]).all(), i   # columns 0/1 (status/action) are owned by the kernels
+    # the warp walker (records of 16 KB and more, GPU only) resolves the looked-up call from its shared-memory key tables:
+    # its spans must be those of the host thread walker on the same bytes
+    from calfkit.engine._lib import COL
+    n_long = 0
+    for i in range(len(seeds) - len(calls), len(seeds)):
+        if len(recs[i]) < 16384:
+            continue
+        ok, hc = walk(recs[i])
+        assert ok and hc[COL["CALL_VAL_LEN"]] > 0
+        for name in ("CALL_VAL", "TNAME", "ARGS", "RES"):
+            assert cols[COL[name + "_OFF"], i] == hc[COL[name + "_OFF"]] and cols[COL[name + "_LEN"], i] == hc[COL[name + "_LEN"]], (i, name)
+        n_long += 1
+    assert n_long >= 40
 
 def test_fanout_matches_oracle(engine):
     """Agent fan-out (config 3): every pending tool call -> one Call envelope, frame ids injected into
