@@ -4,9 +4,9 @@ Two kinds of tool are distinguished at decoration time:
   * device tools  — `@agent_tool(device_template="It's sunny in {location}")`: the return value is a
     pure string template of string arguments; ToolNodeDef.run happens entirely in
     ck_plan_tool_kernel, no host round trip.
-  * host tools    — any Python callable: the engine gathers each record's `args` JSON on the device,
-    the callable runs on the host (the one thing a GPU cannot do: user Python), and its JSON result is
-    spliced in on the device.  Argument decoding / result encoding of the *user's values* happens here
+  * host tools    — any Python callable: the engine gathers each record's `args` JSON on the device
+    (the same kernel, mode 0), the callable runs on the host (the one thing a GPU cannot do: user
+    Python), and its JSON result is spliced in on the device.  Argument decoding / result encoding of the *user's values* happens here
     with pydantic_core, exactly as reference nodes/tool.py:64 + messages.py:1229-1240 do.
 """
 from __future__ import annotations

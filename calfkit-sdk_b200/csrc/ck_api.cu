@@ -412,38 +412,33 @@ static int scan_emit(ck_handle* h, u32 npay, const u8* aux) {
     return 0;
 }
 
-extern "C" int ck_tool_args(ck_handle* h) {
-    cudaSetDevice(h->device);
-    if (!h->tool_set) return fail(h, "ck_tool_args: call ck_set_tool_node first");
-    {
-        KTimer t(h, CK_K_PLAN);
-        if (h->n) CKL(h) ck_plan_tool_kernel<<<(h->n + 127) / 128, 128, 0, h->stream>>>(view_of(h), h->n, h->d_cols, h->n,
-            h->d_tool_cfg, h->d_lit, nullptr, nullptr, h->d_glue, 0, h->d_descs, h->d_pay_len, h->d_pubs);
-        CUDA_TRY(h, cudaGetLastError());
-    }
-    h->n_pubs = 0;
-    return scan_emit(h, h->n, nullptr);
-}
-
-// plan (modes 1 / 2) staged through shared memory, publishes routed in the same kernel (ck_plan2.cuh)
-static int launch_plan2(ck_handle* h, const u8* aux, const long long* aux_off, int mode) {
+// tool plan (modes 0 / 1 / 2) staged through shared memory, publishes routed in the same kernel (ck_plan.cuh)
+static int launch_plan(ck_handle* h, const long long* aux_off, int mode) {
     static bool attr_set = false;
     if (!attr_set) {
-        CUDA_TRY(h, cudaFuncSetAttribute(ck_plan_tool2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CK_P2_SMEM));
+        CUDA_TRY(h, cudaFuncSetAttribute(ck_plan_tool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CK_P2_SMEM));
         attr_set = true;
     }
     KTimer t(h, CK_K_PLAN);
-    if (h->n) CKL(h) ck_plan_tool2_kernel<<<(h->n + CK_P2_THREADS - 1) / CK_P2_THREADS, CK_P2_THREADS, CK_P2_SMEM, h->stream>>>(
-        view_of(h), h->n, h->d_cols, h->n, h->d_tool_cfg, h->d_lit, aux_off, aux, h->d_glue, mode, h->d_descs, h->d_pay_len, h->d_pubs,
+    if (h->n) CKL(h) ck_plan_tool_kernel<<<(h->n + CK_P2_THREADS - 1) / CK_P2_THREADS, CK_P2_THREADS, CK_P2_SMEM, h->stream>>>(
+        view_of(h), h->n, h->d_cols, h->n, h->d_tool_cfg, h->d_lit, aux_off, mode, h->d_descs, h->d_pay_len, h->d_pubs,
         h->tab, h->num_partitions, h->d_topic_hist, h->hist_cap);
     CUDA_TRY(h, cudaGetLastError());
     return 0;
 }
 
+extern "C" int ck_tool_args(ck_handle* h) {
+    cudaSetDevice(h->device);
+    if (!h->tool_set) return fail(h, "ck_tool_args: call ck_set_tool_node first");
+    if (launch_plan(h, nullptr, 0)) return 1;
+    h->n_pubs = 0;
+    return scan_emit(h, h->n, nullptr);
+}
+
 static int tool_plan_common(ck_handle* h, const u8* aux, const long long* aux_off) {
     if (!h->tool_set) return fail(h, "ck_tool_plan: call ck_set_tool_node first");
     if (h->h_tool_cfg.tpl_nparts == 0 && aux_off == nullptr) return fail(h, "ck_tool_plan: node has no device template, host results required");
-    if (launch_plan2(h, aux, aux_off, 1)) return 1;
+    if (launch_plan(h, aux_off, 1)) return 1;
     // NOTE: payload sizes are bounded by in + per-record constant; the caller sizes max_out accordingly
     if (scan_emit(h, h->n, aux)) return 1;
     h->n_pubs = 2 * h->n;
@@ -467,7 +462,7 @@ extern "C" int ck_tool_plan(ck_handle* h, const uint8_t* host_aux, const int64_t
 extern "C" int ck_return_plan(ck_handle* h) {
     cudaSetDevice(h->device);
     if (!h->tool_set) return fail(h, "ck_return_plan: call ck_set_tool_node (publish topic) first");
-    if (launch_plan2(h, nullptr, nullptr, 2)) return 1;
+    if (launch_plan(h, nullptr, 2)) return 1;
     if (scan_emit(h, h->n, nullptr)) return 1;
     h->n_pubs = 2 * h->n;
     return 0;

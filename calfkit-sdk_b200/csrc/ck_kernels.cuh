@@ -2,8 +2,9 @@
 // contraction; everything here is HBM-bound byte/integer work (DESIGN.md §kernels).
 //
 //   ck_walk_kernel        decode: prove each record is a canonical Envelope + extract spans   (a2,a3,a4)
-//   ck_plan_tool_kernel   ToolNodeDef.run + _publish_action(ReturnCall|Silent) as a splice plan  (a5,a6)
-//   ck_plan_fanout_kernel Agent fan-out: one Call envelope per pending tool call               (a9,a6)
+//   ck_plan_tool_kernel   ToolNodeDef.run + _publish_action(ReturnCall|Silent) as a splice plan, routed  (a5,a6,a8)
+//                         (ck_plan.cuh)
+//   ck_fanout2_*_kernel   Agent fan-out: one Call envelope per pending tool call (ck_fanout2.cuh)   (a9,a6)
 //   ck_scan_*             exclusive prefix sum of payload lengths -> output offsets
 //   ck_emit_kernel        encode: gather segments into contiguous output payloads               (a7)
 //   ck_route_kernel       topic string -> registered topic id, Kafka partition of the key        (a8)
@@ -55,7 +56,12 @@ __device__ __forceinline__ const u8* ck_rec(const ck_view& v, u32 i, u32& len) {
 // ------------------------------------------------------------------------------------------------
 // node configuration living in device memory
 // ------------------------------------------------------------------------------------------------
-#define CK_TPL_MAX_PARTS 6
+// Pieces of a tool splice besides the template's, in the worst case (no existing result, frame overrides): 4 before
+// the return value (prefix, `,"` or `"`, id, `":{"return_value":`), 3 after it (lit_mid, id, lit_close), 2 for the
+// overrides rule and 2 for the unwind.  With the template's parts on top they must fit one descriptor.
+#define CK_TOOL_FIXED_PIECES 11
+#define CK_TPL_MAX_PARTS 5
+static_assert(CK_TOOL_FIXED_PIECES + CK_TPL_MAX_PARTS <= CK_MAX_SEGS, "a tool splice must fit one descriptor");
 struct ck_tool_cfg {
     int32_t  publish_topic_id;          // registered id of node.publish_topic, -1 = none
     uint32_t tpl_nparts;                // 0 = results come from the host (aux blob)
@@ -89,12 +95,6 @@ struct ck_topic_table {                  // open addressing, power-of-two capaci
     const uint32_t* name_len;
     const uint8_t*  names;
 };
-
-__device__ __forceinline__ u32 ck_fnv1a(const u8* p, u32 n) {
-    u32 h = 2166136261u;
-    for (u32 i = 0; i < n; i++) h = (h ^ p[i]) * 16777619u;
-    return h ? h : 1u;
-}
 
 // ------------------------------------------------------------------------------------------------
 // decode
@@ -230,29 +230,16 @@ __device__ __forceinline__ Span ck_dict_find(Rd& r, u32 obj, u32 key_off, u32 ke
 }
 
 // ------------------------------------------------------------------------------------------------
-// Output layout planner for the producers that generate text (uuid7 frame ids, merged values) and for the
-// global-memory tool plan.  The emit kernel accepts segments at any byte boundary (ck_out_desc); this writer
-// keeps the stricter aligned layout — every segment starts at a 16-byte aligned offset of the output payload
-// and every segment but the last is a multiple of 16 bytes long — so each output vector it describes comes
-// from exactly one segment and takes the emitter's single-gather path.
+// Output layout planner for the producers that generate text (uuid7 frame ids, merged values): the fan-out,
+// tail-call, reply and gate plans.  The emit kernel accepts segments at any byte boundary (ck_out_desc); this
+// writer keeps the stricter aligned layout — every segment starts at a 16-byte aligned offset of the output
+// payload and every segment but the last is a multiple of 16 bytes long — so each output vector it describes
+// comes from exactly one segment and takes the emitter's single-gather path.
 // Pieces arrive in output order.  Long input / aux pieces become DIRECT segments (copied from where
-// they lie); everything short — the literals and ids of the inserted entry, and the <= 15 bytes on
-// either side of a splice point that do not fill a vector — is packed by this thread, 8 aligned bytes
-// per store, into the payload's glue slot and becomes a GLUE segment.
+// they lie); everything short — literals, generated ids, and the <= 15 bytes on either side of a splice
+// point that do not fill a vector — is packed by this thread, 8 aligned bytes per store, into the
+// payload's glue slot and becomes a GLUE segment.
 // ------------------------------------------------------------------------------------------------
-#ifndef CK_PLAN_PF
-#define CK_PLAN_PF 1
-#endif
-#ifndef CK_PLAN_MINB
-#define CK_PLAN_MINB 1
-#endif
-__device__ __forceinline__ void ck_prefetch_l2(const u8* p) {
-#if CK_PLAN_PF == 2
-    asm volatile("prefetch.global.L1 [%0];" :: "l"(p));
-#else
-    asm volatile("prefetch.global.L2 [%0];" :: "l"(p));
-#endif
-}
 #define CK_DIRECT_MIN 48u
 struct SegWriter {
     ck_out_desc* d;
@@ -327,183 +314,6 @@ struct SegWriter {
         return !overflow;
     }
 };
-
-// ------------------------------------------------------------------------------------------------
-// tool node: ToolNodeDef.run (reference nodes/tool.py:37-86) + handler dispatch rule
-// (nodes/base.py:157-160) + _publish_action(ReturnCall | Silent) (nodes/base.py:105-118,137-145)
-// + prepare_context's overrides rule (nodes/base.py:66-67), expressed as a splice plan.
-//   mode 0: classify + locate the tool call; payload = the args JSON span (1 segment) so a host
-//           tool can be given its arguments (only used when the node has no device template)
-//   mode 1: classify + build the final payload from the device template or the host's results (aux)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void
-ck_plan_tool_one(ck_view v, u32 i, u32* __restrict__ cols, u32 stride,
-                 const ck_tool_cfg* __restrict__ cfgp, const u8* __restrict__ lit,
-                 const long long* __restrict__ aux_off,    // per record [n+1] spans of the host results blob, or NULL
-                 const u8* __restrict__ aux, u8* __restrict__ glue,
-                 int mode, ck_out_desc* __restrict__ descs, u32* __restrict__ pay_len, ck_pub* __restrict__ pubs) {
-#define COL(k) cols[(size_t)(k) * stride + i]
-    const ck_tool_cfg& cfg = *cfgp;
-    ck_pub none; none.payload = 0xffffffffu; none.topic_id = -1; none.topic_off = none.topic_len = 0; none.record = i;
-    none.has_key = 0; none.partition = -1; none.pad = 0;
-    ck_out_desc* d = descs + i;
-    u32 status = COL(CK_COL_STATUS);
-    u32 action = CK_ACT_NONE;
-    u32 rlen; const u8* rec = ck_rec(v, i, rlen);
-    Rd r; r.init(rec, rlen);
-    pubs[2 * i] = none; pubs[2 * i + 1] = none;
-    pay_len[i] = 0; d->nseg = 0; d->total_len = 0; d->record = i;
-    if (status != CK_OK) { COL(CK_COL_ACTION) = CK_ACT_NONE; COL(CK_COL_NOUT) = 0; return; }
-
-    u32 nframes = COL(CK_COL_NFRAMES), nargs = COL(CK_COL_NARGS), kinds = COL(CK_COL_ARGKINDS);
-#if CK_PLAN_PF
-    // the plan reads ~10 short, far-apart pieces of the record, one after the other (each a DRAM miss): start all
-    // those fetches now so that they overlap instead of queueing behind each other
-    if (mode != 0 && nframes > 0) {
-        u32 tro = COL(CK_COL_TR_OFF) + COL(CK_COL_TR_LEN), tpo = COL(CK_COL_TOP_OFF);
-        ck_prefetch_l2(rec + (tro > 16 ? tro - 16 : 0)); ck_prefetch_l2(rec + COL(CK_COL_ARG0_OFF)); ck_prefetch_l2(rec + COL(CK_COL_ARGS_OFF));
-        ck_prefetch_l2(rec + (tpo > 16 ? tpo - 16 : 0)); ck_prefetch_l2(rec + tpo + COL(CK_COL_TOP_LEN)); ck_prefetch_l2(rec + COL(CK_COL_CB_OFF));
-        ck_prefetch_l2(rec + COL(CK_COL_FOV_OFF)); ck_prefetch_l2(rec + COL(CK_COL_SOV_OFF));
-    }
-#endif
-    SegWriter w; w.init(d, &r, lit, aux, glue + (size_t)i * CK_GLUE_STRIDE);
-    Span call = {0, 0};
-    if (mode == 2) {
-        // plain ReturnCall(state) of a node whose run() left the state as it is on the wire
-        // (Agent final output after the host LLM step): overrides rule + unwind + two publishes
-        if (nframes == 0) { COL(CK_COL_ACTION) = CK_ACT_RAISES; COL(CK_COL_NOUT) = 0; return; }
-        u32 cur2 = 0;
-        u32 fo = COL(CK_COL_FOV_OFF), fl = COL(CK_COL_FOV_LEN);
-        if (r.at(fo) != 'n') { u32 so = COL(CK_COL_SOV_OFF), sl = COL(CK_COL_SOV_LEN); w.add(CK_SRC_INPUT, 0, so); w.add(CK_SRC_INPUT, fo, fl); cur2 = so + sl; }
-        u32 to = COL(CK_COL_TOP_OFF), tl = COL(CK_COL_TOP_LEN);
-        u32 c0 = nframes > 1 ? to - 1 : to;
-        w.add(CK_SRC_INPUT, cur2, c0 - cur2);
-        w.add(CK_SRC_INPUT, to + tl, r.n - (to + tl));
-        w.finish(i);
-        pay_len[i] = w.total;
-        ck_pub p = none; p.payload = i; p.topic_off = COL(CK_COL_CB_OFF); p.topic_len = COL(CK_COL_CB_LEN); p.has_key = 1;
-        pubs[2 * i] = p;
-        u32 no = 1;
-        if (cfg.publish_topic_id >= 0) { ck_pub q = none; q.payload = i; q.topic_id = cfg.publish_topic_id; pubs[2 * i + 1] = q; no = 2; }
-        COL(CK_COL_ACTION) = CK_ACT_RETURN; COL(CK_COL_NOUT) = no;
-        return;
-    }
-    if (nframes == 0 || nargs != 2) action = CK_ACT_RAISES;       // peek on empty stack / run() arity TypeError
-    else if (!(kinds & 1u)) {
-        u8 c0 = r.at(COL(CK_COL_ARG0_OFF));
-        action = (c0 == '[' || c0 == '{') ? CK_ACT_RAISES : CK_ACT_SILENT;   // unhashable key raises; other scalars miss
-    } else {
-        call.off = COL(CK_COL_CALL_VAL_OFF); call.len = COL(CK_COL_CALL_VAL_LEN);   // resolved by the walker
-        action = call.len ? CK_ACT_RETURN : CK_ACT_SILENT;
-    }
-    if (action == CK_ACT_RAISES) { COL(CK_COL_ACTION) = action; COL(CK_COL_NOUT) = 0; return; }
-    if (action == CK_ACT_SILENT) {
-        if (mode == 0) { COL(CK_COL_ACTION) = action; COL(CK_COL_NOUT) = 0; return; }
-        // only the handler-return publish: the input envelope, unchanged (nodes/base.py:142, worker.py:52-53)
-        w.add(CK_SRC_INPUT, 0, r.n);
-        w.finish(i);
-        pay_len[i] = cfg.publish_topic_id >= 0 ? r.n : 0;
-        if (cfg.publish_topic_id >= 0) { ck_pub p = none; p.payload = i; p.topic_id = cfg.publish_topic_id; pubs[2 * i + 1] = p; }
-        COL(CK_COL_ACTION) = action; COL(CK_COL_NOUT) = cfg.publish_topic_id >= 0 ? 1 : 0;
-        return;
-    }
-    // ---- the ToolCallPart and an existing result for the same id (spans resolved by the walker)
-    Span args = {COL(CK_COL_ARGS_OFF), COL(CK_COL_ARGS_LEN)};
-    u32 id_off = COL(CK_COL_ARG0_OFF), id_len = COL(CK_COL_ARG0_LEN);
-    Span existing = {COL(CK_COL_RES_OFF), COL(CK_COL_RES_LEN)};
-
-    // ---- the tool's return value as JSON
-    u32 rv_src[CK_TPL_MAX_PARTS], rv_off[CK_TPL_MAX_PARTS], rv_len[CK_TPL_MAX_PARTS], rv_n = 0;
-    if (mode == 0) {
-        // hand the args span to the host: payload = args JSON (1 segment); results come back in mode 1
-        w.add(CK_SRC_INPUT, args.off, args.len);
-        w.finish(i);
-        pay_len[i] = args.len;
-        COL(CK_COL_ACTION) = CK_ACT_HOST_TOOL; COL(CK_COL_NOUT) = 0;
-        return;
-    }
-    if (cfg.tpl_nparts == 0 || aux_off != nullptr) {             // host results, when supplied, win over the template
-        if (aux_off == nullptr) { COL(CK_COL_ACTION) = CK_ACT_HOST_TOOL; COL(CK_COL_NOUT) = 0; return; }
-        long long r0 = aux_off[i], r1 = aux_off[i + 1];
-        rv_src[0] = CK_SRC_AUX; rv_off[0] = (u32)r0; rv_len[0] = (u32)(r1 - r0); rv_n = 1;
-    } else {
-        // device template: literal pieces + raw string arguments of the (object) args
-        bool ok = (r.at(args.off) == '{');
-        for (u32 k = 0; k < cfg.tpl_nparts && ok; k++) {
-            if (cfg.tpl_kind[k] == 0) { rv_src[rv_n] = CK_SRC_LIT; rv_off[rv_n] = cfg.tpl_off[k]; rv_len[rv_n] = cfg.tpl_len[k]; rv_n++; }
-            else {
-                // find member by name in the args object
-                u32 p = args.off + 1; bool found = false;
-                while (p < args.off + args.len && r.at(p) != '}') {
-                    Span k2; ck_string(r, p, k2); p++;
-                    u32 v = p; ck_skip_value(r, p);
-                    bool eq = (k2.len == cfg.tpl_len[k]);
-                    for (u32 b = 0; eq && b < k2.len; b++) eq = (r.at(k2.off + b) == lit[cfg.tpl_off[k] + b]);
-                    if (eq) {
-                        if (r.at(v) != '"') { ok = false; break; }          // non-string argument: host formats it
-                        rv_src[rv_n] = CK_SRC_INPUT; rv_off[rv_n] = v + 1; rv_len[rv_n] = p - v - 2; rv_n++;
-                        found = true; break;
-                    }
-                    if (p < r.n && r.at(p) == ',') p++;
-                }
-                if (!found) ok = false;
-            }
-        }
-        if (!ok) { COL(CK_COL_ACTION) = CK_ACT_RAISES; COL(CK_COL_STATUS) = CK_UNSUPPORTED; COL(CK_COL_NOUT) = 0; return; }
-    }
-
-    // ---- splice plan
-    u32 tr_off = COL(CK_COL_TR_OFF), tr_len = COL(CK_COL_TR_LEN);
-    u32 cur;
-    if (existing.len == 0) {
-        w.add(CK_SRC_INPUT, 0, tr_off + tr_len - 1);                         // up to (not incl.) the closing '}'
-        if (tr_len > 2) w.add(CK_SRC_LIT, cfg.lit_comma_q[0], cfg.lit_comma_q[1]); else w.add(CK_SRC_LIT, cfg.lit_q[0], cfg.lit_q[1]);
-        w.add(CK_SRC_INPUT, id_off, id_len);
-        w.add(CK_SRC_LIT, cfg.lit_open[0], cfg.lit_open[1]);
-        cur = tr_off + tr_len - 1;
-    } else {
-        w.add(CK_SRC_INPUT, 0, existing.off);                                // dict assignment keeps the key's position
-        w.add(CK_SRC_LIT, cfg.lit_value_open[0], cfg.lit_value_open[1]);
-        cur = existing.off + existing.len;
-    }
-    for (u32 k = 0; k < rv_n; k++) w.add(rv_src[k], rv_off[k], rv_len[k]);
-    w.add(CK_SRC_LIT, cfg.lit_mid[0], cfg.lit_mid[1]);
-    w.add(CK_SRC_INPUT, id_off, id_len);
-    w.add(CK_SRC_LIT, cfg.lit_close[0], cfg.lit_close[1]);
-    // state.overrides <- current frame's overrides when that is set (nodes/base.py:66-67)
-    u32 fov_off = COL(CK_COL_FOV_OFF), fov_len = COL(CK_COL_FOV_LEN);
-    if (r.at(fov_off) != 'n') {
-        u32 sov_off = COL(CK_COL_SOV_OFF), sov_len = COL(CK_COL_SOV_LEN);
-        w.add(CK_SRC_INPUT, cur, sov_off - cur);
-        w.add(CK_SRC_INPUT, fov_off, fov_len);
-        cur = sov_off + sov_len;
-    }
-    // unwind the current frame (nodes/base.py:107): drop the last list element and its comma
-    u32 top_off = COL(CK_COL_TOP_OFF), top_len = COL(CK_COL_TOP_LEN);
-    u32 cut0 = nframes > 1 ? top_off - 1 : top_off;
-    w.add(CK_SRC_INPUT, cur, cut0 - cur);
-    w.add(CK_SRC_INPUT, top_off + top_len, r.n - (top_off + top_len));
-    if (!w.finish(i)) { COL(CK_COL_ACTION) = CK_ACT_RAISES; COL(CK_COL_STATUS) = CK_UNSUPPORTED; COL(CK_COL_NOUT) = 0; d->nseg = 0; d->total_len = 0; return; }
-    pay_len[i] = w.total;
-    // publishes: callback (keyed by correlation id), then the handler return value to publish_topic
-    ck_pub p = none; p.payload = i; p.topic_off = COL(CK_COL_CB_OFF); p.topic_len = COL(CK_COL_CB_LEN); p.has_key = 1;
-    pubs[2 * i] = p;
-    u32 nout = 1;
-    if (cfg.publish_topic_id >= 0) { ck_pub q = none; q.payload = i; q.topic_id = cfg.publish_topic_id; pubs[2 * i + 1] = q; nout = 2; }
-    COL(CK_COL_ACTION) = CK_ACT_RETURN; COL(CK_COL_NOUT) = nout;
-#undef COL
-}
-
-__global__ void __launch_bounds__(128, CK_PLAN_MINB)
-ck_plan_tool_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride,
-                    const ck_tool_cfg* __restrict__ cfgp, const u8* __restrict__ lit,
-                    const long long* __restrict__ aux_off, const u8* __restrict__ aux, u8* __restrict__ glue,
-                    int mode, ck_out_desc* __restrict__ descs, u32* __restrict__ pay_len, ck_pub* __restrict__ pubs) {
-    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ck_plan_tool_one(v, i, cols, stride, cfgp, lit, aux_off, aux, glue, mode, descs, pay_len, pubs);
-}
-
 
 // ------------------------------------------------------------------------------------------------
 // agent fan-out: Agent.run's list[Call] branch (reference nodes/agent.py:177-211) followed by
@@ -954,20 +764,86 @@ ck_emit_kernel(ck_view vw, const u8* __restrict__ lit,
 // partition of the key (murmur2, the default partitioner's hash), and a per-topic histogram
 // aggregated inside the warp (match_any + popc: one atomic per distinct topic per warp).
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ u32 ck_murmur2(const u8* data, u32 len) {
-    const u32 m = 0x5bd1e995u; const int rr = 24;
-    u32 h = 0x9747b28cu ^ len;
-    u32 len4 = len >> 2;
-    for (u32 i = 0; i < len4; i++) {
-        u32 k = (u32)data[4 * i] | ((u32)data[4 * i + 1] << 8) | ((u32)data[4 * i + 2] << 16) | ((u32)data[4 * i + 3] << 24);
-        k *= m; k ^= k >> rr; k *= m; h *= m; h ^= k;
+// Kafka's default partitioner hashes the KEY bytes = correlation_id.encode() (nodes/base.py:86): the JSON string
+// content unescaped.  Raw content without a backslash is its own unescaped form (the common case: ids are hex /
+// uuid text); otherwise the escapes pydantic emits (\" \\ \n \t \r \b \f \u00xx) are decoded on the fly.
+template <class R>
+__device__ __forceinline__ u32 ck_key_byte(R& r, u32& p) {
+    u8 c = r.at(p++);
+    if (c != '\\') return c;
+    u8 e = r.at(p++);
+    switch (e) {
+        case 'n': return '\n'; case 't': return '\t'; case 'r': return '\r'; case 'b': return '\b'; case 'f': return '\f';
+        case 'u': {
+            u32 v = 0;
+            for (int k = 0; k < 4; k++) { u8 h = r.at(p++); v = (v << 4) | (u32)(h <= '9' ? h - '0' : (h | 0x20) - 'a' + 10); }
+            return v & 0xffu;                       // canonical \u00xx only (controls); wider code points are emitted raw
+        }
+        default: return e;                           // \" and \\ (and \/ which pydantic never emits)
     }
-    u32 tail = len & 3u, b = len4 << 2;
-    if (tail == 3) h ^= (u32)data[b + 2] << 16;
-    if (tail >= 2) h ^= (u32)data[b + 1] << 8;
-    if (tail >= 1) { h ^= (u32)data[b]; h *= m; }
+}
+template <class R>
+__device__ __forceinline__ u32 ck_murmur2_key(R& r, u32 off, u32 len) {
+    const u32 m = 0x5bd1e995u;
+    // one pass over the raw content, 8 bytes per read: its hash, and whether it holds a backslash at all
+    u32 h = 0x9747b28cu ^ len, len4 = len >> 2, tail = len & 3u;
+    u64 esc = 0;
+    for (u32 i = 0; i < len4; i += 2) {
+        u64 x = r.load8(off + 4 * i);
+        if (i + 1 == len4) x &= 0xffffffffull;          // the last 4-byte block: the bytes after it are not the key's
+        esc |= ck_haszero(x ^ CK_REP8('\\'));
+        u32 k = (u32)x;
+        k *= m; k ^= k >> 24; k *= m; h *= m; h ^= k;
+        if (i + 1 < len4) { k = (u32)(x >> 32); k *= m; k ^= k >> 24; k *= m; h *= m; h ^= k; }
+    }
+    if (tail) {
+        u32 t = (u32)r.load8(off + (len4 << 2)) & (0xffffffu >> (8 * (3 - tail)));
+        esc |= ck_haszero((u64)t ^ CK_REP8('\\'));
+        h ^= t; h *= m;
+    }
+    if (!esc) { h ^= h >> 13; h *= m; h ^= h >> 15; return h; }
+    u32 ulen = 0;
+    for (u32 p = off; p < off + len; ulen++) ck_key_byte(r, p);
+    h = 0x9747b28cu ^ ulen;
+    u32 p = off, k = 0, nb = 0, left = ulen;
+    while (left >= 4) {
+        k = ck_key_byte(r, p); k |= ck_key_byte(r, p) << 8; k |= ck_key_byte(r, p) << 16; k |= ck_key_byte(r, p) << 24;
+        k *= m; k ^= k >> 24; k *= m; h *= m; h ^= k;
+        left -= 4;
+    }
+    u32 t0 = 0, t1 = 0, t2 = 0;
+    nb = left;
+    if (nb >= 1) t0 = ck_key_byte(r, p);
+    if (nb >= 2) t1 = ck_key_byte(r, p);
+    if (nb >= 3) t2 = ck_key_byte(r, p);
+    if (nb == 3) h ^= t2 << 16;
+    if (nb >= 2) h ^= t1 << 8;
+    if (nb >= 1) { h ^= t0; h *= m; }
     h ^= h >> 13; h *= m; h ^= h >> 15;
     return h;
+}
+
+// topic string (raw JSON content at [off, off+len) of the record) -> registered id, -1 if not registered
+template <class R>
+__device__ __forceinline__ int ck_topic_lookup(R& r, u32 off, u32 len, const ck_topic_table& tab, u32* hash_out = nullptr) {
+    u32 h = 2166136261u;
+    for (u32 i = 0; i < len; i++) h = (h ^ r.at(off + i)) * 16777619u;
+    if (!h) h = 1u;
+    if (hash_out) *hash_out = h;          // unregistered topics (a client's reply topic): the host groups them by this hash
+    if (!len || !tab.cap) return -1;
+    u32 slot = h & (tab.cap - 1);
+    for (u32 probe = 0; probe < tab.cap; probe++) {
+        u32 th = tab.hash[slot];
+        if (th == 0) return -1;
+        if (th == h && tab.name_len[slot] == len) {
+            const u8* nm = tab.names + tab.name_off[slot];
+            bool eq = true;
+            for (u32 b = 0; b < len; b++) if (nm[b] != r.at(off + b)) { eq = false; break; }
+            if (eq) return tab.id[slot];
+        }
+        slot = (slot + 1) & (tab.cap - 1);
+    }
+    return -1;
 }
 
 __global__ void __launch_bounds__(256)
@@ -980,27 +856,13 @@ ck_route_kernel(ck_view vw, const u32* __restrict__ cols, u32 stride,
     int tid = -1;
     if (live) {
         u32 rec_len; const u8* rec = ck_rec(vw, p.record, rec_len);
+        GRd r; r.init(rec, rec_len);
         tid = p.topic_id;
-        if (tid < 0 && p.topic_len && tab.cap) {
-            u32 h = ck_fnv1a(rec + p.topic_off, p.topic_len);
-            pubs[j].pad = h;
-            u32 slot = h & (tab.cap - 1);
-            for (u32 probe = 0; probe < tab.cap; probe++) {
-                u32 th = tab.hash[slot];
-                if (th == 0) break;
-                if (th == h && tab.name_len[slot] == p.topic_len) {
-                    const u8* nm = tab.names + tab.name_off[slot];
-                    bool eq = true;
-                    for (u32 b = 0; b < p.topic_len; b++) if (nm[b] != rec[p.topic_off + b]) { eq = false; break; }
-                    if (eq) { tid = tab.id[slot]; break; }
-                }
-                slot = (slot + 1) & (tab.cap - 1);
-            }
-        }
+        if (tid < 0 && p.topic_len && tab.cap) tid = ck_topic_lookup(r, p.topic_off, p.topic_len, tab, &pubs[j].pad);
         int part = -1;
         if (p.has_key && num_partitions) {
             u32 co = cols[(size_t)CK_COL_CORR_OFF * stride + p.record], cl = cols[(size_t)CK_COL_CORR_LEN * stride + p.record];
-            part = (int)((ck_murmur2(rec + co, cl) & 0x7fffffffu) % num_partitions);
+            part = (int)((ck_murmur2_key(r, co, cl) & 0x7fffffffu) % num_partitions);
         }
         pubs[j].topic_id = tid;
         pubs[j].partition = part;
@@ -1014,7 +876,7 @@ ck_route_kernel(ck_view vw, const u32* __restrict__ cols, u32 stride,
 }
 
 #include "ck_walk_long.cuh"
-#include "ck_plan2.cuh"
+#include "ck_plan.cuh"
 #include "ck_fanout2.cuh"
 #include "ck_gate.cuh"
 #include "ck_kafka.cuh"

@@ -54,7 +54,8 @@ int  ck_register_topics(ck_handle* h, const uint8_t* names, const uint32_t* offs
 /* configure the handle for one @agent_tool node (calfkit/nodes/tool.py:24-35,89-95).
  * publish_topic_id: registered id of node.publish_topic or -1.
  * Result template (optional, nparts > 0): the tool's return value is the JSON string made of
- * literal pieces (kind 0, already JSON-escaped) and raw string arguments (kind 1, blob = key name);
+ * literal pieces (kind 0, already JSON-escaped) and raw string arguments (kind 1, blob = key name),
+ * at most 5 parts (more is an error: the splice would not fit one output descriptor);
  * nparts == 0: results are supplied by the host through ck_tool_plan(aux). */
 int  ck_set_tool_node(ck_handle* h, int32_t publish_topic_id, uint32_t nparts, const uint32_t* kinds,
                       const uint8_t* blob, const uint32_t* part_offsets);

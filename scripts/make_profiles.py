@@ -19,7 +19,7 @@ for name in ("launches.csv", "pytest_gpu.log", "sass_mnemonics.txt", "exchange_p
         shutil.copy(src, os.path.join(P, f"{R}_{name}"))
 traffic = {}
 def nrec_of(k): return 4096 if k == "walk_long" else (65536 if k in ("prescan_mixed", "walk_elems") else NREC)
-for k, short in (("walk", "walk"), ("plan_tool2", "plan"), ("emit", "emit"), ("walk_long", "walk_long"), ("prescan_mixed", "prescan_mixed"), ("walk_elems", "walk_elems")):
+for k, short in (("walk", "walk"), ("plan_tool", "plan"), ("emit", "emit"), ("walk_long", "walk_long"), ("prescan_mixed", "prescan_mixed"), ("walk_elems", "walk_elems")):
     rep = os.path.join(G, f"{R}_{k}.ncu-rep")
     if not os.path.exists(rep):
         continue

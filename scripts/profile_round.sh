@@ -16,7 +16,7 @@ timeout 600 python bench.py --impl reference --steps 3 --warmup 1 > $O/${R}_benc
 timeout 900 ncu --metrics gpu__time_duration.sum --clock-control none -c 800 --csv --log-file $O/${R}_launches.csv \
     python bench.py --steps 2 --warmup 3 --events 262144 --cpu-sample 2000 > $O/${R}_launches_bench.log 2>&1
 # full captures of the heaviest kernels (one launch each, after warm-up launches)
-for k in walk plan_tool2 emit; do
+for k in walk plan_tool emit; do
   timeout 900 ncu --set full --clock-control none --import-source on -k regex:ck_${k}_kernel -s 3 -c 1 -f -o $O/${R}_${k} \
       python scripts/quick_bench.py 1048576 > $O/${R}_ncu_${k}.log 2>&1
 done

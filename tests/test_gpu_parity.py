@@ -201,16 +201,39 @@ def test_device_walker_equals_host_build_on_fuzz(engine):
         n_long += 1
     assert n_long >= 40
 
+# correlation ids whose JSON spelling has escapes: the Kafka key is the unescaped string (reference nodes/base.py:86)
+ESCAPED_CORR_IDS = ['q"uote', "back\\slash", "new\nline", "ctl\x01", "Zürich-東京", 'all"\\\n\x01é']
+
+
+def _with_corr_ids(recs: list[bytes], ids: list[str]) -> list[bytes]:
+    """`recs` with their correlation ids replaced by `ids`, canonical again through the oracle"""
+    from oracle import port
+    out = []
+    for r, cid in zip(recs, ids):
+        obj = json.loads(r)
+        obj["context"]["deps"]["correlation_id"] = cid
+        out.append(port.encode(port.decode(json.dumps(obj, ensure_ascii=False).encode())))
+    return out
+
+
+def _check_partitions(pubs, want):
+    """every keyed publish is on the Kafka default partitioner's partition of the oracle's key"""
+    for p, (_t, key, *_rest) in zip(pubs, want):
+        if key is not None:
+            assert p.partition == (_murmur2(key) & 0x7FFFFFFF) % 8, (key, p.partition)
+
+
 def test_fanout_matches_oracle(engine):
     """Agent fan-out (config 3): every pending tool call -> one Call envelope, frame ids injected into
-    the oracle from the device's own uuid7 generator (seed, slot index)."""
+    the oracle from the device's own uuid7 generator (seed, slot index).  Some correlation ids need JSON escapes."""
     from oracle import port
     from calfkit import _ids, synth
     from calfkit.engine.batch import device_uuid7_hex
     from calfkit.engine import BatchEngine
     F = 16
     recs = synth.fanout_events(40, seed=9, fanout=F) + synth.fanout_events(5, seed=10, fanout=1) + \
-        [as_bytes(golden("actions.json")[0]["input"])]
+        [as_bytes(golden("actions.json")[0]["input"])] + \
+        _with_corr_ids(synth.fanout_events(3, seed=11, fanout=3) + synth.fanout_events(3, seed=12, fanout=1), ESCAPED_CORR_IDS)
     registry = {f"tool_{j:02d}": f"tool.tool_{j:02d}.input" for j in range(64)}
     e = BatchEngine(0, max_records=256, max_in_bytes=8 << 20, max_out_bytes=256 << 20, max_payloads=256 * (F + 1))
     try:
@@ -235,6 +258,7 @@ def test_fanout_matches_oracle(engine):
                 _ids.set_id_source(None)
             got = [(p.topic, p.key, p.payload) for p in pubs[k:k + len(want)]]
             assert got == [(t, kk, pl) for (t, kk, c, pl) in want], i
+            _check_partitions(pubs[k:k + len(want)], want)
             k += len(want)
             slot += npend + (1 if npend > 1 else 0)
         assert k == len(pubs)
@@ -244,14 +268,16 @@ def test_fanout_matches_oracle(engine):
 
 def test_sequential_call_and_tailcall_match_oracle(engine):
     """Agent(sequential_only_mode=True): first pending call only, as a single Call; no pending call at
-    all -> TailCall to the agent's own topic (reference nodes/agent.py:94-108,171-175; nodes/base.py:90-136)."""
+    all -> TailCall to the agent's own topic (reference nodes/agent.py:94-108,171-175; nodes/base.py:90-136).  Some
+    correlation ids need JSON escapes."""
     from oracle import port
     from calfkit import _ids, synth
     from calfkit.engine.batch import device_uuid7_hex
     from calfkit.engine import BatchEngine
-    recs = synth.fanout_events(12, seed=3, fanout=5) + synth.fanout_events(3, seed=4, fanout=1)
+    recs = synth.fanout_events(12, seed=3, fanout=5) + synth.fanout_events(3, seed=4, fanout=1) + \
+        _with_corr_ids(synth.fanout_events(6, seed=13, fanout=4), ESCAPED_CORR_IDS)
     registry = {f"tool_{j:02d}": f"tool.tool_{j:02d}.input" for j in range(64)}
-    e = BatchEngine(0, max_records=64, max_in_bytes=8 << 20, max_out_bytes=64 << 20, max_payloads=256)
+    e = BatchEngine(0, max_records=128, max_in_bytes=8 << 20, max_out_bytes=64 << 20, max_payloads=256)
     try:
         e.register_topics(list(registry.values()) + ["planner.input", "planner.output"], num_partitions=8)
         e.set_agent_node("planner", "planner.input", "planner.output", registry)
@@ -270,8 +296,10 @@ def test_sequential_call_and_tailcall_match_oracle(engine):
             finally:
                 _ids.set_id_source(None)
             assert [(p.topic, p.key, p.payload) for p in pubs[2 * i:2 * i + 2]] == [(t, k, pl) for (t, k, c, pl) in want], i
+            _check_partitions(pubs[2 * i:2 * i + 2], want)
         # TailCall: tool-stage events (a frame with input_args, overrides on some) + the golden TailCall input
-        recs2 = synth.tool_events(40, seed=5) + synth.mixed_events(20, seed=6)
+        recs2 = synth.tool_events(40, seed=5) + synth.mixed_events(20, seed=6) + \
+            _with_corr_ids(synth.tool_events(6, seed=14), ESCAPED_CORR_IDS)
         b2 = synth.pack(recs2)
         e.submit(b2.data, b2.offsets)
         e.tailcall_plan(ms, seed)
@@ -292,6 +320,7 @@ def test_sequential_call_and_tailcall_match_oracle(engine):
                 _ids.set_id_source(None)
             want = [(t, kk, port.encode(en)) for (t, kk, c, en) in got_pubs] + [("planner.output", None, port.encode(returned))]
             assert [(p.topic, p.key, p.payload) for p in pubs[k:k + 2]] == want, i
+            _check_partitions(pubs[k:k + 2], want)
             k += 2
         assert k == len(pubs)
     finally:

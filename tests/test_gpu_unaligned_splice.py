@@ -1,7 +1,7 @@
 """Tool plans whose pieces fall at any byte of the payload: call ids and template arguments shorter than a 16-byte
 vector (an empty argument included), 1-byte template literals, frame overrides and existing results, so that many
-output vectors overlap three or more segments of the splice.  Every publish is compared with the oracle.  The last
-case needs more segments than a descriptor holds and goes, record by record, to the global-memory planner."""
+output vectors overlap three or more segments of the splice.  Every publish is compared with the oracle.  A splice
+never needs more segments than a descriptor holds: templates of more than five parts are refused."""
 import json
 import random
 import string
@@ -84,23 +84,40 @@ def test_short_ids_and_arguments_match_oracle(engine, fmt):
     _check(engine, recs, port.ToolNode(get_weather, "tool_get_weather", [TOPICS[0]], TOPICS[1]))
 
 
-def test_more_pieces_than_a_descriptor_holds_match_oracle(engine):
-    """A template of six parts (four adjacent arguments): with frame overrides the splice has 17 pieces, one more than a
-    descriptor holds, so those records take the global-memory planner; without overrides they stay on the staged path."""
+def _pieces(r: bytes) -> int:
+    """non-empty pieces of the splice (ck_plan_tool_one) under the five-part template "<{a}|{b}>" """
+    obj = json.loads(r)
+    st, top = obj["context"]["state"], obj["internal_workflow_state"]["call_stack"]["_internal_list"][-1]
+    (cid, part), = st["tool_calls"].items()
+    return (2 if cid in st["tool_results"] else 4) + 3 + sum(1 for v in part["args"].values() if v) + 3 + \
+        (2 if top["overrides"] is not None else 0) + 2
+
+
+def _concat_node():
     from oracle import port
+
+    def concat(a: str, b: str) -> str:
+        return f"<{a}|{b}>"
+    return port.ToolNode(concat, "tool_get_weather", [TOPICS[0]], TOPICS[1])
+
+
+def test_worst_case_splice_fills_a_descriptor_and_matches_oracle(engine):
+    """A five-part template with three non-empty literals and non-empty arguments: records with frame overrides and no
+    existing result have 16 pieces, as many as a descriptor holds (CK_TOOL_FIXED_PIECES + CK_TPL_MAX_PARTS)."""
     from calfkit.engine import ToolTemplate
+    engine.set_tool_node("tool.get_weather.output", ToolTemplate.from_format("<{a}|{b}>"))
+    recs = _records(200, 73, lambda rng, k: {key: rng.choice(VALUES[1:]) for key in ("b", "a")})
+    n = [_pieces(r) for r in recs]
+    assert max(n) == 16 and sum(k == 16 for k in n) >= 10 and sum(k < 16 for k in n) >= 10
+    _check(engine, recs, _concat_node())
 
-    def concat(a: str, b: str, c: str, d: str) -> str:
-        return a + b + c + d
-    engine.set_tool_node("tool.get_weather.output", ToolTemplate([0, 1, 1, 1, 1, 0], [b'"', b"a", b"b", b"c", b"d", b'"']))
-    recs = _records(200, 73, lambda rng, k: {key: rng.choice(VALUES) for key in ("d", "b", "a", "c")})
 
-    def pieces(r: bytes) -> int:           # non-empty pieces of the splice (ck_plan_tool2_one)
-        obj = json.loads(r)
-        st, top = obj["context"]["state"], obj["internal_workflow_state"]["call_stack"]["_internal_list"][-1]
-        (part,) = st["tool_calls"].values()
-        return (2 if st["tool_results"] else 4) + 2 + sum(1 for v in part["args"].values() if v) + 3 + \
-            (2 if top["overrides"] is not None else 0) + 2
-    n = [pieces(r) for r in recs]
-    assert sum(k > 16 for k in n) >= 10 and sum(k <= 16 for k in n) >= 10
-    _check(engine, recs, port.ToolNode(concat, "tool_get_weather", [TOPICS[0]], TOPICS[1]))
+def test_six_part_template_is_refused(engine):
+    """A descriptor has no room for a six-part template's splice: set_tool_node refuses it, and the node's template
+    stays usable afterwards."""
+    from calfkit.engine import ToolTemplate
+    from calfkit.exceptions import EngineError
+    with pytest.raises(EngineError, match="too many template parts"):
+        engine.set_tool_node("tool.get_weather.output", ToolTemplate([0, 1, 1, 1, 1, 0], [b'"', b"a", b"b", b"c", b"d", b'"']))
+    engine.set_tool_node("tool.get_weather.output", ToolTemplate.from_format("<{a}|{b}>"))
+    _check(engine, _records(60, 79, lambda rng, k: {"a": rng.choice(VALUES), "b": rng.choice(VALUES)}), _concat_node())
