@@ -724,8 +724,11 @@ ck_emit_kernel(ck_view vw, const u8* __restrict__ lit,
     u32 nvec = (total + 15u) >> 4;
     // warp-uniform choice per payload: in the aligned layout (SegWriter: every segment starts on a vector, all but the
     // last are whole vectors) no vector crosses a segment, and the segment of a vector is found without a search — the
-    // lanes holding the table mark the vectors where a segment starts, one warp-wide OR gives the mask, a popcount the index
-    bool aligned = __all_sync(0xffffffffu, lane >= nseg || ((start & 15u) == 0 && (lane + 1 == nseg || (my_len & 15u) == 0)));
+    // lanes holding the table mark the vectors where a segment starts, one warp-wide OR gives the mask, a popcount the index.
+    // The popcount counts non-empty segments only, so it is a lane index only if no empty segment comes before the last one:
+    // an empty segment is not a whole vector, and a payload with one before its last segment takes the search below
+    u32 part = my_len ? (my_len & 15u) : 1u;         // 0: the segment is one or more whole vectors
+    bool aligned = __all_sync(0xffffffffu, lane >= nseg || ((start & 15u) == 0 && (lane + 1 == nseg || part == 0)));
     ck_emit_segs* tab = &s_tab[threadIdx.x >> 5];
     if (!aligned) {                          // the table for the boundary lanes
         if (lane < CK_MAX_SEGS) { tab->ptr[lane] = my_ptr; tab->start[lane] = start; tab->end[lane] = end; }

@@ -203,6 +203,28 @@ def test_device_walker_equals_host_build_on_fuzz(engine):
 
 # correlation ids whose JSON spelling has escapes: the Kafka key is the unescaped string (reference nodes/base.py:86)
 ESCAPED_CORR_IDS = ['q"uote', "back\\slash", "new\nline", "ctl\x01", "Zürich-東京", 'all"\\\n\x01é']
+# a keyed publish's partition over this many partitions is 31 bits of the key's murmur2
+ALL_BITS = 0x7FFFFFFF
+
+
+def corr_ids_of_every_length() -> list[str]:
+    """correlation ids whose Kafka key is 0-80 bytes long, and a few of 200 and more: one plain ASCII id per length, and
+    one per length with a quote, backslash, newline, control character or multi-byte character on or across a 4- or
+    8-byte block edge and a backslash every 9 bytes after it (the key hash reads the raw JSON 8 bytes at a time)"""
+    fill = "0123456789abcdef-_xyzXYZ"
+    specials = ['"', "\\", "\n", "\x01", "é", "東", "😀"]
+    out = []
+    for L in list(range(81)) + [200, 203, 256, 301]:
+        out.append("".join(fill[(L + k) % len(fill)] for k in range(L)))
+        c = specials[L % len(specials)]
+        w = len(c.encode())
+        if L < w:
+            continue
+        edge = 8 * (L // 16) + (4 if L % 2 else 0)          # a 4- or 8-byte block edge inside the id
+        p = max(0, min(edge - w // 2, L - w))               # the special starts on it or straddles it
+        tail = "".join("\\" if k % 9 == 4 else fill[k % len(fill)] for k in range(L - p - w))
+        out.append("".join(fill[k % len(fill)] for k in range(p)) + c + tail)
+    return out
 
 
 def _with_corr_ids(recs: list[bytes], ids: list[str]) -> list[bytes]:
@@ -216,16 +238,17 @@ def _with_corr_ids(recs: list[bytes], ids: list[str]) -> list[bytes]:
     return out
 
 
-def _check_partitions(pubs, want):
+def _check_partitions(pubs, want, nparts=8):
     """every keyed publish is on the Kafka default partitioner's partition of the oracle's key"""
     for p, (_t, key, *_rest) in zip(pubs, want):
         if key is not None:
-            assert p.partition == (_murmur2(key) & 0x7FFFFFFF) % 8, (key, p.partition)
+            assert p.partition == (_murmur2(key) & 0x7FFFFFFF) % nparts, (key, p.partition)
 
 
 def test_fanout_matches_oracle(engine):
     """Agent fan-out (config 3): every pending tool call -> one Call envelope, frame ids injected into
-    the oracle from the device's own uuid7 generator (seed, slot index).  Some correlation ids need JSON escapes."""
+    the oracle from the device's own uuid7 generator (seed, slot index).  Some correlation ids need JSON escapes; ids of
+    every length 0-80 and some of 200+ check 31 bits of the key hash through the route kernel."""
     from oracle import port
     from calfkit import _ids, synth
     from calfkit.engine.batch import device_uuid7_hex
@@ -234,10 +257,12 @@ def test_fanout_matches_oracle(engine):
     recs = synth.fanout_events(40, seed=9, fanout=F) + synth.fanout_events(5, seed=10, fanout=1) + \
         [as_bytes(golden("actions.json")[0]["input"])] + \
         _with_corr_ids(synth.fanout_events(3, seed=11, fanout=3) + synth.fanout_events(3, seed=12, fanout=1), ESCAPED_CORR_IDS)
+    long_ids = corr_ids_of_every_length()
+    recs += _with_corr_ids(synth.fanout_events(len(long_ids), seed=15, fanout=2), long_ids)
     registry = {f"tool_{j:02d}": f"tool.tool_{j:02d}.input" for j in range(64)}
     e = BatchEngine(0, max_records=256, max_in_bytes=8 << 20, max_out_bytes=256 << 20, max_payloads=256 * (F + 1))
     try:
-        e.register_topics(list(registry.values()) + ["planner.input", "planner.output"], num_partitions=8)
+        e.register_topics(list(registry.values()) + ["planner.input", "planner.output"], num_partitions=ALL_BITS)
         e.set_agent_node("planner", "planner.input", "planner.output", registry)
         b = synth.pack(recs)
         ms, seed = 1767225600000, 1234
@@ -258,7 +283,7 @@ def test_fanout_matches_oracle(engine):
                 _ids.set_id_source(None)
             got = [(p.topic, p.key, p.payload) for p in pubs[k:k + len(want)]]
             assert got == [(t, kk, pl) for (t, kk, c, pl) in want], i
-            _check_partitions(pubs[k:k + len(want)], want)
+            _check_partitions(pubs[k:k + len(want)], want, ALL_BITS)
             k += len(want)
             slot += npend + (1 if npend > 1 else 0)
         assert k == len(pubs)
@@ -269,17 +294,19 @@ def test_fanout_matches_oracle(engine):
 def test_sequential_call_and_tailcall_match_oracle(engine):
     """Agent(sequential_only_mode=True): first pending call only, as a single Call; no pending call at
     all -> TailCall to the agent's own topic (reference nodes/agent.py:94-108,171-175; nodes/base.py:90-136).  Some
-    correlation ids need JSON escapes."""
+    correlation ids need JSON escapes; ids of every length 0-80 and some of 200+ check 31 bits of the key hash."""
     from oracle import port
     from calfkit import _ids, synth
     from calfkit.engine.batch import device_uuid7_hex
     from calfkit.engine import BatchEngine
     recs = synth.fanout_events(12, seed=3, fanout=5) + synth.fanout_events(3, seed=4, fanout=1) + \
         _with_corr_ids(synth.fanout_events(6, seed=13, fanout=4), ESCAPED_CORR_IDS)
+    long_ids = corr_ids_of_every_length()
+    recs += _with_corr_ids(synth.fanout_events(len(long_ids), seed=16, fanout=3), long_ids)
     registry = {f"tool_{j:02d}": f"tool.tool_{j:02d}.input" for j in range(64)}
-    e = BatchEngine(0, max_records=128, max_in_bytes=8 << 20, max_out_bytes=64 << 20, max_payloads=256)
+    e = BatchEngine(0, max_records=256, max_in_bytes=8 << 20, max_out_bytes=64 << 20, max_payloads=512)
     try:
-        e.register_topics(list(registry.values()) + ["planner.input", "planner.output"], num_partitions=8)
+        e.register_topics(list(registry.values()) + ["planner.input", "planner.output"], num_partitions=ALL_BITS)
         e.set_agent_node("planner", "planner.input", "planner.output", registry)
         b = synth.pack(recs)
         ms, seed = 1767225600000, 77
@@ -296,10 +323,11 @@ def test_sequential_call_and_tailcall_match_oracle(engine):
             finally:
                 _ids.set_id_source(None)
             assert [(p.topic, p.key, p.payload) for p in pubs[2 * i:2 * i + 2]] == [(t, k, pl) for (t, k, c, pl) in want], i
-            _check_partitions(pubs[2 * i:2 * i + 2], want)
+            _check_partitions(pubs[2 * i:2 * i + 2], want, ALL_BITS)
         # TailCall: tool-stage events (a frame with input_args, overrides on some) + the golden TailCall input
         recs2 = synth.tool_events(40, seed=5) + synth.mixed_events(20, seed=6) + \
-            _with_corr_ids(synth.tool_events(6, seed=14), ESCAPED_CORR_IDS)
+            _with_corr_ids(synth.tool_events(6, seed=14), ESCAPED_CORR_IDS) + \
+            _with_corr_ids(synth.tool_events(len(long_ids), seed=17), long_ids)
         b2 = synth.pack(recs2)
         e.submit(b2.data, b2.offsets)
         e.tailcall_plan(ms, seed)
@@ -320,7 +348,7 @@ def test_sequential_call_and_tailcall_match_oracle(engine):
                 _ids.set_id_source(None)
             want = [(t, kk, port.encode(en)) for (t, kk, c, en) in got_pubs] + [("planner.output", None, port.encode(returned))]
             assert [(p.topic, p.key, p.payload) for p in pubs[k:k + 2]] == want, i
-            _check_partitions(pubs[k:k + 2], want)
+            _check_partitions(pubs[k:k + 2], want, ALL_BITS)
             k += 2
         assert k == len(pubs)
     finally:
@@ -698,21 +726,6 @@ def test_mixed_sizes_256_topics_config5(engine):
         assert len({t for t, *_ in got}) > 200             # 700 records spread over 256 callback topics + the publish topic
     finally:
         e.close()
-
-
-def _murmur2(data: bytes) -> int:
-    m, h = 0x5BD1E995, (0x9747B28C ^ len(data)) & 0xFFFFFFFF
-    n4 = len(data) // 4
-    for i in range(n4):
-        k = int.from_bytes(data[4 * i:4 * i + 4], "little")
-        k = (k * m) & 0xFFFFFFFF; k ^= k >> 24; k = (k * m) & 0xFFFFFFFF
-        h = (h * m) & 0xFFFFFFFF; h ^= k
-    t = data[4 * n4:]
-    if len(t) == 3: h ^= t[2] << 16
-    if len(t) >= 2: h ^= t[1] << 8
-    if len(t) >= 1: h ^= t[0]; h = (h * m) & 0xFFFFFFFF
-    h ^= h >> 13; h = (h * m) & 0xFFFFFFFF; h ^= h >> 15
-    return h
 
 
 DECLARED_UNSUPPORTED = {"frame_missing_frame_id": "default_factory field: the reference invents a fresh id"}

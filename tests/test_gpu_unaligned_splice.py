@@ -1,12 +1,15 @@
 """Tool plans whose pieces fall at any byte of the payload: call ids and template arguments shorter than a 16-byte
 vector (an empty argument included), 1-byte template literals, frame overrides and existing results, so that many
 output vectors overlap three or more segments of the splice.  Every publish is compared with the oracle.  A splice
-never needs more segments than a descriptor holds: templates of more than five parts are refused."""
+never needs more segments than a descriptor holds: templates of more than five parts are refused.  Correlation ids of
+every length and host results of every length put the key hash and the host's piece at every alignment; the engine has
+2^31 - 1 partitions, so a publish's partition is 31 bits of its key's hash."""
 import json
 import random
 import string
 
 import pytest
+from test_gpu_parity import ALL_BITS, _host_tool, _murmur2, _with_corr_ids, corr_ids_of_every_length
 
 pytestmark = pytest.mark.gpu
 
@@ -23,7 +26,7 @@ def engine():
         pytest.skip("no CUDA device")
     from calfkit.engine import BatchEngine
     e = BatchEngine(device=0, max_records=1 << 12, max_in_bytes=16 << 20)
-    e.register_topics(TOPICS, num_partitions=8)
+    e.register_topics(TOPICS, num_partitions=ALL_BITS)
     yield e
     e.close()
 
@@ -59,14 +62,15 @@ def _records(n: int, seed: int, make_args) -> list[bytes]:
     return out
 
 
-def _check(engine, recs, node):
+def _check(engine, recs, node, host_tool=None):
     from oracle import port
     from calfkit import synth
     b = synth.pack(recs)
-    out = engine.run_tool_batch(b.data, b.offsets)
+    out = engine.run_tool_batch(b.data, b.offsets, host_tool)
     assert (out.cols[0] == 0).all()
-    got = [(p.topic, p.key, p.payload) for p in out.publishes()]
-    want = [(t, k, pl) for r in recs for (t, k, _c, pl) in port.tool_node_event(node, r)]
+    got = [(p.topic, p.key, p.payload, p.partition) for p in out.publishes()]
+    want = [(t, k, pl, -1 if k is None else (_murmur2(k) & 0x7FFFFFFF) % ALL_BITS)
+            for r in recs for (t, k, _c, pl) in port.tool_node_event(node, r)]
     assert len(got) == len(want) == 2 * len(recs)
     for i in range(len(recs)):
         assert got[2 * i:2 * i + 2] == want[2 * i:2 * i + 2], (i, recs[i][:120])
@@ -81,7 +85,26 @@ def test_short_ids_and_arguments_match_oracle(engine, fmt):
         return fmt.format(location=location)
     engine.set_tool_node("tool.get_weather.output", ToolTemplate.from_format(fmt))
     recs = _records(600, 71, lambda rng, k: {"location": VALUES[k % len(VALUES)] if k < 300 else rng.choice(VALUES)})
+    ids = corr_ids_of_every_length()            # the key hash through the plan's shared-memory window
+    recs += _with_corr_ids(_records(len(ids), 72, lambda rng, k: {"location": rng.choice(VALUES)}), ids)
     _check(engine, recs, port.ToolNode(get_weather, "tool_get_weather", [TOPICS[0]], TOPICS[1]))
+
+
+def _text(rng, n: int) -> str:
+    """n characters of ASCII, multi-byte UTF-8 and characters JSON escapes"""
+    return "".join(rng.choice(string.ascii_letters + ' "\\\n\t\x01\x1féü東😀') for _ in range(n))
+
+
+def test_host_results_of_every_length_match_oracle(engine):
+    """A host tool that returns its string argument: results of 0-300 characters with escapes and multi-byte UTF-8, so
+    that the host's piece of the splice starts and ends at every alignment of the payload."""
+    from oracle import port
+
+    def get_weather(location: str) -> str:
+        return location
+    engine.set_tool_node("tool.get_weather.output", None)
+    recs = _records(700, 81, lambda rng, k: {"location": _text(rng, k % 301 if k < 602 else rng.randrange(301))})
+    _check(engine, recs, port.ToolNode(get_weather, "tool_get_weather", [TOPICS[0]], TOPICS[1]), _host_tool(get_weather))
 
 
 def _pieces(r: bytes) -> int:
