@@ -39,7 +39,7 @@ PUB_DTYPE = np.dtype([("payload", "<u4"), ("topic_id", "<i4"), ("topic_off", "<u
 EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_register_topics", "ck_set_tool_node", "ck_submit",
            "ck_submit_device", "ck_tool_args", "ck_tool_plan", "ck_tool_plan_device", "ck_return_plan", "ck_set_agent_node", "ck_set_agent_tool_topic_ids", "ck_fanout_plan", "ck_tailcall_plan", "ck_exchange_plan", "ck_launch_count", "ck_reply_plan",
            "ck_sync", "ck_out_size", "ck_fetch_columns", "ck_fetch_output", "ck_fetch_overlay", "ck_fetch_topic_hist", "ck_stream",
-           "ck_device_buffers", "ck_device_buffers2", "ck_gather_spans", "ck_profile", "ck_profile_read", "ck_fetch_cols",
+           "ck_device_buffers", "ck_device_buffers2", "ck_profile", "ck_profile_read", "ck_fetch_cols",
            "ck_host_alloc", "ck_host_free", "ck_canon_stats", "ck_fetch_output_async",
            "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_reset", "ck_submit_recordbatch",
            "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option"]
@@ -113,7 +113,6 @@ def load() -> C.CDLL:
         "ck_stream": (vp, [vp]),
         "ck_device_buffers": (C.c_int, [vp] + [C.POINTER(vp)] * 5),
         "ck_device_buffers2": (C.c_int, [vp] + [C.POINTER(vp)] * 3),
-        "ck_gather_spans": (C.c_int, [vp, u8p, i64p, i64p, C.c_uint32, u8p, i64p]),
         "ck_profile": (C.c_int, [vp, C.c_int]),
         "ck_profile_read": (C.c_int, [vp, vp, vp, C.c_int]),
     }

@@ -1,18 +1,17 @@
 """Cross-partition exchange (SURVEY.md §8e): records shard by Kafka partition across the GPUs of a
-box; the only data-path collective is ONE variable-size all-to-all per batch that forwards the keyed
-payloads whose partition (murmur2(correlation_id) % num_partitions, computed by ck_route_kernel) is
-owned by another rank.  Reference analogue: the record would simply be produced to a topic-partition
-that a different worker process consumes (calfkit/nodes/base.py:82-87 key=correlation_id).
+box, and each batch forwards the keyed payloads whose partition (murmur2(correlation_id) % num_partitions,
+computed by ck_route_kernel) is owned by another rank.  Reference analogue: the record would simply be produced
+to a topic-partition that a different worker process consumes (calfkit/nodes/base.py:82-87 key=correlation_id).
 
-Production path (`PeerExchange`): every rank maps its peers' receive buffers (CUDA IPC over NVSwitch) and
-`ck_exchange_send` plans, packs and transfers in one pass on the device — a warp per forwarded payload stores it straight
-into the owner's region — with no host synchronisation and no library collective (the two barriers of a step are flag
-words in peer memory); torch.distributed is used once, for the handle exchange.  The tensor-level `plan_exchange` / `exchange` below is the device-agnostic statement of the
-same plan (CPU tensors under the gloo tests; the kernels are pinned to it on the GPU)."""
+`PeerExchange`: every rank maps its peers' receive buffers (CUDA IPC over NVSwitch) and `ck_exchange_send` plans,
+packs and transfers in one pass on the device — a warp per forwarded payload stores it straight into the owner's
+region — with no host synchronisation and no library collective (the two barriers of a step are flag words in peer
+memory); torch.distributed is used once, for the handle exchange.  `plan_exchange` below is the device-agnostic
+tensor statement of the same selection (tested on CPU tensors); `plan_exchange_device` runs the library's plan
+kernels, which are pinned to it on the GPU."""
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable
 
 import torch
 import torch.distributed as dist
@@ -56,7 +55,7 @@ class _DevArray:
 def plan_exchange_device(engine, rank: int, world: int, device) -> ExchangePlan:
     """The same plan as plan_exchange(), computed by the library's own kernels (ck_exchange_plan: histogram ->
     scan -> stable scatter -> scan) instead of a dozen tensor ops over the whole publish table; one host
-    synchronisation instead of three.  `counts` / `nbytes` are host tensors (the all-to-all split sizes)."""
+    synchronisation instead of three.  `counts` / `nbytes` are host tensors (payloads / bytes per destination)."""
     import ctypes as C
     src, ln, dst, pub = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
     counts = torch.zeros(world, dtype=torch.int64)
@@ -70,27 +69,6 @@ def plan_exchange_device(engine, rank: int, world: int, device) -> ExchangePlan:
         return ExchangePlan(z, z, z, z, counts, nbytes)
     as_t = lambda p, ts: torch.as_tensor(_DevArray(p.value, n, ts), device=device)   # noqa: E731
     return ExchangePlan(as_t(pub, "<u4"), as_t(src, "<i8"), as_t(ln, "<i8"), as_t(dst, "<i8"), counts, nbytes)
-
-
-def exchange(plan: ExchangePlan, gather: Callable[[ExchangePlan, torch.Tensor], None], send_buf: torch.Tensor,
-             recv_buf: torch.Tensor) -> tuple[int, int, torch.Tensor]:
-    """gather(plan, send_buf) packs the selected payloads; returns (n received payloads, received bytes,
-    their lengths)."""
-    if int(plan.nbytes.sum()) > send_buf.numel():
-        raise RuntimeError("exchange send buffer too small")          # before the pack kernel writes anything
-    gather(plan, send_buf)
-    meta_out = torch.stack([plan.counts, plan.nbytes], 1).contiguous().to(plan.lens.device)
-    meta_in = torch.empty_like(meta_out)
-    dist.all_to_all_single(meta_in, meta_out)
-    mo, mi = torch.stack([plan.counts, plan.nbytes], 1).tolist(), meta_in.tolist()
-    sc, sb = [x[0] for x in mo], [x[1] for x in mo]
-    rc, rb = [x[0] for x in mi], [x[1] for x in mi]
-    if sum(rb) > recv_buf.numel() or sum(sb) > send_buf.numel():
-        raise RuntimeError("exchange buffers too small")
-    dist.all_to_all_single(recv_buf[: sum(rb)], send_buf[: sum(sb)], rb, sb)
-    rlens = torch.empty(sum(rc), dtype=torch.int64, device=plan.lens.device)
-    dist.all_to_all_single(rlens, plan.lens.contiguous(), rc, sc)
-    return sum(rc), sum(rb), rlens
 
 
 META_DTYPE = None

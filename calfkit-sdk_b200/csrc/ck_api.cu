@@ -312,8 +312,6 @@ static int group_sort(ck_handle* h, KeyFn keyf, u32 n, int timer) {
 // decode = walk every submitted record; re-emit the ones that are valid but not canonical into the overlay
 // (count -> scan -> write) and walk those again in their canonical spelling
 static int launch_decode(ck_handle* h) {
-    static int mode = -1;
-    if (mode < 0) { const char* e = getenv("CK_WALKER"); mode = (e && !strcmp(e, "global")) ? 2 : 0; }   // development A/B switch
     u32 n = h->n;
     if (!n) return 0;
     ck_view v = view_of(h);
@@ -327,8 +325,7 @@ static int launch_decode(ck_handle* h) {
         h->cur_perm = h->d_g_o2;
         v = view_of(h);
     }
-    if (mode == 2) v.hist_skip = nullptr;                    // A/B walker: no pre-scan, every list walked in place
-    if (mode != 2) {
+    {
         // records of CK_HIST_MIN bytes or more, one warp each: structural pre-scan; message_history listed message by message
         // for the element pass, or (long records that are long for another reason) the whole record walked by the warp.
         // Both kernels exit at once when there are no such records.
@@ -340,8 +337,7 @@ static int launch_decode(ck_handle* h) {
     }
     {
         KTimer t(h, CK_K_WALK);
-        if (mode == 2) CKL(h) ck_walk_global_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(v, n, h->d_cols, n, 0);
-        else CKL(h) ck_walk_kernel<<<(n + 127) / 128, 128, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, n, h->d_cols, n, 0);
+        CKL(h) ck_walk_kernel<<<(n + 127) / 128, 128, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, n, h->d_cols, n);
         CUDA_TRY(h, cudaGetLastError());
     }
     {
@@ -1058,16 +1054,6 @@ extern "C" int ck_exchange_plan(ck_handle* h, uint32_t rank, uint32_t world, con
         CUDA_TRY(h, cudaGetLastError());
     }
     if (total && run_scan(h, h->d_x_len32, (u32)total, h->d_x_dst_off, 0, h->d_x_tile, h->d_x_grand)) return 1;
-    return 0;
-}
-
-extern "C" int ck_gather_spans(ck_handle* h, const uint8_t* dev_src, const int64_t* dev_src_off, const int64_t* dev_src_len,
-                               uint32_t n, uint8_t* dev_dst, const int64_t* dev_dst_off) {
-    cudaSetDevice(h->device);
-    KTimer t(h, CK_K_EMIT);
-    if (n) CKL(h) ck_gather_spans_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(dev_src, (const long long*)dev_src_off, (const long long*)dev_src_len, n,
-                                                                     dev_dst, (const long long*)dev_dst_off);
-    CUDA_TRY(h, cudaGetLastError());
     return 0;
 }
 

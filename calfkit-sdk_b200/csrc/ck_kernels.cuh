@@ -100,37 +100,6 @@ struct ck_topic_table {                  // open addressing, power-of-two capaci
 // decode
 // ------------------------------------------------------------------------------------------------
 #define CK_WALK_THREADS 128
-// recursive-descent walker (csrc/ck_walk.cuh), one thread per record.  R = WRd: the record is staged through a
-// per-thread shared-memory window (dynamic shared memory: blockDim.x * CK_WIN_STRIDE bytes); R = GRd: plain
-// global loads (kept for A/B, CK_WALKER=global).
-template <class R>
-__device__ __forceinline__ void ck_walk_one(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, u32 mode) {
-    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (v.perm) i = v.perm[i];                                                                       // bucketed batch: neighbours in a warp are of one size class
-    u32 len; const u8* rec;
-    if (mode == 0) rec = ck_rec_in(v, i, len);                                                       // the submitted spelling
-    else { if (v.ovl_off[i] < 0) return; rec = ck_rec(v, i, len); }                                  // re-walk of canonicalised records
-    uint2 skip = make_uint2(0u, 0u);
-    if (mode == 0 && len >= CK_HIST_MIN && v.hist_skip) skip = v.hist_skip[i];   // written by ck_hist_prescan_kernel for every such record
-    if (skip.x == 0xffffffffu) return;                               // long record, not history-dominated: a whole warp has walked it (ck_walk_long_kernel)
-    WalkOut o; o.base = cols + i; o.stride = stride; o.skip_open = skip.x; o.skip_close = skip.y;
-    u32 status, stop = 0;
-    if (len == 0) status = CK_EMPTY;
-    else {
-        R r; r.init(rec, len);
-        AnyCtx cx;
-        cx.kfill = 0;
-        // a canonicalised record the walker cannot prove stays loud (never happens by construction: hostsim fuzz)
-        status = ck_walk_envelope(r, o, cx, stop) ? CK_OK : (mode ? CK_UNSUPPORTED : CK_NOT_CANONICAL);
-    }
-    o.set(CK_COL_STATUS, status);
-    o.set(CK_COL_ERR, stop);
-    if (mode == 0 && status == CK_NOT_CANONICAL && v.canon_ctl) {      // rare: hand the record to the canonicaliser pass
-        u32 k = atomicAdd(&v.canon_ctl->count, 1u);
-        v.canon_list[k] = i;
-    }
-}
 // 6 blocks of 128 threads per SM: <= 80 registers (at 64 the walker spills about twice as much) and room for the
 // CK_WIN_BYTES = 224 windows.  Measured on H100 against 8 blocks with 160-byte windows: config-2 walk 1.30 -> 1.14 ms
 // (DESIGN.md §7)
@@ -150,10 +119,36 @@ ck_classify_kernel(ck_view v, u32 n, u32* __restrict__ cand) {
     base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
     if (take) cand[base + __popc(m & ((1u << lane) - 1u))] = i;
 }
+// recursive-descent walker (csrc/ck_walk.cuh), one thread per submitted record, read through a per-thread
+// shared-memory window (WRd; dynamic shared memory: blockDim.x * CK_WIN_STRIDE bytes).  Records it cannot prove
+// canonical are listed for the canonicaliser pass.
 __global__ void __launch_bounds__(CK_WALK_THREADS, CK_WALK_MINB)
-ck_walk_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, u32 mode) { ck_walk_one<WRd>(v, n, cols, stride, mode); }
-__global__ void __launch_bounds__(CK_WALK_THREADS, 8)
-ck_walk_global_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, u32 mode) { ck_walk_one<GRd>(v, n, cols, stride, mode); }
+ck_walk_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride) {
+    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (v.perm) i = v.perm[i];                                                                       // bucketed batch: neighbours in a warp are of one size class
+    u32 len; const u8* rec = ck_rec_in(v, i, len);
+    uint2 skip = make_uint2(0u, 0u);
+    if (len >= CK_HIST_MIN && v.hist_skip) {
+        skip = v.hist_skip[i];                                       // written by ck_hist_prescan_kernel for every such record
+        if (skip.x == 0xffffffffu) return;                           // long record, not history-dominated: a whole warp has walked it (ck_walk_long_kernel)
+    }
+    WalkOut o; o.base = cols + i; o.stride = stride; o.skip_open = skip.x; o.skip_close = skip.y;
+    u32 stop = 0;
+    bool ok = true;
+    if (len) {
+        WRd r; r.init(rec, len);
+        AnyCtx cx;
+        cx.kfill = 0;
+        ok = ck_walk_envelope(r, o, cx, stop);
+    }
+    o.set(CK_COL_STATUS, len == 0 ? CK_EMPTY : ok ? CK_OK : CK_NOT_CANONICAL);
+    o.set(CK_COL_ERR, stop);
+    if (!ok && v.canon_ctl) {      // rare: hand the record to the canonicaliser pass
+        u32 k = atomicAdd(&v.canon_ctl->count, 1u);
+        v.canon_list[k] = i;
+    }
+}
 
 // ------------------------------------------------------------------------------------------------
 // canonicaliser kernels (ck_canon.cuh): one thread per record that the walker left as CK_NOT_CANONICAL.
@@ -513,11 +508,6 @@ ck_xplan_scatter_kernel(const ck_pub* __restrict__ pubs, u32 npubs, const u32* _
     }
 }
 
-// generic span gather (used to pack cross-partition payloads for the NCCL all-to-all): one warp per span
-__global__ void __launch_bounds__(256)
-ck_gather_spans_kernel(const u8* __restrict__ src, const long long* __restrict__ src_off, const long long* __restrict__ src_len,
-                       u32 n, u8* __restrict__ dst, const long long* __restrict__ dst_off);
-
 // ------------------------------------------------------------------------------------------------
 // exclusive scan u32 -> int64 (three small kernels; lengths are tiny next to the payload bytes)
 // ------------------------------------------------------------------------------------------------
@@ -628,16 +618,6 @@ __device__ __forceinline__ void ck_warp_copy(u8* __restrict__ dst, const u8* __r
     }
     u32 done = nvec << 4, tail = len - done;
     if (lane < tail) dst[done + lane] = src[done + lane];
-}
-
-__global__ void __launch_bounds__(256)
-ck_gather_spans_kernel(const u8* __restrict__ src, const long long* __restrict__ src_off, const long long* __restrict__ src_len,
-                       u32 n, u8* __restrict__ dst, const long long* __restrict__ dst_off) {
-    u32 warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= n) return;
-    long long len = src_len[warp];
-    if (len <= 0) return;
-    ck_warp_copy(dst + dst_off[warp], src + src_off[warp], (u32)len, lane);
 }
 
 // ------------------------------------------------------------------------------------------------

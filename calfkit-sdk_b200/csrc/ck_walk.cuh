@@ -200,9 +200,6 @@ struct URd : GRd {
 #define CK_WIN_BYTES 224
 #endif
 #define CK_WIN_BACK 16
-#ifndef CK_WIN_L2PF
-#define CK_WIN_L2PF 0
-#endif
 #define CK_WIN_STRIDE (CK_WIN_BYTES + 16)     // per-thread slot; the pad spreads the slots over the banks
 #define CK_WIN_NONE 0x80000000u     // o = ap - wbase is then >= 2^31 for every position: always refills
 #if defined(__CUDA_ARCH__)
@@ -222,12 +219,6 @@ CK_HD_NOINLINE u32 ck_win_refill(const u8* gb, u32 ap, u32 lim) {
 #pragma unroll
     for (u32 k = 0; k < CK_WIN_BYTES; k += 16)
         if (wb + k < lim) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(dst + k), "l"(src + k) : "memory");
-#if CK_WIN_L2PF
-    // the NEXT window's lines start their trip from HBM to L2 now: the refill that needs them (one window of parsing
-    // later) then waits for an L2 hit instead of a DRAM access
-    if (wb + CK_WIN_BYTES < lim) asm volatile("prefetch.global.L2 [%0];" :: "l"(src + CK_WIN_BYTES));
-    if (wb + CK_WIN_BYTES + 128u < lim) asm volatile("prefetch.global.L2 [%0];" :: "l"(src + CK_WIN_BYTES + 128u));
-#endif
     asm volatile("cp.async.wait_all;" ::: "memory");
 #else
     for (u32 k = 0; k < CK_WIN_BYTES; k += 16) if (wb + k < lim) for (u32 j = 0; j < 16; j++) ck_win_host[k + j] = gb[wb + k + j];
@@ -303,32 +294,6 @@ struct WRd {
 struct WRdT : WRd { static const bool kTrustFloats = true; };
 struct GRdT : GRd { static const bool kTrustFloats = true; };
 
-// Look-ahead prefetch of the record stream into L1 (experiment knob, off by default): every lane walks its
-// own record, so almost every warp-level load has some lane missing L1; pulling the line CK_PF_DIST
-// bytes ahead turns those into hits.  CK_PF: 0 off, 1 once per 128 B line (entry lands in its first
-// 32 B), 2 unconditional, 4 = 1 with a dummy load instead of prefetch.global.L1.
-#ifndef CK_PF
-#define CK_PF 0
-#endif
-#ifndef CK_PF_DIST
-#define CK_PF_DIST 256
-#endif
-CK_HD void ck_pf(const u8* a) {
-#if defined(__CUDA_ARCH__) && CK_PF
-#if CK_PF == 2
-    asm volatile("prefetch.global.L1 [%0];" :: "l"(a + CK_PF_DIST));
-#elif CK_PF == 4
-    if (((uintptr_t)a & 127) < 32) { unsigned d; asm volatile("ld.global.ca.u32 %0, [%1];" : "=r"(d) : "l"((const void*)((uintptr_t)(a + CK_PF_DIST) & ~(uintptr_t)3))); }
-#elif CK_PF == 3
-    if (((uintptr_t)a & 31) < 16) asm volatile("prefetch.global.L1 [%0];" :: "l"(a + CK_PF_DIST));
-#else
-    if (((uintptr_t)a & 127) < 32) asm volatile("prefetch.global.L1 [%0];" :: "l"(a + CK_PF_DIST));
-#endif
-#else
-    (void)a;
-#endif
-}
-
 #define CK_REP8(b) ((u64)(b) * 0x0101010101010101ull)
 
 // 0x80 in every byte of x that is zero; false positives only ABOVE a true hit (callers use ctz)
@@ -357,7 +322,6 @@ CK_HD u32 ck_ctz64(u64 x) {
 template <class R>
 CK_HD_NOINLINE u32 ck_match8_core(const u8* g, u32 n, u32 pos, u32 st, u64 want, u32 nb) {
     R r; r.init(g, n, st);
-    ck_pf(g + pos);
     u64 got = r.load8(pos);
     u64 mask = ~0ull >> (8 * (8 - nb));
     return (r.st() & ~1u) | (u32)(((got ^ want) & mask) == 0);
@@ -365,7 +329,6 @@ CK_HD_NOINLINE u32 ck_match8_core(const u8* g, u32 n, u32 pos, u32 st, u64 want,
 template <class R>
 CK_HD_NOINLINE u32 ck_match16_core(const u8* g, u32 n, u32 pos, u32 st, u64 want0, u64 want1, u32 nb1) {
     R r; r.init(g, n, st);
-    ck_pf(g + pos);
     u64 g0, g1;
     r.load16(pos, g0, g1);
     u64 mask1 = ~0ull >> (8 * (8 - nb1));
@@ -378,20 +341,10 @@ CK_HD u64 ck_lit_word(const char* lit, u32 L, u32 k) {      // bytes [k, k+8) of
     return w;
 }
 CK_HD u32 ck_lit_nb(u32 L, u32 k) { return (L - k >= 8) ? 8u : (L - k); }      // valid bytes of the word at k
-// Speculative fused literals: pydantic emits every optional field, and in practice most of them are `null`, so
-// long runs of `"key":null` pairs are tried as ONE literal first; a miss costs one 16-byte compare and falls back to
-// the field-by-field path, which accepts exactly the same bytes (the fused literal is one of its spellings).
-#ifndef CK_SPEC
-#define CK_SPEC 1
-#endif
-#ifndef CK_MATCH_INLINE
-#define CK_MATCH_INLINE 1
-#endif
 template <class R>
 CK_HD bool ck_match(R& r, u32& pos, const char* lit, u32 L) {
     if (pos + L > r.n) return false;
     u32 k = 0;
-#if CK_MATCH_INLINE
     if (R::kWindow) {          // shared-memory reads are short enough to inline: no call, no parameter traffic
 #pragma unroll
         for (; k + 8 < L; k += 16) {
@@ -403,7 +356,6 @@ CK_HD bool ck_match(R& r, u32& pos, const char* lit, u32 L) {
         pos += L;
         return true;
     }
-#endif
 #pragma unroll
     for (; k + 8 < L; k += 16) {
         u32 s = ck_match16_core<R>(r.g, r.n, pos + k, r.st(), ck_lit_word(lit, L, k), ck_lit_word(lit, L, k + 8), ck_lit_nb(L, k + 8));
@@ -420,6 +372,9 @@ CK_HD bool ck_match(R& r, u32& pos, const char* lit, u32 L) {
 }
 #define M(lit) ck_match(r, pos, lit, (u32)(sizeof(lit) - 1))
 #define PEEK(c) (pos < r.n && r.at(pos) == (u8)(c))
+// Speculative fused literals: pydantic emits every optional field, and in practice most of them are `null`, so
+// long runs of `"key":null` pairs are tried as ONE literal first; a miss costs one 16-byte compare and falls back to
+// the field-by-field path, which accepts exactly the same bytes (the fused literal is one of its spellings).
 
 // -------------------------------------------------------------------------------------------------
 // Strings.  pos is AT the opening quote; on success pos is just after the closing quote and
@@ -454,16 +409,10 @@ template <class R>
 CK_HD_NOINLINE u64 ck_string_core(const u8* g, u32 n, u32 pos, u32 st) {
     R r; r.init(g, n, st);
     if (!(pos < r.n) || r.at(pos) != '"') return 0;
-    ck_pf(g + pos);
     pos++;
     for (;;) {
         if (pos >= r.n) return false;
         u64 x = r.load8(pos);
-#if CK_PF == 2 || CK_PF == 3
-        if (((uintptr_t)(g + pos) & 31) < 8) ck_pf((const u8*)((uintptr_t)(g + pos) & ~(uintptr_t)31));
-#elif CK_PF
-        if (((uintptr_t)(g + pos) & 127) < 8) ck_pf((const u8*)((uintptr_t)(g + pos) & ~(uintptr_t)127));
-#endif
         u64 special = (x & CK_REP8(0x80)) | ck_haszero(x ^ CK_REP8('"')) | ck_haszero(x ^ CK_REP8('\\')) | ck_lt20(x);
         if (special == 0) { pos += 8; continue; }
         u32 bi = ck_ctz64(special) >> 3;
@@ -644,18 +593,11 @@ struct AnyCtx {
     u32 kfill;
 };
 
-#ifndef CK_HASH8
-#define CK_HASH8 1
-#endif
 // hash of a key span, eight bytes a step (equal spans -> equal hashes is all the duplicate checks and the key tables
 // need; every hit is confirmed by a byte compare or sends the record to the canonicaliser)
 template <class R>
 CK_HD u32 ck_hash_span(R& r, u32 off, u32 len) {
     u32 h = 2166136261u ^ len;
-#if !CK_HASH8
-    for (u32 b = 0; b < len; b++) h = (h ^ r.at(off + b)) * 16777619u;
-    return h;
-#endif
     u32 i = 0;
     for (; i + 8 <= len; i += 8) {
         u64 w = r.load8(off + i);
@@ -828,9 +770,7 @@ CK_HD u32 ck_tool_call_part(R& r, u32& pos, u32 d, AnyCtx& cx, ToolCallSpans& o)
     else if (!ck_any_obj_or_null(r, pos, d + 1, cx)) return 0;
     o.args.len = pos - o.args.off;
     if (!M(",\"tool_call_id\":") || !ck_string(r, pos, o.tool_call_id)) return 0;
-#if CK_SPEC
     if (M(",\"id\":null,\"provider_name\":null,\"provider_details\":null,\"part_kind\":\"tool-call\"}")) return 1;
-#endif
     if (!M(",\"id\":") || !ck_string_or_null(r, pos, t) ||
         !M(",\"provider_name\":") || !ck_string_or_null(r, pos, t) || !M(",\"provider_details\":") ||
         !ck_any_obj_or_null(r, pos, d + 1, cx) || !M(",\"part_kind\":\"")) return 0;
@@ -864,9 +804,7 @@ CK_HD u32 ck_message_part(R& r, u32& pos, u32 d, AnyCtx& cx) {
                     !M(",\"part_kind\":\"system-prompt\"}")) return 0;
                 return 1;
             }
-#if CK_SPEC
             if (M(",\"name\":null,\"part_kind\":\"user-prompt\"}")) return 1;
-#endif
             if (!M(",\"name\":") || !ck_string_or_null(r, pos, t) || !M(",\"part_kind\":\"user-prompt\"}")) return 0;
             return 1;
         }
@@ -973,9 +911,7 @@ CK_HD_NOINLINE u64 ck_message_core(const u8* g, u32 n, u32 pos, u32 st, u32 d, A
     if (M(",\"timestamp\":")) {
         if (seen & 2) return 0;
         if (!ck_datetime_or_null(r, pos)) return 0;
-#if CK_SPEC
         if (M(",\"instructions\":null,\"kind\":\"request\",\"run_id\":null,\"metadata\":null}")) return CK_RET(pos | (1u << 30));
-#endif
         if (!M(",\"instructions\":") || !ck_string_or_null(r, pos, t) ||
             !M(",\"kind\":\"request\",\"run_id\":") || !ck_string_or_null(r, pos, t) || !M(",\"metadata\":") ||
             !ck_any_obj_or_null(r, pos, d + 1, cx) || !M("}")) return 0;
@@ -1343,7 +1279,6 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     if (!M("}")) FAIL;
     SETSPAN(CK_COL_TC_OFF, a, pos);
 
-#if CK_SPEC
     bool spec_tr = M(",\"tool_results\":{},\"uncommitted_message\":null,\"message_history\":[");
     if (spec_tr) {
         // ,"tool_results":{}  ,"uncommitted_message":null  ,"message_history":[      (lengths 18 / 27 / 20)
@@ -1351,7 +1286,6 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
         o.set(CK_COL_TR_OFF, e - 20 - 27 - 2); o.set(CK_COL_TR_LEN, 2);
         o.set(CK_COL_UNC_OFF, e - 20 - 4); o.set(CK_COL_UNC_LEN, 4);
     } else {
-#endif
     if (!M(",\"tool_results\":{")) FAIL;
     a = pos - 1;
     if (!PEEK('}')) {
@@ -1409,9 +1343,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     SETSPAN(CK_COL_UNC_OFF, a, pos);
 
     if (!M(",\"message_history\":[")) FAIL;
-#if CK_SPEC
     }
-#endif
     a = pos - 1;
     if (o.skip_close && o.skip_open == a) pos = o.skip_close;      // the messages are validated one thread each, batch-wide
     else if (!PEEK(']')) {
@@ -1466,7 +1398,6 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     if (!M("]")) FAIL;
     SETSPAN(CK_COL_HIST_OFF, a, pos);
 
-#if CK_SPEC
     if (M(",\"final_output_parts\":[],\"temp_instructions\":null,\"metadata\":null,\"overrides\":null},\"deps\":{\"correlation_id\":")) {
         // ,"final_output_parts":[]  ,"temp_instructions":null  ,"metadata":null  ,"overrides":null  },"deps":{"correlation_id":
         //  lengths                24                        25               16                17                          27
@@ -1477,7 +1408,6 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
         o.set(CK_COL_SMETA_OFF, e - 27 - 17 - 4); o.set(CK_COL_SMETA_LEN, 4);
         o.set(CK_COL_SOV_OFF, e - 27 - 4); o.set(CK_COL_SOV_LEN, 4);
     } else {
-#endif
     if (!M(",\"final_output_parts\":[")) FAIL;
     a = pos - 1;
     Span odata = {0, 0}, otext = {0, 0};
@@ -1514,9 +1444,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
 
     // ---- context.deps ----------------------------------------------------------------------
     if (!M("},\"deps\":{\"correlation_id\":")) FAIL;
-#if CK_SPEC
     }
-#endif
     if (!ck_string(r, pos, t)) FAIL;
     o.set(CK_COL_CORR_OFF, t.off); o.set(CK_COL_CORR_LEN, t.len);
     if (!M(",\"provided_deps\":")) FAIL;
@@ -1538,9 +1466,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
             if (!M("{\"target_topic\":") || !ck_string(r, pos, tgt) || !M(",\"callback_topic\":") || !ck_string(r, pos, cb)) FAIL;
             u32 nargs = CK_NARGS_NULL, kinds = 0;
             Span a0 = {0, 0}, a1 = {0, 0};
-#if CK_SPEC
             if (!M(",\"input_args\":null,\"frame_id\":")) {
-#endif
             if (!M(",\"input_args\":")) FAIL;
             if (PEEK('n')) { if (!ck_null(r, pos)) FAIL; }
             else {
@@ -1563,14 +1489,10 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
                 if (!M("]")) FAIL;
             }
             if (!M(",\"frame_id\":")) FAIL;
-#if CK_SPEC
             }
-#endif
             if (!ck_string(r, pos, t)) FAIL;
             u32 ov0, ov1;
-#if CK_SPEC
             if (M(",\"overrides\":null}")) { ov1 = pos - 1; ov0 = ov1 - 4; } else
-#endif
             {
                 if (!M(",\"overrides\":")) FAIL;
                 ov0 = pos;
@@ -1592,14 +1514,12 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     o.set(CK_COL_ARG0_OFF, top_a0.off); o.set(CK_COL_ARG0_LEN, top_a0.len);
     o.set(CK_COL_ARG1_OFF, top_a1.off); o.set(CK_COL_ARG1_LEN, top_a1.len);
     SETSPAN(CK_COL_FOV_OFF, fov0, fov1);
-#if CK_SPEC
     if (M("]},\"metadata\":null}}")) {             // ]  },"metadata":  null  }}     (lengths 1 / 13 / 4 / 2)
         u32 e = pos;
         o.set(CK_COL_FRAMES_OFF, a); o.set(CK_COL_FRAMES_LEN, e - 19 - a);
         o.set(CK_COL_NFRAMES, nframes);
         o.set(CK_COL_WFMETA_OFF, e - 6); o.set(CK_COL_WFMETA_LEN, 4);
     } else {
-#endif
     if (!M("]")) FAIL;
     SETSPAN(CK_COL_FRAMES_OFF, a, pos);
     o.set(CK_COL_NFRAMES, nframes);
@@ -1608,9 +1528,7 @@ CK_HD bool ck_walk_envelope(R& r, WalkOut& o, AnyCtx& cx, u32& stop) {
     if (!ck_any(r, pos, 3, cx)) FAIL;
     SETSPAN(CK_COL_WFMETA_OFF, a, pos);
     if (!M("}}")) FAIL;
-#if CK_SPEC
     }
-#endif
     if (pos != r.n) FAIL;                 // trailing bytes (even whitespace) are not a fixed point
     // resolve tool_calls[input_args[0]] and tool_results[input_args[0]] (what ToolNodeDef.run looks up,
     // reference nodes/tool.py:45, models/state.py:78-79) from the recorded key spans

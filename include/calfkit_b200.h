@@ -180,10 +180,6 @@ int  ck_fetch_received_async(ck_handle* h, uint32_t src, uint64_t count, uint64_
 int  ck_exchange_plan(ck_handle* h, uint32_t rank, uint32_t world, const int64_t** dev_src_off, const int64_t** dev_len,
                       const int64_t** dev_dst_off, const uint32_t** dev_pub, int64_t* host_counts, int64_t* host_nbytes,
                       uint32_t* n_sel);
-/* copy n spans src[src_off[i] .. +src_len[i]) -> dst[dst_off[i] ..) on the handle's stream (device pointers);
- * used to pack cross-partition payloads before the NCCL all-to-all */
-int  ck_gather_spans(ck_handle* h, const uint8_t* dev_src, const int64_t* dev_src_off, const int64_t* dev_src_len,
-                     uint32_t n, uint8_t* dev_dst, const int64_t* dev_dst_off);
 
 /* results ---------------------------------------------------------------------------------------- */
 int  ck_sync(ck_handle* h);

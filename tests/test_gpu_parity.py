@@ -530,9 +530,9 @@ def test_element_list_overflow_falls_back_to_the_warp_walk():
 
 
 def test_exchange_plan_kernels_match_tensor_plan(engine):
-    """ck_exchange_plan (histogram -> scan -> stable scatter -> scan) against the device-agnostic tensor plan that
-    the world-size-2 gloo test covers (calfkit/engine/exchange.py), on a real publish table, for every rank of
-    several world sizes."""
+    """ck_exchange_plan (histogram -> scan -> stable scatter -> scan) against the device-agnostic tensor plan
+    (calfkit/engine/exchange.py, checked against a plain loop in test_exchange_plan.py), on a real publish table,
+    for every rank of several world sizes.  The same ck_xplan_* kernels plan ck_exchange_send."""
     import torch
     from calfkit import synth
     from calfkit.engine._lib import PUB_DTYPE
