@@ -15,6 +15,13 @@ Two granularities share the topics:
     splits it per topic with vectorised index selections — no Python object per record.  `poll_arena` hands a consumer the
     next batch for its topics, bounded by records AND bytes (a batch never exceeds what an engine was sized for), zero-copy
     when the entry is contiguous.
+Kafka's own granularity — record batches — at both ends:
+  * `produce_fetch(topic, buf)` enqueues a fetch response's record set (engine.lane.FetchArena); `poll_arena` splits such
+    entries only at frame boundaries and the device checks, splits and decodes them;
+  * `frame_sink(topic, fn)`: `fn(topic, partition_or_None, frame, n_records)` once per produce-ready RecordBatch v2 frame.
+    A lane's frames are handed out as they are; per-record Records produced to such a topic are collected and framed by
+    the engine's record form at `flush_frames` (the Worker calls it once per step and installs the `framer`).  There is no
+    CPU encoder: without a framer, flushing them fails loudly.
 Publishes to topics nobody subscribes to are counted and dropped when they arrive batch-wise (a long-running worker must
 not grow without bound); per-record publishes are kept (tests read such topics afterwards).
 Limitation (documented, not hidden): one shared queue per topic — consumer GROUPS are not modelled (two subscriptions to
@@ -26,6 +33,8 @@ import asyncio
 from collections import defaultdict, deque
 from dataclasses import dataclass
 from typing import Any, Awaitable, Callable
+
+import numpy as np
 
 
 @dataclass
@@ -69,6 +78,9 @@ class MemoryBroker:
         self.arenas: dict[str, deque] = defaultdict(deque)            # topic -> deque[Arena]
         self.frags: dict[str, deque] = defaultdict(deque)             # topic -> deque[(PublishBatch, pub indices)]
         self.sinks: dict[str, Any] = {}                               # topic -> callable(PublishBatch, pub indices)
+        self.frame_sinks: dict[str, Any] = {}                         # topic -> callable(topic, partition | None, frame, n_records)
+        self.framer: Callable[[str, list[Record]], Any] | None = None  # records -> engine Frames (the Worker installs it)
+        self._frame_pending: dict[str, list[Record]] = defaultdict(list)
         self.subscriptions: list[Subscription] = []
         self.subscribed: set[str] = set()
         self.produced: int = 0
@@ -85,6 +97,12 @@ class MemoryBroker:
         """bulk consumer of one topic: fn(batch, pub_indices) is called from produce_publishes with the lane's batch (a
         Kafka producer would encode record batches from it; benchmarks count bytes).  The batch is valid during the call."""
         self.sinks[topic] = fn
+
+    def frame_sink(self, topic: str, fn) -> None:
+        """Kafka-shaped consumer of one topic: fn(topic, partition or None, frame, n_records) is called once per
+        RecordBatch v2 frame built on the device (partition None: unkeyed records, the producer client picks one).  The
+        frame (uint8 array) is valid during the call, like `sink`'s batch."""
+        self.frame_sinks[topic] = fn
 
     def publisher(self, topic: str, **kwargs: Any):
         def attach(ref: _HandlerRef):
@@ -109,12 +127,41 @@ class MemoryBroker:
         self.produce(Record(topic, value, key, correlation_id))
 
     def produce(self, rec: Record) -> None:
-        self.queues[rec.topic].append(rec)
+        if rec.topic in self.frame_sinks:                 # framed with the others of this step (flush_frames), never queued
+            self._frame_pending[rec.topic].append(rec)
+        else:
+            self.queues[rec.topic].append(rec)
         self.produced += 1
+
+    def flush_frames(self) -> None:
+        """frame the per-record Records collected for frame-sink topics (engine record form) and hand the frames out"""
+        for topic in list(self._frame_pending):
+            recs = self._frame_pending.pop(topic)
+            if not recs:
+                continue
+            if self.framer is None:
+                from calfkit.exceptions import EngineError
+                raise EngineError(f"{len(recs)} records for frame-sink topic {topic!r} and no engine to frame them (Worker installs one)")
+            for frames in self.framer(topic, recs):
+                try:
+                    self._hand_frames(frames)
+                finally:
+                    frames.release()
+
+    def _hand_frames(self, frames) -> None:
+        for topic, part, frame, n in frames:
+            self.frame_sinks[topic](topic, part, frame, n)
 
     def produce_batch(self, records: list[Record]) -> None:
         for r in records:
             self.produce(r)
+
+    def produce_fetch(self, topic: str, buf) -> None:
+        """a fetch response's record set for one topic (bytes, a uint8 array or an engine.lane.FetchArena)"""
+        from calfkit.engine.lane import FetchArena
+        fa = buf if isinstance(buf, FetchArena) else FetchArena.of(buf)
+        self.arenas[topic].append(fa)
+        self.produced += fa.n
 
     def produce_arena(self, topic: str, arena) -> None:
         """a whole batch of records for one topic (engine.lane.Arena)"""
@@ -122,9 +169,16 @@ class MemoryBroker:
         self.produced += arena.n
 
     def produce_publishes(self, batch) -> None:
-        """split what a GPU lane produced (engine.lane.PublishBatch) over the topics, by index selection"""
+        """split what a GPU lane produced (engine.lane.PublishBatch) over the topics, by index selection; the topics the lane
+        framed go to their frame sinks as frames"""
+        framed = set()
+        if batch.frames is not None:
+            framed = {batch.topic_names[i] for i in batch.frame_topic_ids}
+            self._hand_frames(batch.frames)
         for tid, cnt in batch.topic_counts().items():
             self.produced += cnt
+            if tid >= 0 and batch.topic_names.get(tid) in framed:
+                continue
             if tid < 0 and batch.source is None:
                 # forwarded by another rank without a registered topic id: the name stayed with the source record there.
                 # Workers of one deployment register each other's topics (Worker(route_topics=...)): loud, not silent
@@ -135,7 +189,6 @@ class MemoryBroker:
             if tid < 0:
                 # topics the engine has no id for (another worker's node, a client's private reply topic): the kernel left
                 # the FNV-1a of the name in `pad`, so they are grouped vectorised and the name is decoded once per group
-                import numpy as np
                 idx = batch.select(-1)
                 hashes = np.ascontiguousarray(batch.pubs["pad"][idx])
                 for hv in np.unique(hashes):
@@ -151,7 +204,10 @@ class MemoryBroker:
         batch.release()
 
     def _route(self, batch, name: str, idx) -> None:
-        if name in self.sinks:
+        if name in self.frame_sinks:                       # publishes the lane did not frame: the record form frames them
+            for topic, key, payload, _j in batch.iter_records(idx):
+                self._frame_pending[topic].append(Record(topic, payload, key, key.decode() if key is not None else None))
+        elif name in self.sinks:
             self.sinks[name](batch, idx)
         elif name in self.subscribed:
             self.frags[name].append((batch.retain(), idx))
@@ -170,6 +226,9 @@ class MemoryBroker:
                     return out
                 nbytes += len(q[0].value)
                 out.append(q.popleft())
+            if self.arenas.get(t) and type(self.arenas[t][0]).__name__ == "FetchArena":
+                from calfkit.exceptions import EngineError
+                raise EngineError(f"topic {t!r} holds fetch responses: they are decoded on the device by a device-template node")
             if len(out) < max_records and (self.arenas.get(t) or self.frags.get(t)):
                 arena = self.poll_arena((t,), max_records - len(out), None if max_bytes is None else max(max_bytes - nbytes, 1),
                                         records_too=False)
@@ -186,6 +245,24 @@ class MemoryBroker:
         from calfkit.engine.lane import Arena
         for t in topics:
             q = self.arenas.get(t)
+            from calfkit.engine.lane import FetchArena
+            while q and isinstance(q[0], FetchArena) and len(q[0].frames()[1]) == 0:
+                q.popleft().release()                       # nothing but a truncated frame: no record in it
+            if q and isinstance(q[0], FetchArena):
+                # split only at frame boundaries, at least one frame (an oversized frame alone: the engine reports it)
+                a = q[0]
+                starts, counts = a.frames()
+                cum_rec, cum_bytes = np.cumsum(counts), starts[1:] - starts[0]
+                fits = cum_rec <= max_records
+                if max_bytes is not None:
+                    fits &= cum_bytes <= max_bytes
+                k = max(int(np.argmin(fits)) if not fits.all() else len(counts), 1)
+                if k >= len(counts):
+                    return q.popleft()                      # the truncated tail (if any) goes along and is ignored
+                head, rest = a.slice_frames(0, k), a.slice_frames(k, None)
+                rest._on_release, a._on_release = a._on_release, None
+                q[0] = rest
+                return head
             if q:
                 a = q[0]
                 k = _fit(a.offsets, max_records, max_bytes)
@@ -200,7 +277,6 @@ class MemoryBroker:
             if f:
                 batch, idx = f[0]
                 lens = batch.out_len[batch.pubs["payload"][idx]].astype("int64")
-                import numpy as np
                 k = _fit(np.concatenate(([0], np.cumsum(lens))), max_records, max_bytes)
                 arena = batch.gather(idx[:k])        # a zero-copy view retains the batch until the arena is released
                 if k >= len(idx):
@@ -215,7 +291,7 @@ class MemoryBroker:
         return None
 
     def pending(self) -> int:
-        return (sum(len(q) for q in self.queues.values()) + sum(a.n for q in self.arenas.values() for a in q)
+        return (sum(len(q) for q in self.queues.values()) + sum(len(r) for r in self._frame_pending.values()) + sum(a.n for q in self.arenas.values() for a in q)
                 + sum(len(i) for q in self.frags.values() for _b, i in q))
 
 
@@ -226,7 +302,6 @@ def _fit(offsets, max_records: int, max_bytes: int | None) -> int:
     if n and (max_bytes is None or int(offsets[k] - offsets[0]) <= max_bytes):
         return k                                            # the common case: no array work at all
     if max_bytes is not None and n:
-        import numpy as np
         k = min(k, int(np.searchsorted(offsets - offsets[0], max_bytes, side="right")) - 1)
     return max(k, 1) if n else 0
 

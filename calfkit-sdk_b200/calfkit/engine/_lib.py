@@ -30,11 +30,13 @@ COLS = ["STATUS", "ACTION", "ERR", "CORR_OFF", "CORR_LEN", "NFRAMES", "FRAMES_OF
 COL = {name: i for i, name in enumerate(COLS)}
 NUM_COLS = len(COLS)
 
-KERNELS = ["walk", "plan", "scan", "emit", "route", "fanout", "canon", "walk_long", "walk_elems"]
+KERNELS = ["walk", "plan", "scan", "emit", "route", "fanout", "canon", "walk_long", "walk_elems", "frame"]
 NUM_KERNELS = len(KERNELS)
 
 PUB_DTYPE = np.dtype([("payload", "<u4"), ("topic_id", "<i4"), ("topic_off", "<u4"), ("topic_len", "<u4"),
                       ("record", "<u4"), ("has_key", "<u4"), ("partition", "<i4"), ("pad", "<u4")])
+FRAME_DTYPE = np.dtype([("topic_id", "<i4"), ("partition", "<i4"), ("n_records", "<u4"), ("first", "<u4"), ("offset", "<i8"),
+                        ("length", "<i8")])
 
 EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_register_topics", "ck_set_tool_node", "ck_submit",
            "ck_submit_device", "ck_tool_args", "ck_tool_plan", "ck_tool_plan_device", "ck_return_plan", "ck_set_agent_node", "ck_set_agent_tool_topic_ids", "ck_fanout_plan", "ck_tailcall_plan", "ck_exchange_plan", "ck_launch_count", "ck_reply_plan",
@@ -42,7 +44,9 @@ EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_registe
            "ck_device_buffers", "ck_device_buffers2", "ck_profile", "ck_profile_read", "ck_fetch_cols",
            "ck_host_alloc", "ck_host_free", "ck_canon_stats", "ck_fetch_output_async",
            "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_reset", "ck_submit_recordbatch",
-           "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option"]
+           "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option",
+           "ck_set_frame_topics", "ck_encode_frames", "ck_encode_frames_records", "ck_frames_size", "ck_fetch_frames_async",
+           "ck_fetch_rb_index_async"]
 
 _lib = None
 
@@ -102,7 +106,13 @@ def load() -> C.CDLL:
         "ck_fetch_groups": (C.c_int, [vp, u32p, u32p, C.c_int]),
         "ck_submit_recordbatch": (C.c_int, [vp, u8p, C.c_uint64, C.POINTER(C.c_uint32)]),
         "ck_fetch_rb_index": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
+        "ck_fetch_rb_index_async": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
         "ck_encode_recordbatch": (C.c_int, [vp, u32p, C.c_uint32, C.c_int64, C.c_int64, u8p, C.c_uint64, C.POINTER(C.c_uint64)]),
+        "ck_set_frame_topics": (C.c_int, [vp, i32p, C.c_uint32]),
+        "ck_encode_frames": (C.c_int, [vp, C.c_int64]),
+        "ck_encode_frames_records": (C.c_int, [vp, C.c_int32, u8p, C.c_uint64, i64p, C.c_uint32, C.c_int64]),
+        "ck_frames_size": (C.c_int, [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
+        "ck_fetch_frames_async": (C.c_int, [vp, vp, C.c_uint32, u8p, C.c_uint64]),
         "ck_gate_create": (C.c_int, [vp, C.c_uint32, C.c_uint32, C.c_uint64]),
         "ck_gate_register": (C.c_int, [vp, C.c_uint32]),
         "ck_gate_arrive": (C.c_int, [vp, C.c_uint64]),

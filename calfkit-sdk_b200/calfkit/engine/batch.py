@@ -18,7 +18,7 @@ from typing import Iterator, Sequence
 import numpy as np
 
 from calfkit.engine import _lib
-from calfkit.engine._lib import COL, NUM_COLS, PUB_DTYPE, ptr
+from calfkit.engine._lib import COL, FRAME_DTYPE, NUM_COLS, PUB_DTYPE, ptr
 from calfkit.exceptions import EngineError
 
 
@@ -119,6 +119,38 @@ class BatchOutput:
                           int(p["partition"]))
 
 
+class Frames:
+    """Kafka RecordBatch v2 frames of one frame pass, produce-ready: `table` (FRAME_DTYPE: topic id, partition, records,
+    first record, offset, length) and the frame bytes back to back in `data`.  Partition -1 holds unkeyed records: the
+    producer client picks their partition."""
+
+    def __init__(self, table: np.ndarray, data: np.ndarray, topic_names: dict[int, str], on_release=None):
+        self.table, self.data, self.topic_names, self._on_release = table, data, topic_names, on_release
+
+    def release(self) -> None:
+        if self._on_release is not None:
+            cb, self._on_release = self._on_release, None
+            cb()
+
+    def __len__(self) -> int:
+        return len(self.table)
+
+    def frame(self, i: int) -> np.ndarray:
+        o = int(self.table["offset"][i])
+        return self.data[o:o + int(self.table["length"][i])]
+
+    def __iter__(self) -> Iterator[tuple[str, int | None, np.ndarray, int]]:
+        """(topic, partition or None, frame bytes, records) per frame"""
+        for i, e in enumerate(self.table):
+            p = int(e["partition"])
+            yield self.topic_names[int(e["topic_id"])], (p if p >= 0 else None), self.frame(i), int(e["n_records"])
+
+
+def json_content(s: str) -> bytes:
+    """a string as the content of a JSON string, the spelling the device unescapes (the envelope's own spelling)"""
+    return json.dumps(s, ensure_ascii=False)[1:-1].encode()
+
+
 _M64 = (1 << 64) - 1
 
 
@@ -177,6 +209,7 @@ class BatchEngine:
         self.num_partitions = 0
         self.n = 0
         self._in_data = self._in_off = None
+        self.frame_topics: list[str] = []
 
     # ------------------------------------------------------------------------------------------
     def close(self) -> None:
@@ -321,6 +354,61 @@ class BatchEngine:
         used = C.c_uint64(0)
         self._check(self.lib.ck_encode_recordbatch(self.h, ptr(idx), len(idx), base_offset, timestamp_ms, ptr(buf), cap, C.byref(used)))
         return buf[:used.value]
+
+    # ---- produce-ready frames: one frame pass per step (csrc/ck_kafka.cuh) -------------------------------------------
+    def set_frame_topics(self, topics: Sequence[str]) -> None:
+        """the registered topics whose publishes encode_frames frames"""
+        missing = [t for t in topics if t not in self.topic_ids]
+        if missing:
+            raise EngineError(f"frame topics not registered: {missing}")
+        ids = np.asarray([self.topic_ids[t] for t in topics] or [0], dtype=np.int32)
+        self._check(self.lib.ck_set_frame_topics(self.h, ptr(ids), len(topics)))
+        self.frame_topics = list(topics)
+
+    def set_frame_bytes(self, window: int) -> None:
+        """the frame split window W: a frame holds at most 61 + W + one record bytes (default 1 MiB)"""
+        self._check(self.lib.ck_set_option(self.h, 2, window))
+
+    def encode_frames(self, timestamp_ms: int) -> None:
+        """queue the frame pass over the current plan: every live publish to a frame topic, grouped by (topic, partition)
+        in send order, as frames with baseOffset 0 and baseTimestamp timestamp_ms (asynchronous; fetch_frames reads them)"""
+        self._check(self.lib.ck_encode_frames(self.h, timestamp_ms))
+
+    def encode_frames_records(self, topic: str, records: Sequence[tuple[bytes, bytes | None, str | None]], timestamp_ms: int) -> None:
+        """queue the frame pass over records a host path produced for `topic`: (value, key or None, correlation id or None)
+        each; keyed records go to partition murmur2(key) % num_partitions, as the plan's publishes do"""
+        if topic not in self.topic_ids:
+            raise EngineError(f"topic {topic!r} is not registered")
+        parts, desc, pos = [], np.full((len(records), 6), -1, dtype=np.int64), 0
+        for i, (value, key, corr) in enumerate(records):
+            for f, b in enumerate((value, None if key is None else json_content(key.decode()), None if corr is None else json_content(corr))):
+                if b is None:
+                    continue
+                desc[i, 2 * f], desc[i, 2 * f + 1] = pos, len(b)
+                parts.append(b)
+                pos += len(b)
+        blob = np.frombuffer(b"".join(parts) or b"\0", dtype=np.uint8)
+        self._frame_src = (blob, desc)                   # the copies to the device read them after this call returns
+        self._check(self.lib.ck_encode_frames_records(self.h, self.topic_ids[topic], ptr(blob), pos, ptr(desc), len(records), timestamp_ms))
+
+    def frames_size(self) -> tuple[int, int]:
+        """(frames, bytes) of the last frame pass; waits for it"""
+        nf, nb = C.c_uint32(), C.c_uint64()
+        self._check(self.lib.ck_frames_size(self.h, C.byref(nf), C.byref(nb)))
+        return nf.value, nb.value
+
+    def fetch_frames(self, pool=None) -> Frames:
+        """the frames of the last frame pass, copied to the host (waits).  With a PinnedPool (engine.lane) they land in
+        page-locked buffers taken from it; Frames.release() gives them back"""
+        nf, nb = self.frames_size()
+        if pool is None:
+            table, data, bufs = np.zeros(nf, dtype=FRAME_DTYPE), np.empty(max(nb, 1), dtype=np.uint8), ()
+        else:
+            bufs = (pool.take(FRAME_DTYPE.itemsize * nf + 64), pool.take(nb + 64))
+            table, data = bufs[0].view(FRAME_DTYPE, nf), bufs[1].array
+        self._check(self.lib.ck_fetch_frames_async(self.h, ptr(table), nf, ptr(data), data.nbytes))
+        self.sync()
+        return Frames(table, data[:nb], self.topic_names, on_release=(lambda: [pool.give(b) for b in bufs]) if bufs else None)
 
     def submit_device(self, dev_data, dev_off, n: int, host_data: np.ndarray | None = None,
                       host_off: np.ndarray | None = None) -> None:

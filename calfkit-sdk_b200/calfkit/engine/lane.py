@@ -6,6 +6,8 @@ goes to HBM with one cudaMemcpyAsync; results come back the same way (payload ar
 table).  No Python object is created per record anywhere on this path.
 
   Arena          inbound batch: pinned uint8 bytes + int64 offsets[n+1]
+  FetchArena     inbound batch as a Kafka fetch response carries it: the record set (RecordBatch v2 frames) in one pinned
+                 buffer; CRC check, record split and field decode run on the device (ck_submit_recordbatch)
   PublishBatch   outbound batch: pinned payload arena + the ck_publish table; resolves topic names / keys lazily,
                  per topic, vectorised
   PinnedPool     recycles page-locked buffers (cudaHostAlloc costs milliseconds; the steady state allocates nothing)
@@ -17,13 +19,14 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import time
 from typing import Callable, Iterator
 
 import numpy as np
 
 from calfkit.engine import _lib
-from calfkit.engine._lib import COL, PUB_DTYPE, ptr
-from calfkit.engine.batch import BatchEngine, ToolTemplate
+from calfkit.engine._lib import COL, FRAME_DTYPE, PUB_DTYPE, ptr
+from calfkit.engine.batch import BatchEngine, Frames, ToolTemplate, _SpanOffsets
 from calfkit.exceptions import EngineError
 
 NO_PAYLOAD = 0xFFFFFFFF
@@ -123,6 +126,74 @@ class Arena:
         return cls(buf.array[:total], offsets, on_release=lambda: pool.give(buf))
 
 
+class FetchArena:
+    """the record set of one fetch response — concatenated RecordBatch v2 frames as they came off the socket — in one
+    buffer.  The host only chains through the 12-byte frame prefixes (baseOffset, batchLength) to count frames and records;
+    a truncated trailing frame (legal in a fetch response) is carried along and ignored by the device"""
+    def __init__(self, data: np.ndarray, on_release: Callable[[], None] | None = None):
+        assert data.dtype == np.uint8
+        self.data, self._on_release, self._index = data, on_release, None
+
+    @classmethod
+    def of(cls, buf, pool: PinnedPool | None = None) -> "FetchArena":
+        """land a fetch response (bytes / uint8 array) in a page-locked buffer"""
+        src = np.frombuffer(bytes(buf), dtype=np.uint8) if not isinstance(buf, np.ndarray) else buf
+        if pool is None:
+            return cls(src)
+        b = pool.take(src.nbytes + 64)
+        b.array[:src.nbytes] = src
+        return cls(b.array[:src.nbytes], on_release=lambda: pool.give(b))
+
+    def frames(self) -> tuple[np.ndarray, np.ndarray]:
+        """(starts[k + 1], records[k]) of the k complete frames; starts[k] is where the truncated tail (if any) begins"""
+        if self._index is None:
+            d, pos, starts, counts = self.data, 0, [0], []
+            while pos + 12 <= d.nbytes:
+                blen = int.from_bytes(d[pos + 8:pos + 12].tobytes(), "big", signed=True)
+                end = pos + 12 + blen
+                if blen < 49 or end > d.nbytes:
+                    break
+                counts.append(int.from_bytes(d[pos + 57:pos + 61].tobytes(), "big"))
+                pos = end
+                starts.append(pos)
+            self._index = (np.asarray(starts, dtype=np.int64), np.asarray(counts, dtype=np.int64))
+        return self._index
+
+    @property
+    def n(self) -> int:
+        return int(self.frames()[1].sum())
+
+    @property
+    def nbytes(self) -> int:
+        return int(self.data.nbytes)
+
+    def slice_frames(self, a: int, b: int | None) -> "FetchArena":
+        """frames [a, b) as a zero-copy view; b None: to the end of the buffer (the truncated tail included)"""
+        starts = self.frames()[0]
+        return FetchArena(self.data[int(starts[a]):(int(starts[b]) if b is not None else self.data.nbytes)])
+
+    def release(self) -> None:
+        if self._on_release is not None:
+            cb, self._on_release = self._on_release, None
+            cb()
+
+
+class FetchRecords:
+    """the records of a submitted FetchArena as the device split them: record i = its value, where it lies in the frame"""
+    def __init__(self, arena: FetchArena, val_off: np.ndarray, val_len: np.ndarray, bad: np.ndarray):
+        self.arena, self.data, self.offsets, self.bad = arena, arena.data, _SpanOffsets(val_off, val_len), bad
+
+    @property
+    def n(self) -> int:
+        return len(self.bad)
+
+    def record(self, i: int) -> bytes:
+        return self.data[int(self.offsets[i]):self.offsets.end(i)].tobytes()
+
+    def release(self) -> None:
+        self.arena.release()
+
+
 class PublishBatch:
     """What one plan + encode produced: unique payloads (16-byte aligned starts in `out`) and the publish table that
     references them (ck_publish: payload index, topic id or topic span, key flag, partition).  Everything is a numpy
@@ -130,7 +201,7 @@ class PublishBatch:
     def __init__(self, out: np.ndarray, out_off: np.ndarray, out_len: np.ndarray, pubs: np.ndarray, topic_names: dict[int, str],
                  source: Arena | None, key_spans: np.ndarray | None, status: np.ndarray | None, action: np.ndarray | None,
                  on_release: Callable[[], None] | None = None, overlay=None, order: np.ndarray | None = None,
-                 key_counts: np.ndarray | None = None):
+                 key_counts: np.ndarray | None = None, frames: Frames | None = None, frame_topic_ids: frozenset = frozenset()):
         self.out, self.out_off, self.out_len, self.pubs, self.topic_names = out, out_off, out_len, pubs, topic_names
         self.source, self.key_spans, self.status, self.action = source, key_spans, status, action
         self.overlay = overlay          # (bytes, off[n], len[n]) canonical re-emissions: column / topic spans of those records refer to them
@@ -138,6 +209,8 @@ class PublishBatch:
         # id, 1 + id = registered topic, 4095 = unused slot), send order kept inside a group; key_counts[4096]
         self.order, self.key_counts = order, key_counts
         self._starts = None if key_counts is None else np.concatenate(([0], np.cumsum(key_counts, dtype=np.int64)))
+        # the frame pass (ck_encode_frames): the publishes to the topics frame_topic_ids as produce-ready frames
+        self.frames, self.frame_topic_ids = frames, frame_topic_ids
         self._on_release = on_release
         self._refs = 1
         self._live = None
@@ -191,7 +264,10 @@ class PublishBatch:
         if self.overlay is not None and self.overlay[1][r] >= 0:
             o = int(self.overlay[1][r])
             return self.overlay[0][o:o + int(self.overlay[2][r])]
-        return self.source.data[int(self.source.offsets[r]):int(self.source.offsets[r + 1])]
+        o = self.source.offsets
+        if isinstance(o, _SpanOffsets):
+            return self.source.data[int(o[r]):o.end(r)]
+        return self.source.data[int(o[r]):int(o[r + 1])]
 
     def key(self, pub_index: int) -> bytes | None:
         """key = correlation_id.encode() for keyed publishes (nodes/base.py:86,103,117,134)"""
@@ -268,11 +344,21 @@ class Lane:
             rank, world = exchange
             self.px = PeerExchange(self.eng, rank, world, max_fwd=max_records, data_cap=max_in_bytes + 64 * max_records)
 
-    def submit(self, arena: Arena) -> None:
-        """device-template tool node: decode + plan + encode + route (+ forward to the owning ranks), all asynchronous"""
+    def submit(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None) -> None:
+        """device-template tool node: decode + plan + encode + route (+ frame pass, + forward to the owning ranks), all
+        asynchronous.  A FetchArena goes to the device as it is (ck_submit_recordbatch).  With frame topics set on the engine,
+        their publishes are framed with baseTimestamp timestamp_ms (default: now)"""
         self.arena, self.busy = arena, True
-        self.eng.submit(arena.data, arena.offsets)
-        self.eng.tool_plan()
+        eng = self.eng
+        if isinstance(arena, FetchArena):
+            n = C.c_uint32(0)
+            eng._check(eng.lib.ck_submit_recordbatch(eng.h, ptr(arena.data), arena.data.nbytes, C.byref(n)))
+            eng.n = n.value
+        else:
+            eng.submit(arena.data, arena.offsets)
+        eng.tool_plan()
+        if eng.frame_topics:
+            eng.encode_frames(int(time.time() * 1000) if timestamp_ms is None else timestamp_ms)
         if self.px is not None:
             self.step_no += 1
             self.px.send(self.step_no)
@@ -300,6 +386,22 @@ class Lane:
             eng._check(eng.lib.ck_fetch_cols_async(eng.h, ptr(_FAST_COLS), 4, ptr(rows)))
         eng._check(eng.lib.ck_fetch_groups(eng.h, ptr(order), ptr(key_counts), 0))
         self._views = (b_out.array[:nb], off, ln, pubs, rows, order, key_counts)
+        # a fetch response: where every record's value lies in it, and whether its frame failed the check
+        self._b_rb = self._rb = None
+        if isinstance(self.arena, FetchArena):
+            self._b_rb = b_rb = pool.take(16 * n + 64)
+            val_off, val_len, bad = b_rb.view(np.int64, n), b_rb.view(np.uint32, n, 8 * n), b_rb.view(np.uint32, n, 12 * n)
+            if n:
+                eng._check(eng.lib.ck_fetch_rb_index_async(eng.h, ptr(val_off), ptr(val_len), None, None, None, None, ptr(bad)))
+            self._rb = (val_off, val_len, bad)
+        # the frame pass's frames and table (the stream was just synchronised for the sizes above)
+        self._b_fr = self._fr = None
+        if eng.frame_topics:
+            nf, fb = eng.frames_size()
+            self._b_fr = (pool.take(fb + 64), pool.take(FRAME_DTYPE.itemsize * nf + 64))
+            data, table = self._b_fr[0].array[:fb], self._b_fr[1].view(FRAME_DTYPE, nf)
+            eng._check(eng.lib.ck_fetch_frames_async(eng.h, ptr(self._b_fr[1].array), nf, ptr(self._b_fr[0].array), self._b_fr[0].nbytes))
+            self._fr = Frames(table, data, eng.topic_names)
         # what the other ranks forwarded to this one during this step: the regions are complete (the stream was just
         # synchronised for the sizes, the exchange's second barrier is behind it); their copies ride along with the results
         self._recv = []
@@ -328,11 +430,17 @@ class Lane:
         out, off, ln, pubs, rows, order, key_counts = self._views
         b_out, b_meta = self._b_out, self._b_meta
         self.d2h_bytes = int(out.nbytes + off.nbytes + ln.nbytes + pubs.nbytes + rows.nbytes + order.nbytes + key_counts.nbytes)
+        frames, b_fr, b_rb = self._fr, self._b_fr, self._b_rb
+        if frames is not None:
+            self.d2h_bytes += int(frames.data.nbytes + frames.table.nbytes)
+        if self._rb is not None:
+            self.d2h_bytes += int(sum(a.nbytes for a in self._rb))
         listed = C.c_uint32(0)
         eng._check(eng.lib.ck_canon_stats(eng.h, C.byref(listed), None))
         overlay = eng.overlay() if listed.value else None       # rare: some records arrived in a non-canonical spelling
         arena, self.arena, self.busy, self.collecting = self.arena, None, False, False
-        self._views = self._b_out = self._b_meta = None
+        source = FetchRecords(arena, *self._rb) if self._rb is not None else arena
+        self._views = self._b_out = self._b_meta = self._b_fr = self._fr = self._b_rb = self._rb = None
         self.received = []
         for meta, data, b_m, b_d in self._recv:
             self.received.append(received_batch(meta, data, eng.topic_names, on_release=lambda b_m=b_m, b_d=b_d: (pool.give(b_m), pool.give(b_d))))
@@ -341,9 +449,12 @@ class Lane:
         def done():
             pool.give(b_out)
             pool.give(b_meta)
+            for b in (b_fr or ()) + ((b_rb,) if b_rb is not None else ()):
+                pool.give(b)
             arena.release()
-        return PublishBatch(out, off, ln, pubs, eng.topic_names, arena, rows[2:4], rows[0], rows[1], on_release=done, overlay=overlay,
-                            order=order, key_counts=key_counts)
+        return PublishBatch(out, off, ln, pubs, eng.topic_names, source, rows[2:4], rows[0], rows[1], on_release=done, overlay=overlay,
+                            order=order, key_counts=key_counts, frames=frames,
+                            frame_topic_ids=frozenset(eng.topic_ids[t] for t in eng.frame_topics))
 
     def collect(self) -> PublishBatch:
         if not self.collecting:
@@ -367,13 +478,13 @@ class LanePipeline:
         self._k = 0
         self._inflight: list[Lane] = []
 
-    def push(self, arena: Arena) -> PublishBatch | None:
+    def push(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None) -> PublishBatch | None:
         """queue one step; returns the results of an older step once the pipe is full.  Order of work per call:
         (1) H2D + kernels of the new step are queued, (2) the copy-back that was started by the previous call is
         awaited and handed out, (3) the copy-back of the next-oldest step is started — it runs while the caller
         produces the batch just returned and while the new step computes."""
         lane = next(l for l in self.lanes if not l.busy)    # invariant: at most K-1 lanes busy between calls
-        lane.submit(arena)
+        lane.submit(arena, timestamp_ms)
         self._inflight.append(lane)
         ready = None
         if self._inflight[0].collecting:
@@ -415,4 +526,4 @@ class LanePipeline:
         self.pool.close()
 
 
-__all__ = ["Arena", "PublishBatch", "PinnedPool", "PinnedBuffer", "Lane", "LanePipeline", "ToolTemplate"]
+__all__ = ["Arena", "FetchArena", "FetchRecords", "PublishBatch", "PinnedPool", "PinnedBuffer", "Lane", "LanePipeline", "ToolTemplate"]

@@ -18,6 +18,7 @@ from __future__ import annotations
 import asyncio
 import logging
 import os
+import time
 from typing import Any
 
 import numpy as np
@@ -26,6 +27,7 @@ from calfkit.broker import Record
 from calfkit.client import Client
 from calfkit.engine import BatchEngine
 from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_UNSUPPORTED, STATUS_NAMES
+from calfkit.exceptions import EngineError
 from calfkit.engine.lane import LanePipeline, PublishBatch
 from calfkit.nodes import BaseNodeDef
 
@@ -91,6 +93,8 @@ class Worker:
         self._rank, self._world = (rank or 0), (world or 1)
         self._subs: list[tuple[BaseNodeDef, Any]] = []
         self._pipes: dict[int, LanePipeline] = {}
+        self._framer_eng: BatchEngine | None = None
+        self._frame_pool = None
         self.stats = {"records": 0, "publishes": 0, "rejected": 0, "raises": 0, "host_fallback": 0, "steps": 0}
 
     def add_nodes(self, *nodes: BaseNodeDef) -> None:
@@ -114,11 +118,15 @@ class Worker:
     def _pipeline(self, node: BaseNodeDef) -> LanePipeline:
         pipe = self._pipes.get(id(node))
         if pipe is None:
-            topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics
+            # frame-sink topics get ids like route_topics, so that their publishes can be framed on the device
+            frame_topics = list(self._client._connection.frame_sinks)
+            topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics + frame_topics
 
             def configure(eng: BatchEngine) -> None:
                 eng.register_topics(topics, num_partitions=getattr(self._client._connection, "num_partitions", 0))
                 node.configure_engine(eng)
+                if frame_topics:
+                    eng.set_frame_topics(frame_topics)
             pipe = LanePipeline(self._device, configure, lanes=self._lanes, max_records=self._batch_records,
                                 max_in_bytes=self._batch_bytes, exchange=(self._rank, self._world) if self._world > 1 else None)
             self._pipes[id(node)] = pipe
@@ -166,11 +174,41 @@ class Worker:
             self._run_host(node, records[:mid], **kw)
             self._run_host(node, records[mid:], **kw)
 
+    def _frame_records(self, topic: str, records: list[Record]):
+        """the engine's record form over Records produced to a frame-sink topic by host paths, in engine-sized chunks"""
+        broker = self._client._connection
+        if self._framer_eng is None:
+            from calfkit.engine.lane import PinnedPool
+            self._framer_eng = BatchEngine(self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes)
+            self._framer_eng.register_topics(list(broker.frame_sinks), num_partitions=getattr(broker, "num_partitions", 0))
+            self._frame_pool = PinnedPool()
+        eng, ts = self._framer_eng, int(time.time() * 1000)
+        if topic not in eng.topic_ids:
+            eng.register_topics(list(eng.topic_ids) + [topic], num_partitions=eng.num_partitions)
+        limit = min(2 * eng.max_payloads, eng.max_records)
+        a = 0
+        while a < len(records):
+            b, nbytes = a, 0
+            while b < len(records) and b - a < limit:
+                r = records[b]
+                size = len(r.value) + 2 * len(r.key or b"") + 2 * len((r.correlation_id or "").encode())
+                if b > a and nbytes + size > eng.max_in:
+                    break
+                nbytes += size
+                b += 1
+            eng.encode_frames_records(topic, [(r.value, r.key, r.correlation_id) for r in records[a:b]], ts)
+            yield eng.fetch_frames(self._frame_pool)
+            a = b
+
     def step(self) -> int:
         """one pass over all nodes: poll -> CUDA batch -> produce.  Returns the number of records consumed."""
         broker = self._client._connection
         consumed = 0
         self.stats["steps"] += 1
+        if broker.frame_sinks:
+            if self._world > 1:
+                raise EngineError("frame sinks need world == 1: publishes forwarded by other ranks are not framed yet")
+            broker.framer = self._frame_records
         for node, sub in self._subs:
             if getattr(node, "_template", None) is not None:
                 pipe = self._pipeline(node)
@@ -179,7 +217,8 @@ class Worker:
                     arena = _EMPTY_ARENA()                     # lockstep: every rank runs the exchange on every tick
                 if arena is not None:
                     consumed += arena.n
-                    done = pipe.push(arena)
+                    # the step's timestamp is the frames' baseTimestamp (only framing lanes use it)
+                    done = pipe.push(arena, int(time.time() * 1000)) if broker.frame_sinks else pipe.push(arena)
                     if done is not None:
                         self._produce_fast(node, done)
                 elif pipe.pending:                             # input idle (single rank): flush what is in flight
@@ -195,12 +234,17 @@ class Worker:
                 continue
             consumed += len(records)
             self._run_host(node, records)
+        broker.flush_frames()
         return consumed
 
     def close(self) -> None:
         for pipe in self._pipes.values():
             pipe.close()
         self._pipes.clear()
+        if self._framer_eng is not None:
+            self._framer_eng.close()
+            self._frame_pool.close()
+            self._framer_eng = self._frame_pool = None
 
     def _all_idle(self, n: int) -> bool:
         """N > 1: the ranks stop together — a rank with nothing to do still has to run the exchange for the others"""
@@ -236,6 +280,7 @@ class Worker:
                             for rb in pipe.take_received():
                                 flushed += rb.n_publishes
                                 broker.produce_publishes(rb)
+                    broker.flush_frames()
                     if self._all_idle(flushed):            # nothing came out that a subscribed node still has to consume
                         return
                     continue

@@ -10,6 +10,7 @@
 #include "ck_kernels.cuh"
 
 static_assert(sizeof(ck_publish) == sizeof(ck_pub), "ck_publish must mirror ck_pub");
+static_assert(sizeof(ck_frame) == sizeof(ck_frame_ent), "ck_frame must mirror ck_frame_ent");
 
 #define CK_LIT_CAP (256 * 1024)
 #define CK_PAD 256   // tail padding of every byte buffer (readers may touch a few bytes past a span)
@@ -45,9 +46,20 @@ struct ck_handle {
     u32 *d_g_hist = nullptr, *d_g_o1 = nullptr, *d_g_o2 = nullptr, *d_g_keys = nullptr; long long* d_g_base = nullptr; unsigned long long *d_g_tile = nullptr, *d_g_grand = nullptr;
     bool grouped = false; bool opt_bucket = false; const u32* cur_perm = nullptr;
     // Kafka record-batch framing (allocated on first use)
-    long long *d_rb_batch_off = nullptr, *d_rb_rec_pos = nullptr, *d_rb_key_off = nullptr, *d_rb_corr_off = nullptr, *d_rb_rec_off = nullptr, *d_rb_frame_len = nullptr;
-    u32 *d_rb_rec_base = nullptr, *d_rb_batch_bad = nullptr, *d_rb_rec_batch = nullptr, *d_rb_val_len = nullptr, *d_rb_rec_bad = nullptr, *d_rb_idx = nullptr, *d_rb_sizes = nullptr, *d_rb_partial = nullptr;
-    int *d_rb_key_len = nullptr, *d_rb_corr_len = nullptr; u8* d_rb_frame = nullptr; uint64_t rb_frame_cap = 0; uint32_t rb_n = 0;
+    long long *d_rb_batch_off = nullptr, *d_rb_rec_pos = nullptr, *d_rb_key_off = nullptr, *d_rb_corr_off = nullptr;
+    u32 *d_rb_rec_base = nullptr, *d_rb_batch_bad = nullptr, *d_rb_rec_batch = nullptr, *d_rb_val_len = nullptr, *d_rb_rec_bad = nullptr;
+    int *d_rb_key_len = nullptr, *d_rb_corr_len = nullptr; uint32_t rb_n = 0;
+    long long* h_rb_boff = nullptr; u32* h_rb_rbase = nullptr; cudaEvent_t rb_ev = nullptr;   // pinned frame index staging
+    // frame pass (allocated on first use): per slot, then per record in group order; the frames and their table
+    ck_fitem* d_fr_items = nullptr; u32 *d_fr_gkey = nullptr, *d_fr_idx = nullptr, *d_fr_head = nullptr, *d_fr_fstart = nullptr, *d_fr_gfirst = nullptr;
+    u32 *d_fr_ffirst = nullptr, *d_fr_size = nullptr, *d_fr_nlive = nullptr, *d_fr_partial = nullptr;
+    long long *d_fr_gscan = nullptr, *d_fr_S = nullptr, *d_fr_F = nullptr, *d_fr_R = nullptr; unsigned long long *d_fr_tile = nullptr, *d_fr_grand = nullptr;
+    u32 *d_fr_o1 = nullptr, *d_fr_o2 = nullptr;      // its own sort buffers: the per-topic order of ck_group_publishes stays intact
+    ck_frame_ent* d_fr_table = nullptr; u8* d_fr_frames = nullptr; uint64_t fr_cap = 0; u32 fr_max = 0, fr_n = 0; bool fr_info = false, fr_sized = false;
+    const u32* fr_order = nullptr; long long fr_base = 0, fr_ts = 0;   // what the write half of the last pass needs to run again
+    u8* d_fr_blob = nullptr; long long* d_fr_desc = nullptr; long long* h_fr_info = nullptr;   // h_fr_info: pinned {frames, bytes}
+    int32_t* d_fr_slot = nullptr; u32 fr_nslots = 0, fr_ntopics = 0;
+    uint64_t fr_window = 1ull << 20;                 // frame_bytes (ck_set_option 2)
     // exchange planning (allocated on first use)
     u32* d_x_hist = nullptr; long long* d_x_base = nullptr; unsigned long long* d_x_nbytes = nullptr;
     long long *d_x_src_off = nullptr, *d_x_len = nullptr, *d_x_dst_off = nullptr; u32 *d_x_len32 = nullptr, *d_x_pub = nullptr;
@@ -176,15 +188,22 @@ extern "C" void ck_destroy(ck_handle* h) {
                     h->d_x_len32, h->d_x_pub, h->d_x_tile, h->d_x_grand, h->d_x_grand2};
     for (void* p : ptrs) if (p) cudaFree(p);
     void* gptrs[] = {h->gate.keys, h->gate.vals, h->gate.entries, h->gate.slots, h->gate.arena, h->gate.ctr, h->d_rec_entry,
-                     h->d_rb_batch_off, h->d_rb_rec_pos, h->d_rb_key_off, h->d_rb_corr_off, h->d_rb_rec_off, h->d_rb_frame_len, h->d_rb_rec_base, h->d_rb_batch_bad,
+                     h->d_rb_batch_off, h->d_rb_rec_pos, h->d_rb_key_off, h->d_rb_corr_off, h->d_rb_rec_base, h->d_rb_batch_bad,
                      h->d_g_hist, h->d_g_o1, h->d_g_o2, h->d_g_keys, h->d_g_base, h->d_g_tile, h->d_g_grand,
-                     h->d_rb_rec_batch, h->d_rb_val_len, h->d_rb_rec_bad, h->d_rb_idx, h->d_rb_sizes, h->d_rb_partial, h->d_rb_key_len, h->d_rb_corr_len, h->d_rb_frame};
+                     h->d_rb_rec_batch, h->d_rb_val_len, h->d_rb_rec_bad, h->d_rb_key_len, h->d_rb_corr_len,
+                     h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
+                     h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
+                     h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2};
     for (void* p : gptrs) if (p) cudaFree(p);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
     if (h->d_recv) cudaFree(h->d_recv);
     if (h->d_x_overflow) cudaFree(h->d_x_overflow);
     if (h->h_grand) cudaFreeHost(h->h_grand);
     if (h->h_x) cudaFreeHost(h->h_x);
+    if (h->h_fr_info) cudaFreeHost(h->h_fr_info);
+    if (h->h_rb_boff) cudaFreeHost(h->h_rb_boff);
+    if (h->h_rb_rbase) cudaFreeHost(h->h_rb_rbase);
+    if (h->rb_ev) cudaEventDestroy(h->rb_ev);
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
     if (h->xstream) { cudaStreamSynchronize(h->xstream); cudaStreamDestroy(h->xstream); }
     if (h->x_ev0) cudaEventDestroy(h->x_ev0);
@@ -265,7 +284,7 @@ static ck_view view_of(ck_handle* h) {
 }
 
 static int run_scan(ck_handle* h, const u32* len, u32 n, long long* out_off, u32 pad,
-                    unsigned long long* tile_sum = nullptr, unsigned long long* grand = nullptr);
+                    unsigned long long* tile_sum = nullptr, unsigned long long* grand = nullptr, int timer = CK_K_SCAN);
 
 static int group_alloc(ck_handle* h) {
     u32 nb_max = (h->max_pubs + CK_G_BLOCK - 1) / CK_G_BLOCK;
@@ -282,28 +301,46 @@ static int group_alloc(ck_handle* h) {
     return 0;
 }
 
-// stable two-pass radix sort of indices 0..n-1 by a 12-bit key -> d_g_o2 (and per-key counts in d_g_keys)
+// stable LSD radix sort of indices 0..n-1 by a key of 6 * passes bits (6 bits per pass, passes 1..5), ping-ponging between
+// o1 and o2 (default d_g_o1 / d_g_o2; two passes: the result is in o2) -> *result.  key_hist (CK_G_KEYS entries, zeroed here): per-key
+// counts, for keys below CK_G_KEYS
+template <int SHIFT, class KeyFn>
+static void group_pass(ck_handle* h, KeyFn keyf, const u32* in, u32 n, u32 nb, u32* key_hist, bool count, u32* dst) {
+    if (count) CKL(h) ck_group_count_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_hist, key_hist);
+    else CKL(h) ck_group_scatter_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_base, dst);
+}
 template <class KeyFn>
-static int group_sort(ck_handle* h, KeyFn keyf, u32 n, int timer) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_g_keys, 0, sizeof(u32) * CK_G_KEYS, h->stream));
+static void group_launch(ck_handle* h, KeyFn keyf, u32 p, const u32* in, u32 n, u32 nb, u32* key_hist, bool count, u32* dst) {
+    switch (p) {
+        case 0: group_pass<0>(h, keyf, in, n, nb, key_hist, count, dst); break;
+        case 1: group_pass<6>(h, keyf, in, n, nb, key_hist, count, dst); break;
+        case 2: group_pass<12>(h, keyf, in, n, nb, key_hist, count, dst); break;
+        case 3: group_pass<18>(h, keyf, in, n, nb, key_hist, count, dst); break;
+        default: group_pass<24>(h, keyf, in, n, nb, key_hist, count, dst); break;
+    }
+}
+template <class KeyFn>
+static int group_sort(ck_handle* h, KeyFn keyf, u32 n, int timer, u32 passes = 2, u32* key_hist = nullptr, const u32** result = nullptr,
+                      u32* o1 = nullptr, u32* o2 = nullptr) {
+    if (!o1) { o1 = h->d_g_o1; o2 = h->d_g_o2; }
+    if (key_hist) CUDA_TRY(h, cudaMemsetAsync(key_hist, 0, sizeof(u32) * CK_G_KEYS, h->stream));
+    if (result) *result = (passes & 1) ? o1 : o2;
     if (!n) return 0;
+    if (passes < 1 || passes > 5) return fail(h, "group_sort: 1 to 5 passes");
     u32 nb = (n + CK_G_BLOCK - 1) / CK_G_BLOCK;
-    {
-        KTimer t(h, timer);
-        CKL(h) ck_group_count_kernel<0, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, nullptr, n, h->d_g_hist, h->d_g_keys);
-        CUDA_TRY(h, cudaGetLastError());
+    auto out_of = [&](u32 p) -> u32* { return (p & 1) ? o2 : o1; };    // pass p scatters here
+    for (u32 p = 0; p < passes; p++) {
+        {   // the scatter of the previous pass, then the histogram of this one
+            KTimer t(h, timer);
+            if (p) group_launch(h, keyf, p - 1, p > 1 ? out_of(p - 2) : nullptr, n, nb, key_hist, false, out_of(p - 1));
+            group_launch(h, keyf, p, p ? out_of(p - 1) : nullptr, n, nb, key_hist, true, nullptr);
+            CUDA_TRY(h, cudaGetLastError());
+        }
+        if (run_scan(h, h->d_g_hist, 64 * nb, h->d_g_base, 0, h->d_g_tile, h->d_g_grand)) return 1;
     }
-    if (run_scan(h, h->d_g_hist, 64 * nb, h->d_g_base, 0, h->d_g_tile, h->d_g_grand)) return 1;
     {
         KTimer t(h, timer);
-        CKL(h) ck_group_scatter_kernel<0, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, nullptr, n, h->d_g_base, h->d_g_o1);
-        CKL(h) ck_group_count_kernel<6, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, h->d_g_o1, n, h->d_g_hist, h->d_g_keys);
-        CUDA_TRY(h, cudaGetLastError());
-    }
-    if (run_scan(h, h->d_g_hist, 64 * nb, h->d_g_base, 0, h->d_g_tile, h->d_g_grand)) return 1;
-    {
-        KTimer t(h, timer);
-        CKL(h) ck_group_scatter_kernel<6, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, h->d_g_o1, n, h->d_g_base, h->d_g_o2);
+        group_launch(h, keyf, passes - 1, passes > 1 ? out_of(passes - 2) : nullptr, n, nb, key_hist, false, out_of(passes - 1));
         CUDA_TRY(h, cudaGetLastError());
     }
     return 0;
@@ -321,7 +358,7 @@ static int launch_decode(ck_handle* h) {
     if (h->opt_bucket && n > 64) {
         if (group_alloc(h)) return 1;
         ck_key_len kf; kf.v = v;
-        if (group_sort(h, kf, n, CK_K_WALK)) return 1;
+        if (group_sort(h, kf, n, CK_K_WALK, 2, h->d_g_keys)) return 1;
         h->cur_perm = h->d_g_o2;
         v = view_of(h);
     }
@@ -380,8 +417,8 @@ extern "C" int ck_submit_device(ck_handle* h, const uint8_t* dev_in, const int64
 }
 
 static int run_scan(ck_handle* h, const u32* len, u32 n, long long* out_off, u32 pad,
-                    unsigned long long* tile_sum, unsigned long long* grand) {
-    KTimer t(h, CK_K_SCAN);
+                    unsigned long long* tile_sum, unsigned long long* grand, int timer) {
+    KTimer t(h, timer);
     if (!tile_sum) { tile_sum = h->d_tile_sum; grand = h->d_grand; }
     u32 ntiles = (n + CK_SCAN_TILE - 1) / CK_SCAN_TILE;
     if (n) {
@@ -613,7 +650,7 @@ extern "C" int ck_group_publishes(ck_handle* h) {
     if (group_alloc(h)) return 1;
     h->grouped = true;
     ck_key_pub kf; kf.pubs = h->d_pubs; kf.rank = h->comm_rank; kf.world = h->comm_ready ? h->comm_world : 1;
-    return group_sort(h, kf, h->n_pubs, CK_K_ROUTE);
+    return group_sort(h, kf, h->n_pubs, CK_K_ROUTE, 2, h->d_g_keys);
 }
 
 // engine options.  CK_OPT_BUCKET (1): bucket every submitted batch by record length before the thread-per-record walk —
@@ -621,6 +658,7 @@ extern "C" int ck_group_publishes(ck_handle* h) {
 // different schema branches run one after the other); homogeneous batches do not need it (it costs six small launches).
 extern "C" int ck_set_option(ck_handle* h, uint32_t option, uint64_t value) {
     if (option == 1) { h->opt_bucket = value != 0; return 0; }
+    if (option == 2) { if (value < 1) return fail(h, "ck_set_option: frame_bytes must be at least 1"); h->fr_window = value; return 0; }
     return fail(h, "ck_set_option: unknown option");
 }
 
@@ -650,6 +688,9 @@ static int rb_alloc(ck_handle* h) {
     CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_corr_off, sizeof(long long) * mr));
     CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_corr_len, sizeof(int) * mr));
     CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_bad, sizeof(u32) * mr));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_boff, sizeof(long long) * mr));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_rbase, sizeof(u32) * mr));
+    CUDA_TRY(h, cudaEventCreateWithFlags(&h->rb_ev, cudaEventDisableTiming));
     return 0;
 }
 static inline uint32_t host_be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
@@ -661,25 +702,28 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     cudaSetDevice(h->device);
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
     if (rb_alloc(h)) return 1;
-    std::vector<long long> boff; std::vector<u32> rbase;
-    uint64_t pos = 0; uint64_t total = 0;
+    // the frame index is staged in page-locked memory the handle owns: its copies are asynchronous.  The staging is reused
+    // once the copies of the previous call have been done (normally long ago: it waits for those copies only)
+    CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
+    long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
+    uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
     while (pos + 12 <= nbytes) {
         uint32_t blen = host_be32(host_buf + pos + 8);
         uint64_t end = pos + 12 + (uint64_t)blen;
         if ((int32_t)blen < (int32_t)(CK_RB_HEADER - 12) || end > nbytes) break;         // truncated trailing frame: legal in a fetch response
         uint32_t cnt = host_be32(host_buf + pos + 57);
-        if (total + cnt > h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
-        boff.push_back((long long)pos); rbase.push_back((u32)total);
+        if (total + cnt > h->max_records || nb >= h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
+        boff[nb] = (long long)pos; rbase[nb] = (u32)total; nb++;
         total += cnt; pos = end;
     }
-    boff.push_back((long long)pos); rbase.push_back((u32)total);
-    u32 nb = (u32)boff.size() - 1, n = (u32)total;
+    boff[nb] = (long long)pos; rbase[nb] = (u32)total;
+    u32 n = (u32)total;
     if (n_records) *n_records = n;
     CUDA_TRY(h, cudaMemcpyAsync(h->d_in, host_buf, pos, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_in + pos, 0, 16, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff.data(), sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase.data(), sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));           // the two index vectors are pageable stack objects
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaEventRecord(h->rb_ev, h->stream));
     h->rb_n = n;
     if (nb) {
         KTimer t(h, CK_K_WALK);
@@ -698,8 +742,19 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
 
 // per record of the last ck_submit_recordbatch: where value / key / correlation_id header lie in the submitted buffer
 // (key_len / corr_len = -1: absent), and whether its frame failed the CRC / framing check
+static int fetch_rb_index_impl(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
+                               int64_t* corr_off, int32_t* corr_len, uint32_t* bad, bool wait);
 extern "C" int ck_fetch_rb_index(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
                                  int64_t* corr_off, int32_t* corr_len, uint32_t* bad) {
+    return fetch_rb_index_impl(h, val_off, val_len, key_off, key_len, corr_off, corr_len, bad, true);
+}
+// the same copies queued only (page-locked destinations): they ride along with the step's results, complete after ck_sync
+extern "C" int ck_fetch_rb_index_async(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
+                                       int64_t* corr_off, int32_t* corr_len, uint32_t* bad) {
+    return fetch_rb_index_impl(h, val_off, val_len, key_off, key_len, corr_off, corr_len, bad, false);
+}
+static int fetch_rb_index_impl(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
+                               int64_t* corr_off, int32_t* corr_len, uint32_t* bad, bool wait) {
     cudaSetDevice(h->device);
     u32 n = h->rb_n;
     if (!n) return 0;
@@ -710,50 +765,239 @@ extern "C" int ck_fetch_rb_index(ck_handle* h, int64_t* val_off, uint32_t* val_l
     if (corr_off) CUDA_TRY(h, cudaMemcpyAsync(corr_off, h->d_rb_corr_off, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
     if (corr_len) CUDA_TRY(h, cudaMemcpyAsync(corr_len, h->d_rb_corr_len, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
     if (bad) CUDA_TRY(h, cudaMemcpyAsync(bad, h->d_rb_rec_bad, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
 
-// produce side: the publishes host_idx[0..n) of the current plan (one topic-partition, in send order) become ONE
-// RecordBatch v2 frame — varint record headers, key = correlation id when keyed, calfkit's two headers, CRC32C — built
-// on the device from the payloads where they lie in the output buffer, then copied to host_frame.
+// ---- frame pass: the publishes of a step (or host-produced records) as RecordBatch v2 frames (csrc/ck_kafka.cuh) -------
+static int fr_grow(ck_handle* h, uint64_t cap) {
+    if (h->d_fr_frames) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_fr_frames); cudaFree(h->d_fr_partial); }
+    h->d_fr_frames = nullptr; h->d_fr_partial = nullptr; h->fr_cap = 0;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_frames, cap + CK_PAD));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_partial, sizeof(u32) * (cap / CK_RB_CRC_CHUNK + (size_t)h->max_pubs + 2)));
+    h->fr_cap = cap;
+    return 0;
+}
+static int fr_alloc(ck_handle* h) {
+    if (h->d_fr_items) return 0;
+    size_t m = (size_t)h->max_pubs;
+    h->fr_max = h->max_pubs;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_items, sizeof(ck_fitem) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gkey, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_idx, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_head, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_fstart, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gfirst, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_ffirst, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_size, sizeof(u32) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_nlive, sizeof(u32)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gscan, sizeof(long long) * (m + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_S, sizeof(long long) * (m + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_F, sizeof(long long) * (m + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_R, sizeof(long long) * (m + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_tile, sizeof(unsigned long long) * (m / CK_SCAN_TILE + 2)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_grand, sizeof(unsigned long long)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_table, sizeof(ck_frame_ent) * m));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o1, sizeof(u32) * (m + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o2, sizeof(u32) * (m + 1)));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_fr_info, sizeof(long long) * 2));
+    // first size of the frame buffer: every payload framed twice (a payload slot carries at most two publishes) plus the
+    // record and frame overhead of a publish with an id of up to 40 bytes.  A pass that needs more grows it (ck_frames_size)
+    return fr_grow(h, 2 * h->max_out + 160ull * m + 4096);
+}
+
+// group -> split -> size -> table + headers -> write -> CRC over items[0..n) that a source kernel built (gkey: group keys of
+// 6 * passes bits, all ones = not framed; passes 0: one group in the given order).  Queued only.
+static int frame_write(ck_handle* h);
+static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long long window, long long base_offset, long long ts) {
+    h->fr_n = n; h->fr_info = false; h->fr_sized = false;
+    if (!n) return 0;
+    const u32* order = nullptr;
+    if (passes) {
+        if (group_alloc(h)) return 1;
+        ck_key_arr kf; kf.k = h->d_fr_gkey;
+        if (group_sort(h, kf, n, CK_K_FRAME, passes, nullptr, &order, h->d_fr_o1, h->d_fr_o2)) return 1;
+    }
+    h->fr_order = order; h->fr_base = base_offset; h->fr_ts = ts;
+    u32 nb = (n + 255) / 256;
+    unsigned long long* tile = h->d_fr_tile; unsigned long long* grand = h->d_fr_grand;
+    {
+        KTimer t(h, CK_K_FRAME);
+        CUDA_TRY(h, cudaMemsetAsync(h->d_fr_nlive, 0, sizeof(u32), h->stream));
+        CKL(h) ck_fr_heads_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_gkey, n, excl, h->d_fr_head, h->d_fr_nlive);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_head, n, h->d_fr_gscan, 0, tile, grand, CK_K_FRAME)) return 1;
+    {
+        KTimer t(h, CK_K_FRAME);
+        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head, h->d_fr_gscan, n, h->d_fr_gfirst);
+        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_head, h->d_fr_gscan, h->d_fr_gfirst, n, h->d_fr_nlive, h->d_fr_size);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_size, n, h->d_fr_S, 0, tile, grand, CK_K_FRAME)) return 1;
+    {
+        KTimer t(h, CK_K_FRAME);
+        CKL(h) ck_fr_split_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head, h->d_fr_gscan, h->d_fr_gfirst, h->d_fr_S, n, h->d_fr_nlive, window, h->d_fr_fstart);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_fstart, n, h->d_fr_F, 0, tile, grand, CK_K_FRAME)) return 1;
+    {
+        KTimer t(h, CK_K_FRAME);
+        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_fstart, h->d_fr_F, n, h->d_fr_ffirst);
+        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_fstart, h->d_fr_F, h->d_fr_ffirst, n, h->d_fr_nlive, h->d_fr_size);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_size, n, h->d_fr_R, 0, tile, grand, CK_K_FRAME)) return 1;
+    if (frame_write(h)) return 1;
+    // frames and bytes, copied back with the step's results (ck_frames_size reads them)
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info, h->d_fr_F + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info + 1, h->d_fr_R + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    h->fr_info = true;
+    return 0;
+}
+
+// the half of the pass that writes into the frame buffer: table + headers, records, CRC.  Everything it reads stays on the
+// device until the next pass, so it runs again into a larger buffer when the frames did not fit
+static int frame_write(ck_handle* h) {
+    u32 n = h->fr_n, nb = (n + 255) / 256;
+    const u32* order = h->fr_order;
+    {
+        KTimer t(h, CK_K_FRAME);   // chunk counts per frame go to d_fr_head (free again), their scan to d_fr_S
+        CKL(h) ck_fr_table_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_ffirst, h->d_fr_F, h->d_fr_R, n, h->d_fr_nlive,
+                                                          h->fr_base, h->fr_ts, h->fr_cap, h->d_fr_table, h->d_fr_frames, h->d_fr_head);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
+    {
+        KTimer t(h, CK_K_FRAME);
+        CKL(h) ck_fr_write_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_fstart, h->d_fr_F, h->d_fr_ffirst, h->d_fr_R, n,
+                                                                   h->d_fr_nlive, h->fr_cap, h->d_fr_frames);
+        u32 cblocks = (n + 7) / 8; if (cblocks > h->num_sms * 8) cblocks = h->num_sms * 8;
+        CKL(h) ck_fr_crc_chunks_kernel<<<cblocks, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_frames, h->d_fr_partial);
+        CKL(h) ck_fr_crc_fold_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_partial, h->d_fr_frames);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    return 0;
+}
+
+// bits of the group key for `groups` groups (all ones is the key of unframed slots)
+static u32 fr_passes(unsigned long long groups) { u32 p = 1; while (p < 6 && groups >= (1ull << (6 * p)) - 1) p++; return p; }
+
+extern "C" int ck_set_frame_topics(ck_handle* h, const int32_t* topic_ids, uint32_t n) {
+    cudaSetDevice(h->device);
+    int32_t top = -1;
+    for (u32 i = 0; i < n; i++) { if (topic_ids[i] < 0) return fail(h, "ck_set_frame_topics: ids must be >= 0"); if (topic_ids[i] > top) top = topic_ids[i]; }
+    std::vector<int32_t> slot((size_t)top + 1, -1);
+    for (u32 i = 0; i < n; i++) if (slot[topic_ids[i]] < 0) slot[topic_ids[i]] = (int32_t)i;
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (h->d_fr_slot) { cudaFree(h->d_fr_slot); h->d_fr_slot = nullptr; }
+    h->fr_nslots = (u32)slot.size(); h->fr_ntopics = n;
+    if (n) {
+        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_slot, sizeof(int32_t) * slot.size()));
+        CUDA_TRY(h, cudaMemcpy(h->d_fr_slot, slot.data(), sizeof(int32_t) * slot.size(), cudaMemcpyHostToDevice));
+    }
+    return 0;
+}
+
+// the live publishes of the current plan to the frame topics, grouped by (topic, partition), as frames: queued only
+extern "C" int ck_encode_frames(ck_handle* h, int64_t timestamp_ms) {
+    cudaSetDevice(h->device);
+    if (!h->fr_ntopics) return fail(h, "ck_encode_frames: call ck_set_frame_topics first");
+    unsigned long long groups = (unsigned long long)h->fr_ntopics * ((unsigned long long)h->num_partitions + 1);
+    u32 passes = fr_passes(groups);
+    if (passes > 5) return fail(h, "ck_encode_frames: more than 2^30 (topic, partition) groups");
+    if (fr_alloc(h)) return 1;
+    u32 n = h->n_pubs, excl = (u32)((1ull << (6 * passes)) - 1);
+    {
+        KTimer t(h, CK_K_FRAME);
+        if (n) CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, nullptr, n, h->d_pay_len, h->d_out_off, h->d_out,
+            h->d_cols, h->n, h->d_fr_slot, h->fr_nslots, h->num_partitions, excl, h->d_fr_items, h->d_fr_gkey);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    return frame_pass(h, n, passes, excl, h->fr_window, 0, timestamp_ms);
+}
+
+// records a host path produced for one topic (host tools, the LLM boundary, declined records re-run on the host)
+extern "C" int ck_encode_frames_records(ck_handle* h, int32_t topic_id, const uint8_t* host_blob, uint64_t nbytes, const int64_t* host_desc,
+                                        uint32_t n, int64_t timestamp_ms) {
+    cudaSetDevice(h->device);
+    if (n > h->max_pubs) return fail(h, "ck_encode_frames_records: more records than the publish table holds");
+    if (nbytes > h->max_in) return fail(h, "ck_encode_frames_records: records larger than max_in_bytes");
+    for (u32 i = 0; i < n; i++) {
+        const int64_t* d = host_desc + 6 * (size_t)i;
+        for (int f = 0; f < 3; f++) {
+            if (d[2 * f + 1] < (f ? -1 : 0) || (d[2 * f + 1] >= 0 && (d[2 * f] < 0 || (uint64_t)(d[2 * f] + d[2 * f + 1]) > nbytes)))
+                return fail(h, "ck_encode_frames_records: span outside the records");
+        }
+    }
+    u32 passes = fr_passes((unsigned long long)h->num_partitions + 1);
+    if (passes > 5) return fail(h, "ck_encode_frames_records: too many partitions");
+    if (fr_alloc(h)) return 1;
+    if (!h->d_fr_blob) {
+        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_blob, h->max_in + CK_PAD));
+        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_desc, sizeof(long long) * 6 * (size_t)h->max_pubs));
+    }
+    if (nbytes) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_blob, host_blob, nbytes, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_fr_blob + nbytes, 0, 16, h->stream));
+    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_desc, host_desc, sizeof(long long) * 6 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+    {
+        KTimer t(h, CK_K_FRAME);
+        if (n) CKL(h) ck_fr_src_recs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_fr_blob, h->d_fr_desc, n, topic_id, h->num_partitions,
+                                                                                   h->d_fr_items, h->d_fr_gkey);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    return frame_pass(h, n, passes, (u32)((1ull << (6 * passes)) - 1), h->fr_window, 0, timestamp_ms);
+}
+
+// frames and bytes of the last pass (waits for it).  Frames that did not fit the frame buffer are written again into a
+// buffer grown to their size (one more wait): a step is sized for whatever its ids and payloads need
+extern "C" int ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes) {
+    cudaSetDevice(h->device);
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    long long nf = h->fr_info ? h->h_fr_info[0] : 0, nb = h->fr_info ? h->h_fr_info[1] + (long long)CK_RB_HEADER * nf : 0;
+    if ((uint64_t)nb > h->fr_cap) {
+        if (fr_grow(h, (uint64_t)nb + (uint64_t)nb / 8 + 4096) || frame_write(h)) return 1;
+        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    }
+    h->fr_sized = true;
+    if (n_frames) *n_frames = (u32)nf;
+    if (nbytes) *nbytes = (uint64_t)nb;
+    return 0;
+}
+
+// copies of the frame table and the frames of the last pass, queued only: page-locked destinations, complete after the
+// next ck_sync.  ck_frames_size must have been called since the pass (it gives the sizes and makes sure the frames fit)
+extern "C" int ck_fetch_frames_async(ck_handle* h, ck_frame* host_table, uint32_t table_cap, uint8_t* host_frames, uint64_t cap) {
+    cudaSetDevice(h->device);
+    if (h->fr_info && !h->fr_sized) return fail(h, "ck_fetch_frames_async: call ck_frames_size after the frame pass first");
+    long long nf = h->fr_info ? h->h_fr_info[0] : 0, nb = h->fr_info ? h->h_fr_info[1] + (long long)CK_RB_HEADER * nf : 0;
+    if ((uint64_t)nb > h->fr_cap) return fail(h, "ck_fetch_frames_async: frames larger than the frame buffer");
+    if ((uint64_t)nf > table_cap || (uint64_t)nb > cap) return fail(h, "ck_fetch_frames_async: host buffers too small");
+    if (nf) CUDA_TRY(h, cudaMemcpyAsync(host_table, h->d_fr_table, sizeof(ck_frame) * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
+    if (nb) CUDA_TRY(h, cudaMemcpyAsync(host_frames, h->d_fr_frames, (size_t)nb, cudaMemcpyDeviceToHost, h->stream));
+    return 0;
+}
+
+// produce side, one topic-partition: the publishes host_idx[0..n) of the current plan (in send order) become ONE frame —
+// the frame pass with one group, offsetDelta = position in the list — copied to host_frame (waits)
 extern "C" int ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uint32_t n, int64_t base_offset, int64_t timestamp_ms,
                                      uint8_t* host_frame, uint64_t cap, uint64_t* frame_len) {
     cudaSetDevice(h->device);
     if (!n || n > h->n_pubs) return fail(h, "ck_encode_recordbatch: index list empty or longer than the publish table");
-    if (!h->d_rb_idx) {
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_idx, sizeof(u32) * (size_t)h->max_pubs));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_sizes, sizeof(u32) * (size_t)h->max_pubs));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_off, sizeof(long long) * ((size_t)h->max_pubs + 1)));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_frame_len, sizeof(long long)));
-        h->rb_frame_cap = h->max_out + 256ull * h->max_payloads + 4096;
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_frame, h->rb_frame_cap + CK_PAD));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_partial, sizeof(u32) * (h->rb_frame_cap / CK_RB_CRC_CHUNK + 2)));
-    }
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_idx, host_idx, sizeof(u32) * n, cudaMemcpyHostToDevice, h->stream));
+    if (fr_alloc(h)) return 1;
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_idx, host_idx, sizeof(u32) * n, cudaMemcpyHostToDevice, h->stream));
     {
-        KTimer t(h, CK_K_EMIT);
-        CKL(h) ck_rb_size_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_pubs, h->d_rb_idx, n, h->d_pay_len, h->d_cols, h->n, h->d_rb_sizes);
+        KTimer t(h, CK_K_FRAME);
+        CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, h->d_fr_idx, n, h->d_pay_len, h->d_out_off, h->d_out,
+            h->d_cols, h->n, nullptr, 0, 0, CK_RB_NONE, h->d_fr_items, h->d_fr_gkey);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_rb_sizes, n, h->d_rb_rec_off, 0)) return 1;
-    // the frame's size is known on the device only; bound it on the host to size the launches and the copy
-    uint64_t out_total = 0;
-    { unsigned long long g = 0; CUDA_TRY(h, cudaMemcpyAsync(&g, h->d_grand, sizeof g, cudaMemcpyDeviceToHost, h->stream)); CUDA_TRY(h, cudaStreamSynchronize(h->stream)); out_total = g; }
-    uint64_t total = CK_RB_HEADER + out_total;
-    if (total > h->rb_frame_cap) return fail(h, "ck_encode_recordbatch: frame larger than the frame buffer");
+    if (frame_pass(h, n, 0, CK_RB_NONE, ~0ull, base_offset, timestamp_ms)) return 1;
+    uint32_t nf = 0; uint64_t total = 0;
+    if (ck_frames_size(h, &nf, &total)) return 1;
+    if (nf != 1) return fail(h, "ck_encode_recordbatch: the index list holds no live publish");
     if (total > cap) return fail(h, "ck_encode_recordbatch: host buffer too small");
-    {
-        KTimer t(h, CK_K_EMIT);
-        CKL(h) ck_rb_write_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(view_of(h), h->d_pubs, h->d_rb_idx, n, h->d_pay_len, h->d_out_off, h->d_out, h->d_cols, h->n,
-                                                                h->d_rb_rec_off, h->d_rb_frame);
-        CKL(h) ck_rb_header_kernel<<<1, 32, 0, h->stream>>>(h->d_rb_frame, h->d_rb_rec_off, n, base_offset, timestamp_ms, h->d_rb_frame_len);
-        u32 nchunks = (u32)((total - CK_RB_CRC_FROM + CK_RB_CRC_CHUNK - 1) / CK_RB_CRC_CHUNK);
-        CKL(h) ck_rb_crc_chunks_kernel<<<(nchunks + 7) / 8, 256, 0, h->stream>>>(h->d_rb_frame, h->d_rb_frame_len, h->d_rb_partial);
-        CKL(h) ck_rb_crc_fold_kernel<<<1, 32, 0, h->stream>>>(h->d_rb_frame, h->d_rb_frame_len, h->d_rb_partial);
-        CUDA_TRY(h, cudaGetLastError());
-    }
-    CUDA_TRY(h, cudaMemcpyAsync(host_frame, h->d_rb_frame, total, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_frame, h->d_fr_frames, total, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (frame_len) *frame_len = total;
     return 0;

@@ -10,7 +10,7 @@
 //     key 1 + id      live publish to registered topic `id` (ids above 4093 share the last live key)
 //     key 4095        unused slot
 // Result: order[] = publish indices grouped by key, send order preserved inside a group, and the number of publishes per
-// key — the host slices, it never scans.
+// key — the host slices, it never scans.  The same sort runs over wider keys in more passes (group_sort in ck_api.cu).
 #ifndef CK_GROUP_CUH
 #define CK_GROUP_CUH
 
@@ -44,7 +44,15 @@ struct ck_key_len {
     __device__ __forceinline__ u32 operator()(u32 i) const { u32 len; ck_rec_in(v, i, len); u32 k = len >> 5; return CK_G_KEYS - 1 - (k < CK_G_KEYS - 1 ? k : CK_G_KEYS - 1); }
 };
 
+// the group keys of the frame pass (ck_kafka.cuh), one per slot, computed by its source kernel: (frame topic, partition)
+// composites that need up to five passes
+struct ck_key_arr {
+    const u32* k;
+    __device__ __forceinline__ u32 operator()(u32 i) const { return k[i]; }
+};
+
 // pass over `in` (NULL = identity order): digit histogram per block -> hist[digit][block]; pass 0 also counts whole keys
+// (keys below CK_G_KEYS) when key_hist is given
 template <int SHIFT, class KeyFn>
 __global__ void __launch_bounds__(CK_G_BLOCK)
 ck_group_count_kernel(KeyFn keyf, const u32* __restrict__ in, u32 n, u32* __restrict__ hist, u32* __restrict__ key_hist) {
@@ -55,7 +63,7 @@ ck_group_count_kernel(KeyFn keyf, const u32* __restrict__ in, u32 n, u32* __rest
     bool live = j < n;
     u32 key = 0;
     if (live) { key = keyf(in ? in[j] : j); atomicAdd(&s_cnt[(key >> SHIFT) & 63u], 1u); }
-    if (SHIFT == 0) {
+    if (SHIFT == 0 && key_hist) {
         u32 act = __ballot_sync(0xffffffffu, live);
         if (live) {
             u32 peers = __match_any_sync(act, key);

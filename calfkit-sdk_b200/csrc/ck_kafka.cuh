@@ -12,11 +12,8 @@
 //   ck_rb_fields_kernel  thread per record: zig-zag varints -> key span, value span, the `correlation_id` header span
 // The walker then reads every value where it lies inside the raw buffer (ck_view.len): no per-record slicing on the host.
 //
-// encode (produce): the payloads of one topic-partition (an index list the producer side already has) become one frame:
-//   ck_rb_size_kernel    thread per record: encoded size (varints depend on the record's offsetDelta = its rank)
-//   (scan)               -> byte offset of every record inside the frame
-//   ck_rb_write_kernel   warp per record: varint header, key, value, the two headers calfkit's publishes carry
-//   ck_rb_header_kernel + ck_rb_crc_chunks/fold: the 61-byte batch header, CRC32C over the frame in 16 KB chunks
+// encode (produce): the publishes of a step to the frame topics, grouped by (topic, partition), become frames in one
+// asynchronous pass (ck_fr_*_kernel, below); ck_encode_recordbatch is its one-group case
 #ifndef CK_KAFKA_CUH
 #define CK_KAFKA_CUH
 
@@ -201,6 +198,21 @@ ck_rb_mark_bad_kernel(const u32* __restrict__ rec_bad, u32 n, u32* __restrict__ 
 }
 
 // ---- encode -------------------------------------------------------------------------------------------------------------
+// Every live publish to a frame topic of the current plan (or every record of a small host-produced batch) becomes one
+// record of a frame, in one pass queued on the stream (nothing in it waits for the host):
+//   source   thread per publish / record: its value, key and correlation id (ck_fitem) and its group key (frame topic,
+//            partition + 1); partition -1 (unkeyed) is a group of its own per topic, the producer client picks its partition
+//   group    stable LSD radix sort by the group key (group_sort, ck_group.cuh): one run per group, send order kept
+//   split    s_k = encoded size of record k with offsetDelta = its rank in the group, P_k = exclusive prefix of s inside the
+//            group; record k starts a frame when it heads its group or floor(P_k / W) != floor(P_{k-1} / W), W = frame_bytes.
+//            The real records of a frame (offsetDelta = rank in the frame) are no larger than their s_k, so a frame holds at
+//            most 61 + W + one record bytes
+//   size     exact sizes -> scan -> byte offset of every record; frames lie back to back, each behind its 61-byte header
+//   table    thread per frame: frame table entry (topic id, partition, offset, length, records), header, CRC chunk count
+//   write    warp per record: varint header, key, value, the headers calfkit's publishes carry
+//   crc      warp per 16 KB chunk of any frame (chunk -> frame by binary search over the chunk scan), fold per frame
+// Key and correlation id are JSON string content as they lie in the envelope: written unescaped (ck_key_byte), the bytes
+// correlation_id.encode() gives and ck_murmur2_key hashes.
 __device__ __forceinline__ u32 ck_varint_size(long long v) {
     unsigned long long u = ((unsigned long long)v << 1) ^ (unsigned long long)(v >> 63);
     u32 n = 1;
@@ -217,110 +229,240 @@ __device__ __forceinline__ u32 ck_put_varint(u8* p, long long v) {
 // what calfkit's publishes carry (SURVEY.md Appendix A): key = correlation id bytes when keyed, headers
 // content-type: application/json and correlation_id (FastStream)
 #define CK_RB_CT_HDR 30u             // varint(12) "content-type" varint(16) "application/json" = 1 + 12 + 1 + 16
-struct ck_rb_rec { u32 body_len, key_len, corr_len, val_len; };
+#define CK_RB_NONE 0xffffffffu       // absent key / correlation id
+#define CK_RB_CRC_CHUNK 16384u
 
-__device__ __forceinline__ ck_rb_rec ck_rb_measure(u32 rank, u32 val_len, u32 corr_len, bool keyed) {
-    ck_rb_rec r; r.val_len = val_len; r.corr_len = corr_len; r.key_len = keyed ? corr_len : 0xffffffffu;
+struct ck_fitem {                    // one record to frame
+    const u8* val; const u8* key; const u8* corr;
+    u32 val_len;
+    u32 key_raw, key_len;            // JSON string content: bytes in the source, bytes unescaped (CK_RB_NONE: no key)
+    u32 corr_raw, corr_len;          // same for the correlation_id header (CK_RB_NONE: no header)
+    int32_t topic_id, partition;
+};
+struct ck_frame_ent {                // one frame of the frame table (mirrors ck_frame in include/calfkit_b200.h)
+    int32_t topic_id, partition;     // partition -1: unkeyed records, the producer client picks the partition
+    uint32_t n_records, first;       // records, first record in group order
+    long long offset, length;        // bytes in the frame buffer
+};
+
+__device__ __forceinline__ u32 ck_unescaped_len(const u8* p, u32 raw) {
+    if (raw == CK_RB_NONE) return CK_RB_NONE;
+    GRd r; r.init(p, raw);
+    u32 n = 0;
+    for (u32 q = 0; q < raw; n++) ck_key_byte(r, q);
+    return n;
+}
+// body length of a record whose offsetDelta is `rank` (timestampDelta 0)
+__device__ __forceinline__ u32 ck_rb_measure(const ck_fitem& it, u32 rank) {
     u32 body = 1 + 1 + ck_varint_size(rank);                                    // attributes, timestampDelta 0, offsetDelta
-    body += keyed ? ck_varint_size(corr_len) + corr_len : 1;                    // key (or null)
-    body += ck_varint_size(val_len) + val_len;
-    body += 1 + CK_RB_CT_HDR + (1 + 14 + ck_varint_size(corr_len) + corr_len);  // 2 headers
-    r.body_len = body;
-    return r;
+    body += it.key_len != CK_RB_NONE ? ck_varint_size(it.key_len) + it.key_len : 1;   // key (or null)
+    body += ck_varint_size(it.val_len) + it.val_len;
+    body += 1 + CK_RB_CT_HDR;                                                   // header count, content-type
+    if (it.corr_len != CK_RB_NONE) body += 1 + 14 + ck_varint_size(it.corr_len) + it.corr_len;
+    return body;
 }
+__device__ __forceinline__ u32 ck_rb_encoded_size(const ck_fitem& it, u32 rank) { u32 b = ck_rb_measure(it, rank); return ck_varint_size(b) + b; }
 
-// idx[k] = index into the publish table of the k-th record of this topic-partition (its offsetDelta = k)
+// source: publishes idx[i] (NULL: publish i) of the plan.  frame_slot[topic id] = index of the frame topic or -1; NULL: one
+// group for all of them (ck_encode_recordbatch).  Unframed slots get the key `excl`, which sorts last
 __global__ void __launch_bounds__(256)
-ck_rb_size_kernel(const ck_pub* __restrict__ pubs, const u32* __restrict__ idx, u32 n, const u32* __restrict__ pay_len,
-                  const u32* __restrict__ cols, u32 stride, u32* __restrict__ sizes) {
-    u32 k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= n) return;
-    ck_pub p = pubs[idx[k]];
-    ck_rb_rec r = ck_rb_measure(k, pay_len[p.payload], cols[(size_t)CK_COL_CORR_LEN * stride + p.record], p.has_key != 0);
-    sizes[k] = ck_varint_size(r.body_len) + r.body_len;
-}
-
-// warp per record; corr bytes are the raw JSON string content of deps.correlation_id (ids without escapes: the hashing
-// rule of ck_murmur2_key applies to escaped ones — those are rejected here by the host side before encoding)
-__global__ void __launch_bounds__(256)
-ck_rb_write_kernel(ck_view vw, const ck_pub* __restrict__ pubs, const u32* __restrict__ idx, u32 n, const u32* __restrict__ pay_len,
-                   const long long* __restrict__ out_off, const u8* __restrict__ out, const u32* __restrict__ cols, u32 stride,
-                   const long long* __restrict__ rec_off, u8* __restrict__ frame) {
-    u32 k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (k >= n) return;
-    ck_pub p = pubs[idx[k]];
+ck_fr_src_pubs_kernel(ck_view vw, const ck_pub* __restrict__ pubs, const u32* __restrict__ idx, u32 n, const u32* __restrict__ pay_len,
+                      const long long* __restrict__ out_off, const u8* __restrict__ out, const u32* __restrict__ cols, u32 stride,
+                      const int32_t* __restrict__ frame_slot, u32 n_slots, u32 nparts, u32 excl,
+                      ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
+    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ck_pub p = pubs[idx ? idx[i] : i];
+    int slot = -1;
+    if (p.payload != 0xffffffffu) slot = !frame_slot ? 0 : (p.topic_id >= 0 && (u32)p.topic_id < n_slots ? frame_slot[p.topic_id] : -1);
+    if (slot < 0) { gkey[i] = excl; return; }
+    ck_fitem it;
     u32 rl; const u8* rec = ck_rec(vw, p.record, rl);
     u32 co = cols[(size_t)CK_COL_CORR_OFF * stride + p.record], cl = cols[(size_t)CK_COL_CORR_LEN * stride + p.record];
-    ck_rb_rec r = ck_rb_measure(k, pay_len[p.payload], cl, p.has_key != 0);
-    u8* d = frame + CK_RB_HEADER + rec_off[k];
-    u32 pos = 0, vpos = 0, kpos = 0, cpos = 0;
-    // every lane computes the same layout; lane 0 writes the small pieces, the warp copies key / value / header value
+    it.val = out + out_off[p.payload]; it.val_len = pay_len[p.payload];
+    it.corr = rec + co; it.corr_raw = cl; it.corr_len = ck_unescaped_len(it.corr, cl);
+    it.key = it.corr; it.key_raw = p.has_key ? cl : CK_RB_NONE; it.key_len = p.has_key ? it.corr_len : CK_RB_NONE;
+    it.topic_id = p.topic_id; it.partition = p.has_key ? p.partition : -1;
+    items[i] = it;
+    gkey[i] = frame_slot ? (u32)slot * (nparts + 1) + (u32)(it.partition + 1) : 0u;
+}
+
+// source: records a host path produced for one topic.  desc[i] = {value off, len, key off, len, correlation id off, len}
+// into blob (len -1: absent); key and id are JSON string content, the partition is the plan's: murmur2(key) % nparts
+__global__ void __launch_bounds__(256)
+ck_fr_src_recs_kernel(const u8* __restrict__ blob, const long long* __restrict__ desc, u32 n, int32_t topic_id, u32 nparts,
+                      ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
+    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long* d = desc + 6 * (size_t)i;
+    ck_fitem it;
+    it.val = blob + d[0]; it.val_len = (u32)d[1];
+    it.key = blob + (d[3] >= 0 ? d[2] : 0); it.key_raw = d[3] >= 0 ? (u32)d[3] : CK_RB_NONE; it.key_len = ck_unescaped_len(it.key, it.key_raw);
+    it.corr = blob + (d[5] >= 0 ? d[4] : 0); it.corr_raw = d[5] >= 0 ? (u32)d[5] : CK_RB_NONE; it.corr_len = ck_unescaped_len(it.corr, it.corr_raw);
+    int part = -1;
+    if (it.key_raw != CK_RB_NONE && nparts) { GRd r; r.init(it.key, it.key_raw); part = (int)((ck_murmur2_key(r, 0, it.key_raw) & 0x7fffffffu) % nparts); }
+    it.topic_id = topic_id; it.partition = part;
+    items[i] = it;
+    gkey[i] = (u32)(part + 1);
+}
+
+__device__ __forceinline__ u32 ck_fr_src(const u32* order, u32 k) { return order ? order[k] : k; }
+
+// head[k]: record k (in group order) starts a group; *n_live = records that are framed (they sort before the rest)
+__global__ void __launch_bounds__(256)
+ck_fr_heads_kernel(const u32* __restrict__ order, const u32* __restrict__ gkey, u32 n, u32 excl, u32* __restrict__ head, u32* __restrict__ n_live) {
+    u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    u32 key = gkey[ck_fr_src(order, k)];
+    bool live = key != excl;
+    head[k] = live && (k == 0 || gkey[ck_fr_src(order, k - 1)] != key);
+    if (live && (k + 1 == n || gkey[ck_fr_src(order, k + 1)] == excl)) *n_live = k + 1;
+}
+// first[id] = k for every k that starts group / frame id (scan = exclusive scan of flag)
+__global__ void __launch_bounds__(256)
+ck_fr_first_kernel(const u32* __restrict__ flag, const long long* __restrict__ scan, u32 n, u32* __restrict__ first) {
+    u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n && flag[k]) first[scan[k]] = k;
+}
+// encoded size of record k with offsetDelta = its rank in its group / frame
+__global__ void __launch_bounds__(256)
+ck_fr_size_kernel(const u32* __restrict__ order, const ck_fitem* __restrict__ items, const u32* __restrict__ flag,
+                  const long long* __restrict__ scan, const u32* __restrict__ first, u32 n, const u32* __restrict__ n_live, u32* __restrict__ size) {
+    u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    if (k >= *n_live) { size[k] = 0; return; }
+    u32 id = (u32)(scan[k] + flag[k]) - 1;
+    size[k] = ck_rb_encoded_size(items[ck_fr_src(order, k)], k - first[id]);
+}
+// the split rule (see above); S = exclusive scan of the group-rank sizes
+__global__ void __launch_bounds__(256)
+ck_fr_split_kernel(const u32* __restrict__ head, const long long* __restrict__ gscan, const u32* __restrict__ gfirst,
+                   const long long* __restrict__ S, u32 n, const u32* __restrict__ n_live, unsigned long long window, u32* __restrict__ fstart) {
+    u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    if (k >= *n_live) { fstart[k] = 0; return; }
+    if (head[k]) { fstart[k] = 1; return; }
+    long long base = S[gfirst[gscan[k] - 1]];
+    fstart[k] = (unsigned long long)(S[k] - base) / window != (unsigned long long)(S[k - 1] - base) / window;
+}
+
+__device__ __forceinline__ void ck_rb_put_header(u8* __restrict__ f, unsigned long long total, u32 n, long long base_offset, long long ts) {
+    ck_put_be64(f, (unsigned long long)base_offset);
+    ck_put_be32(f + 8, (u32)(total - 12));
+    ck_put_be32(f + 12, 0);                                  // partitionLeaderEpoch
+    f[16] = 2;
+    ck_put_be32(f + 17, 0);                                  // crc: folded in last
+    f[21] = 0; f[22] = 0;                                    // attributes: no compression, CreateTime
+    ck_put_be32(f + 23, n - 1);                              // lastOffsetDelta
+    ck_put_be64(f + 27, (unsigned long long)ts);
+    ck_put_be64(f + 35, (unsigned long long)ts);
+    ck_put_be64(f + 43, ~0ull);                              // producerId -1
+    f[51] = 0xff; f[52] = 0xff;                              // producerEpoch -1
+    ck_put_be32(f + 53, 0xffffffffu);                        // baseSequence -1
+    ck_put_be32(f + 57, n);
+}
+// thread per frame (F = exclusive scan of the frame starts, R = of the exact sizes; both n + 1 long).  A frame that does not
+// fit the buffer is listed but not written: the size query reports the overflow
+__global__ void __launch_bounds__(256)
+ck_fr_table_kernel(const u32* __restrict__ order, const ck_fitem* __restrict__ items, const u32* __restrict__ ffirst,
+                   const long long* __restrict__ F, const long long* __restrict__ R, u32 n, const u32* __restrict__ n_live,
+                   long long base_offset, long long ts, unsigned long long cap, ck_frame_ent* __restrict__ table, u8* __restrict__ frames,
+                   u32* __restrict__ chunks) {
+    u32 f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    u32 nf = (u32)F[n];
+    if (f >= nf) { chunks[f] = 0; return; }
+    u32 a = ffirst[f], b = f + 1 < nf ? ffirst[f + 1] : *n_live;
+    ck_frame_ent e;
+    const ck_fitem& it = items[ck_fr_src(order, a)];
+    e.topic_id = it.topic_id; e.partition = it.partition; e.n_records = b - a; e.first = a;
+    e.offset = R[a] + (long long)CK_RB_HEADER * f; e.length = CK_RB_HEADER + R[b] - R[a];
+    table[f] = e;
+    bool fits = (unsigned long long)(e.offset + e.length) <= cap;
+    chunks[f] = fits ? (u32)((e.length - CK_RB_CRC_FROM + CK_RB_CRC_CHUNK - 1) / CK_RB_CRC_CHUNK) : 0u;
+    if (fits) ck_rb_put_header(frames + e.offset, (unsigned long long)e.length, b - a, base_offset, ts);
+}
+
+// key / header value: JSON string content written unescaped (warp copy when it holds no escape)
+__device__ __forceinline__ void ck_fr_put_str(u8* __restrict__ d, const u8* __restrict__ src, u32 raw, u32 len, u32 lane) {
+    if (raw == len) { for (u32 b = lane; b < len; b += 32) d[b] = src[b]; return; }
+    if (lane == 0) { GRd r; r.init(src, raw); u32 o = 0; for (u32 q = 0; q < raw;) d[o++] = (u8)ck_key_byte(r, q); }
+}
+// warp per record: every lane computes the same layout, lane 0 writes the small pieces, the warp copies key / value / id
+__global__ void __launch_bounds__(256)
+ck_fr_write_kernel(const u32* __restrict__ order, const ck_fitem* __restrict__ items, const u32* __restrict__ fstart,
+                   const long long* __restrict__ F, const u32* __restrict__ ffirst, const long long* __restrict__ R, u32 n,
+                   const u32* __restrict__ n_live, unsigned long long cap, u8* __restrict__ frames) {
+    u32 k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (k >= n || k >= *n_live) return;
+    u32 f = (u32)(F[k] + fstart[k]) - 1, a = ffirst[f];
+    unsigned long long at = (unsigned long long)R[a] + (unsigned long long)CK_RB_HEADER * (f + 1) + (unsigned long long)(R[k] - R[a]);
+    if (at + (unsigned long long)(R[k + 1] - R[k]) > cap) return;
+    const ck_fitem it = items[ck_fr_src(order, k)];
+    u32 rank = k - a;
+    u8* d = frames + at;
+    u32 pos = 0, kpos = 0, vpos = 0, cpos = 0;
     u8 tmp[10];
-    u32 m = ck_put_varint(tmp, r.body_len); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m;
+    u32 m = ck_put_varint(tmp, ck_rb_measure(it, rank)); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m;
     if (lane == 0) { d[pos] = 0; d[pos + 1] = 0; } pos += 2;                                  // attributes, timestampDelta = 0
-    m = ck_put_varint(tmp, k); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m;
-    if (p.has_key) { m = ck_put_varint(tmp, cl); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; kpos = pos; pos += cl; }
-    else { if (lane == 0) d[pos] = 1; pos += 1; }                                             // zig-zag(-1) = null key
-    m = ck_put_varint(tmp, r.val_len); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; vpos = pos; pos += r.val_len;
+    m = ck_put_varint(tmp, rank); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m;
+    if (it.key_len != CK_RB_NONE) {
+        m = ck_put_varint(tmp, it.key_len); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; kpos = pos; pos += it.key_len;
+    } else { if (lane == 0) d[pos] = 1; pos += 1; }                                            // zig-zag(-1) = null key
+    m = ck_put_varint(tmp, it.val_len); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; vpos = pos; pos += it.val_len;
+    bool has_corr = it.corr_len != CK_RB_NONE;
     if (lane == 0) {
-        d[pos] = 4;                                                                           // 2 headers
+        d[pos] = has_corr ? 4 : 2;                                                            // 2 headers (1 without an id)
         d[pos + 1] = 24; const char* a = "content-type"; for (u32 b = 0; b < 12; b++) d[pos + 2 + b] = (u8)a[b];
         d[pos + 14] = 32; const char* j = "application/json"; for (u32 b = 0; b < 16; b++) d[pos + 15 + b] = (u8)j[b];
-        d[pos + 31] = 28; const char* c = "correlation_id"; for (u32 b = 0; b < 14; b++) d[pos + 32 + b] = (u8)c[b];
+        if (has_corr) { d[pos + 31] = 28; const char* c = "correlation_id"; for (u32 b = 0; b < 14; b++) d[pos + 32 + b] = (u8)c[b]; }
     }
-    pos += 1 + CK_RB_CT_HDR + 15;
-    m = ck_put_varint(tmp, cl); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; cpos = pos;
-    if (p.has_key) for (u32 b = lane; b < cl; b += 32) d[kpos + b] = rec[co + b];
-    for (u32 b = lane; b < cl; b += 32) d[cpos + b] = rec[co + b];
-    ck_warp_copy(d + vpos, out + out_off[p.payload], r.val_len, lane);
+    pos += 1 + CK_RB_CT_HDR;
+    if (has_corr) {
+        pos += 15;
+        m = ck_put_varint(tmp, it.corr_len); if (lane == 0) for (u32 b = 0; b < m; b++) d[pos + b] = tmp[b]; pos += m; cpos = pos;
+        ck_fr_put_str(d + cpos, it.corr, it.corr_raw, it.corr_len, lane);
+    }
+    if (it.key_len != CK_RB_NONE) ck_fr_put_str(d + kpos, it.key, it.key_raw, it.key_len, lane);
+    ck_warp_copy(d + vpos, it.val, it.val_len, lane);
 }
 
-// frame header (everything but the crc), by one thread
-__global__ void ck_rb_header_kernel(u8* __restrict__ frame, const long long* __restrict__ rec_off, u32 n, long long base_offset,
-                                    long long timestamp_ms, long long* __restrict__ frame_len_out) {
-    if (threadIdx.x || blockIdx.x) return;
-    unsigned long long total = CK_RB_HEADER + (unsigned long long)rec_off[n];
-    ck_put_be64(frame, (unsigned long long)base_offset);
-    ck_put_be32(frame + 8, (u32)(total - 12));
-    ck_put_be32(frame + 12, 0);                              // partitionLeaderEpoch
-    frame[16] = 2;
-    frame[21] = 0; frame[22] = 0;                            // attributes: no compression, CreateTime
-    ck_put_be32(frame + 23, n - 1);                          // lastOffsetDelta
-    ck_put_be64(frame + 27, (unsigned long long)timestamp_ms);
-    ck_put_be64(frame + 35, (unsigned long long)timestamp_ms);
-    ck_put_be64(frame + 43, ~0ull);                          // producerId -1
-    frame[51] = 0xff; frame[52] = 0xff;                      // producerEpoch -1
-    ck_put_be32(frame + 53, 0xffffffffu);                    // baseSequence -1
-    ck_put_be32(frame + 57, n);
-    *frame_len_out = (long long)total;
-}
-
-// CRC32C of a large frame: one warp per 16 KB chunk of the covered bytes, then one warp folds the partials
-#define CK_RB_CRC_CHUNK 16384u
+// CRC32C of every frame: warps stride over the chunks of all frames (C = exclusive scan of the per-frame chunk counts)
 __global__ void __launch_bounds__(256)
-ck_rb_crc_chunks_kernel(const u8* __restrict__ frame, const long long* __restrict__ frame_len, u32* __restrict__ partial) {
+ck_fr_crc_chunks_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ C, const long long* __restrict__ F, u32 n,
+                        const u8* __restrict__ frames, u32* __restrict__ partial) {
     __shared__ u32 t[1024];
     ck_crc_tables(t);
-    u32 w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    unsigned long long covered = (unsigned long long)*frame_len - CK_RB_CRC_FROM;
-    unsigned long long start = (unsigned long long)w * CK_RB_CRC_CHUNK;
-    if (start >= covered) return;
-    u32 len = (u32)min((unsigned long long)CK_RB_CRC_CHUNK, covered - start);
-    u32 c = ck_crc32c_warp(t, frame + CK_RB_CRC_FROM + start, len, lane);
-    if (lane == 0) partial[w] = c;
+    u32 lane = threadIdx.x & 31, nw = (gridDim.x * blockDim.x) >> 5;
+    u32 nf = (u32)F[n];
+    unsigned long long total = (unsigned long long)C[n];
+    for (unsigned long long c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < total; c += nw) {
+        u32 lo = 0, hi = nf;                                   // last frame whose first chunk is <= c
+        while (hi - lo > 1) { u32 mid = (lo + hi) >> 1; if ((unsigned long long)C[mid] <= c) lo = mid; else hi = mid; }
+        ck_frame_ent e = table[lo];
+        unsigned long long start = (c - (unsigned long long)C[lo]) * CK_RB_CRC_CHUNK, covered = (unsigned long long)e.length - CK_RB_CRC_FROM;
+        u32 len = (u32)min((unsigned long long)CK_RB_CRC_CHUNK, covered - start);
+        u32 crc = ck_crc32c_warp(t, frames + e.offset + CK_RB_CRC_FROM + start, len, lane);
+        if (lane == 0) partial[c] = crc;
+    }
 }
-__global__ void ck_rb_crc_fold_kernel(u8* __restrict__ frame, const long long* __restrict__ frame_len, const u32* __restrict__ partial) {
-    if (blockIdx.x || threadIdx.x) return;
-    unsigned long long covered = (unsigned long long)*frame_len - CK_RB_CRC_FROM;
-    u32 nchunks = (u32)((covered + CK_RB_CRC_CHUNK - 1) / CK_RB_CRC_CHUNK);
+__global__ void __launch_bounds__(256)
+ck_fr_crc_fold_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ C, const long long* __restrict__ F, u32 n,
+                      const u32* __restrict__ partial, u8* __restrict__ frames) {
+    u32 f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n || f >= (u32)F[n]) return;
+    u32 c0 = (u32)C[f], nc = (u32)(C[f + 1] - C[f]);
+    if (!nc) return;
+    ck_frame_ent e = table[f];
+    unsigned long long covered = (unsigned long long)e.length - CK_RB_CRC_FROM;
     u32 xp = ck_gf_xpow8(CK_RB_CRC_CHUNK);
     u32 c = 0;                                               // crc of the empty prefix
-    for (u32 k = 0; k < nchunks; k++) {
+    for (u32 k = 0; k < nc; k++) {
         unsigned long long start = (unsigned long long)k * CK_RB_CRC_CHUNK;
         u32 len = (u32)min((unsigned long long)CK_RB_CRC_CHUNK, covered - start);
-        c = ck_crc_combine(c, partial[k], len == CK_RB_CRC_CHUNK ? xp : ck_gf_xpow8(len));
+        c = ck_crc_combine(c, partial[c0 + k], len == CK_RB_CRC_CHUNK ? xp : ck_gf_xpow8(len));
     }
-    ck_put_be32(frame + 17, c);
+    ck_put_be32(frames + e.offset + 17, c);
 }
 
 #endif  // CK_KAFKA_CUH

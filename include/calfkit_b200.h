@@ -37,6 +37,15 @@ typedef struct {           /* one publish; mirrors struct ck_pub in csrc/ck_kern
     uint32_t pad;          /* FNV-1a of the topic name (set when the name was looked up): groups unregistered topics */
 } ck_publish;
 
+typedef struct {           /* one frame of a frame pass; mirrors struct ck_frame_ent in csrc/ck_kafka.cuh */
+    int32_t  topic_id;     /* registered topic id */
+    int32_t  partition;    /* -1: unkeyed records (the handler-return publish, worker/worker.py:52-53): the producer picks */
+    uint32_t n_records;
+    uint32_t first;        /* first record, counted in group order */
+    int64_t  offset;       /* into the frame bytes */
+    int64_t  length;       /* 12 + batchLength */
+} ck_frame;
+
 /* lifecycle ------------------------------------------------------------------------------------ */
 int  ck_create(int device, uint64_t max_in_bytes, uint64_t max_out_bytes, uint32_t max_records,
                uint32_t max_payloads /* >= max_records; fan-out needs records * (fanout + 1) */,
@@ -72,7 +81,9 @@ int  ck_submit_device(ck_handle* h, const uint8_t* dev_in, const int64_t* dev_of
 
 /* engine options.  option 1 (bucket): value != 0 -> every submitted batch is bucketed by record length (stable radix sort of
  * the record indices on the device) before the thread-per-record walk, so that the lanes of a warp walk records of one size
- * class; for topics with mixed sizes / shapes (reference analogue: none — the reference handles one record at a time) */
+ * class; for topics with mixed sizes / shapes (reference analogue: none — the reference handles one record at a time).
+ * option 2 (frame_bytes): the window W of the frame split of ck_encode_frames; a frame holds at most 61 + W + one record
+ * bytes (default 1 MiB) */
 int  ck_set_option(ck_handle* h, uint32_t option, uint64_t value);
 
 /* group the publish table of the current plan by destination topic on the device (stable two-pass radix sort over 12-bit
@@ -85,7 +96,8 @@ int  ck_fetch_groups(ck_handle* h, uint32_t* host_order, uint32_t* host_key_coun
 
 /* Kafka RecordBatch v2 framing on the device (reference: aiokafka under broker.subscriber / broker.publish,
  * calfkit/worker/worker.py:45-53, calfkit/nodes/base.py:82-87).  ck_submit_recordbatch takes a fetch response's record set
- * (concatenated v2 frames, uncompressed) as it came off the socket: one H2D copy, then CRC32C verification, record split and
+ * (concatenated v2 frames, uncompressed) as it came off the socket: one H2D copy (the frame index goes through page-locked
+ * staging the handle owns: nothing waits for the stream), then CRC32C verification, record split and
  * zig-zag varint field decode on the device; the walker reads each value where it lies.  Records of a frame that fails the
  * CRC / framing check get status 6 (bad frame); a truncated trailing frame is ignored.  *n_records = records decoded.
  * ck_fetch_rb_index: per record, where value / key / the `correlation_id` header lie in the submitted buffer (-1 = absent).
@@ -95,8 +107,33 @@ int  ck_fetch_groups(ck_handle* h, uint32_t* host_order, uint32_t* host_key_coun
 int  ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint32_t* n_records);
 int  ck_fetch_rb_index(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
                        int64_t* corr_off, int32_t* corr_len, uint32_t* bad);
+/* the same copies queued only (page-locked destinations, ck_sync before reading): the lanes bring the record index back
+ * with the step's results (Worker consuming fetch responses, worker/worker.py:45-53) */
+int  ck_fetch_rb_index_async(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,
+                             int64_t* corr_off, int32_t* corr_len, uint32_t* bad);
 int  ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uint32_t n, int64_t base_offset, int64_t timestamp_ms,
                            uint8_t* host_frame, uint64_t cap, uint64_t* frame_len);
+/* produce side for a whole step (reference: the producer aiokafka runs under broker.publish, nodes/base.py:82-87, and under the
+ * handler's publisher, worker/worker.py:52-53, accumulates one record batch per topic-partition).
+ *   ck_set_frame_topics       registered topic ids whose publishes are framed (replaces the previous set)
+ *   ck_encode_frames          every live publish of the current plan to a frame topic, grouped by (topic, partition) in a
+ *                             stable order (records keep their send order; unkeyed publishes form the group of partition -1
+ *                             of their topic), split into frames of at most 61 + frame_bytes + one record bytes (ck_set_option
+ *                             2, default 1 MiB; rule in DESIGN.md), encoded as ck_encode_recordbatch does with baseOffset 0
+ *                             and baseTimestamp timestamp_ms.  Queued only: nothing waits for the host.
+ *   ck_encode_frames_records  the same for n records a host path produced for one topic: blob + desc[n][6] = {value off, len,
+ *                             key off, len, correlation id off, len} (len -1: absent; key and id as JSON string content,
+ *                             unescaped on the device); partition = murmur2(key) % num_partitions as for the plan's publishes
+ *   ck_frames_size            frames and bytes of the last pass (waits; frames that did not fit the frame buffer are
+ *                             written again into a buffer grown to their size)
+ *   ck_fetch_frames_async     frame table and frame bytes of the last pass, queued into page-locked memory (ck_sync);
+ *                             ck_frames_size must have been called since the pass */
+int  ck_set_frame_topics(ck_handle* h, const int32_t* topic_ids, uint32_t n);
+int  ck_encode_frames(ck_handle* h, int64_t timestamp_ms);
+int  ck_encode_frames_records(ck_handle* h, int32_t topic_id, const uint8_t* host_blob, uint64_t nbytes, const int64_t* host_desc,
+                              uint32_t n, int64_t timestamp_ms);
+int  ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes);
+int  ck_fetch_frames_async(ck_handle* h, ck_frame* host_table, uint32_t table_cap, uint8_t* host_frames, uint64_t cap);
 
 /* tool node, host tools only: gather every record's tool-call `args` JSON into the output buffer
  * (payload i = args of record i, empty when the record does not reach the tool). */
@@ -218,7 +255,7 @@ int  ck_device_buffers2(ck_handle* h, void** pubs, void** pay_len, void** descs)
 int  ck_profile(ck_handle* h, int enable);         /* record (asynchronous) CUDA events around every kernel */
 int  ck_profile_read(ck_handle* h, float* ms /* CK_NUM_KERNELS */, uint32_t* launches /* CK_NUM_KERNELS */, int reset);
 
-enum { CK_K_WALK = 0, CK_K_PLAN, CK_K_SCAN, CK_K_EMIT, CK_K_ROUTE, CK_K_FANOUT, CK_K_CANON, CK_K_WALK_LONG, CK_K_WALK_ELEMS, CK_NUM_KERNELS };
+enum { CK_K_WALK = 0, CK_K_PLAN, CK_K_SCAN, CK_K_EMIT, CK_K_ROUTE, CK_K_FANOUT, CK_K_CANON, CK_K_WALK_LONG, CK_K_WALK_ELEMS, CK_K_FRAME, CK_NUM_KERNELS };
 
 #ifdef __cplusplus
 }
