@@ -21,7 +21,9 @@ Kafka's own granularity — record batches — at both ends:
   * `frame_sink(topic, fn)`: `fn(topic, partition_or_None, frame, n_records)` once per produce-ready RecordBatch v2 frame.
     A lane's frames are handed out as they are; per-record Records produced to such a topic are collected and framed by
     the engine's record form at `flush_frames` (the Worker calls it once per step and installs the `framer`).  There is no
-    CPU encoder: without a framer, flushing them fails loudly.
+    CPU encoder: without a framer, flushing them fails loudly.  `MemoryBroker(compression_type="lz4")` (the keyword a
+    FastStream KafkaBroker takes) makes every frame an LZ4-compressed batch, compressed on the device; other codecs are
+    refused by the Worker when frame sinks are registered.
 Publishes to topics nobody subscribes to are counted and dropped when they arrive batch-wise (a long-running worker must
 not grow without bound); per-record publishes are kept (tests read such topics afterwards).
 Limitation (documented, not hidden): one shared queue per topic — consumer GROUPS are not modelled (two subscriptions to
@@ -72,6 +74,9 @@ class _HandlerRef:
 class MemoryBroker:
     def __init__(self, *servers: Any, middlewares: list | None = None, num_partitions: int = 8, **kwargs: Any):
         self.servers, self.kwargs = servers, kwargs
+        # the codec of the frames handed to frame sinks, as KafkaBroker(compression_type=...) takes it: None or "lz4"
+        # (compressed on the device); the Worker refuses any other codec when frame sinks are registered
+        self.compression_type: str | None = kwargs.get("compression_type")
         self.num_partitions = num_partitions       # partitions per topic (Kafka's default partitioner: murmur2(key) % partitions)
         self._connection: Any = None
         self.queues: dict[str, deque[Record]] = defaultdict(deque)
@@ -101,7 +106,9 @@ class MemoryBroker:
     def frame_sink(self, topic: str, fn) -> None:
         """Kafka-shaped consumer of one topic: fn(topic, partition or None, frame, n_records) is called once per
         RecordBatch v2 frame built on the device (partition None: unkeyed records, the producer client picks one).  The
-        frame (uint8 array) is valid during the call, like `sink`'s batch."""
+        frame (uint8 array) is valid during the call, like `sink`'s batch.  With compression_type="lz4" every frame is an
+        LZ4-compressed batch (attributes 3) as Kafka clients decode it; the table's records count stays the uncompressed
+        one."""
         self.frame_sinks[topic] = fn
 
     def publisher(self, topic: str, **kwargs: Any):

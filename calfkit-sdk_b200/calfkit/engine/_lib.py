@@ -30,7 +30,7 @@ COLS = ["STATUS", "ACTION", "ERR", "CORR_OFF", "CORR_LEN", "NFRAMES", "FRAMES_OF
 COL = {name: i for i, name in enumerate(COLS)}
 NUM_COLS = len(COLS)
 
-KERNELS = ["walk", "plan", "scan", "emit", "route", "fanout", "canon", "walk_long", "walk_elems", "frame"]
+KERNELS = ["walk", "plan", "scan", "emit", "route", "fanout", "canon", "walk_long", "walk_elems", "frame", "lz4"]
 NUM_KERNELS = len(KERNELS)
 
 PUB_DTYPE = np.dtype([("payload", "<u4"), ("topic_id", "<i4"), ("topic_off", "<u4"), ("topic_len", "<u4"),

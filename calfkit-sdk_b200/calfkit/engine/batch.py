@@ -21,6 +21,9 @@ from calfkit.engine import _lib
 from calfkit.engine._lib import COL, FRAME_DTYPE, NUM_COLS, PUB_DTYPE, ptr
 from calfkit.exceptions import EngineError
 
+# frame codecs the device builds, by the name Kafka clients use (KafkaBroker(compression_type=...)) -> Kafka's codec id
+FRAME_CODECS = {None: 0, "lz4": 3}
+
 
 @dataclass
 class ToolTemplate:
@@ -368,6 +371,13 @@ class BatchEngine:
     def set_frame_bytes(self, window: int) -> None:
         """the frame split window W: a frame holds at most 61 + W + one record bytes (default 1 MiB)"""
         self._check(self.lib.ck_set_option(self.h, 2, window))
+
+    def set_frame_compression(self, codec: str | None) -> None:
+        """the codec of the frames the frame passes build: None (uncompressed, the default) or "lz4" (Kafka codec 3: the
+        records section of every frame is one LZ4 frame of independent 64 KB blocks, compressed on the device)"""
+        if codec not in FRAME_CODECS:
+            raise EngineError(f"frame compression {codec!r} is not supported (None or 'lz4')")
+        self._check(self.lib.ck_set_option(self.h, 3, FRAME_CODECS[codec]))
 
     def encode_frames(self, timestamp_ms: int) -> None:
         """queue the frame pass over the current plan: every live publish to a frame topic, grouped by (topic, partition)

@@ -26,6 +26,7 @@ import numpy as np
 from calfkit.broker import Record
 from calfkit.client import Client
 from calfkit.engine import BatchEngine
+from calfkit.engine.batch import FRAME_CODECS
 from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_UNSUPPORTED, STATUS_NAMES
 from calfkit.exceptions import EngineError
 from calfkit.engine.lane import LanePipeline, PublishBatch
@@ -121,12 +122,14 @@ class Worker:
             # frame-sink topics get ids like route_topics, so that their publishes can be framed on the device
             frame_topics = list(self._client._connection.frame_sinks)
             topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics + frame_topics
+            codec = self._frame_codec() if frame_topics else None
 
             def configure(eng: BatchEngine) -> None:
                 eng.register_topics(topics, num_partitions=getattr(self._client._connection, "num_partitions", 0))
                 node.configure_engine(eng)
                 if frame_topics:
                     eng.set_frame_topics(frame_topics)
+                    eng.set_frame_compression(codec)
             pipe = LanePipeline(self._device, configure, lanes=self._lanes, max_records=self._batch_records,
                                 max_in_bytes=self._batch_bytes, exchange=(self._rank, self._world) if self._world > 1 else None)
             self._pipes[id(node)] = pipe
@@ -174,6 +177,13 @@ class Worker:
             self._run_host(node, records[:mid], **kw)
             self._run_host(node, records[mid:], **kw)
 
+    def _frame_codec(self) -> str | None:
+        """the broker's compression_type for the frames built on the device: None or "lz4"; any other codec is refused"""
+        codec = getattr(self._client._connection, "compression_type", None)
+        if codec not in FRAME_CODECS:
+            raise EngineError(f"frame sinks: compression_type {codec!r} is not built on the device (None or 'lz4')")
+        return codec
+
     def _frame_records(self, topic: str, records: list[Record]):
         """the engine's record form over Records produced to a frame-sink topic by host paths, in engine-sized chunks"""
         broker = self._client._connection
@@ -181,6 +191,7 @@ class Worker:
             from calfkit.engine.lane import PinnedPool
             self._framer_eng = BatchEngine(self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes)
             self._framer_eng.register_topics(list(broker.frame_sinks), num_partitions=getattr(broker, "num_partitions", 0))
+            self._framer_eng.set_frame_compression(self._frame_codec())
             self._frame_pool = PinnedPool()
         eng, ts = self._framer_eng, int(time.time() * 1000)
         if topic not in eng.topic_ids:

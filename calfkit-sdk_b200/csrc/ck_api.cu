@@ -60,6 +60,11 @@ struct ck_handle {
     u8* d_fr_blob = nullptr; long long* d_fr_desc = nullptr; long long* h_fr_info = nullptr;   // h_fr_info: pinned {frames, bytes}
     int32_t* d_fr_slot = nullptr; u32 fr_nslots = 0, fr_ntopics = 0;
     uint64_t fr_window = 1ull << 20;                 // frame_bytes (ck_set_option 2)
+    // LZ4 frames (ck_set_option 3; allocated on the first compressed pass): the uncompressed frames, then the block slots,
+    // each fr_raw_cap bytes; per block slot its size and their scan; the offsets of the compressed frames
+    u32 fr_codec = 0, fr_pass_codec = 0;             // option 3, and the codec of the last pass
+    u8* d_fr_raw = nullptr; uint64_t fr_raw_cap = 0; u32 fr_bmax = 0; u32* d_fr_bsize = nullptr;
+    long long *d_fr_bscan = nullptr, *d_fr_zoff = nullptr; unsigned long long* d_fr_btile = nullptr;
     // exchange planning (allocated on first use)
     u32* d_x_hist = nullptr; long long* d_x_base = nullptr; unsigned long long* d_x_nbytes = nullptr;
     long long *d_x_src_off = nullptr, *d_x_len = nullptr, *d_x_dst_off = nullptr; u32 *d_x_len32 = nullptr, *d_x_pub = nullptr;
@@ -193,7 +198,8 @@ extern "C" void ck_destroy(ck_handle* h) {
                      h->d_rb_rec_batch, h->d_rb_val_len, h->d_rb_rec_bad, h->d_rb_key_len, h->d_rb_corr_len,
                      h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
                      h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
-                     h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2};
+                     h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
+                     h->d_fr_zoff, h->d_fr_btile};
     for (void* p : gptrs) if (p) cudaFree(p);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
     if (h->d_recv) cudaFree(h->d_recv);
@@ -659,6 +665,10 @@ extern "C" int ck_group_publishes(ck_handle* h) {
 extern "C" int ck_set_option(ck_handle* h, uint32_t option, uint64_t value) {
     if (option == 1) { h->opt_bucket = value != 0; return 0; }
     if (option == 2) { if (value < 1) return fail(h, "ck_set_option: frame_bytes must be at least 1"); h->fr_window = value; return 0; }
+    if (option == 3) {
+        if (value != 0 && value != 3) return fail(h, "ck_set_option: frame codec must be 0 (none) or 3 (lz4)");
+        h->fr_codec = (u32)value; return 0;
+    }
     return fail(h, "ck_set_option: unknown option");
 }
 
@@ -778,6 +788,21 @@ static int fr_grow(ck_handle* h, uint64_t cap) {
     h->fr_cap = cap;
     return 0;
 }
+// the scratch of the LZ4 stage, sized for uncompressed frames of `cap` bytes: those frames, the block slots (a block's
+// compressed bytes lie at its own offset, and are never longer), and a size per 64 KB block slot
+static int lz_grow(ck_handle* h, uint64_t cap) {
+    if (h->d_fr_raw) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_fr_raw); cudaFree(h->d_fr_bsize); cudaFree(h->d_fr_bscan); cudaFree(h->d_fr_btile); }
+    h->d_fr_raw = nullptr; h->d_fr_bsize = nullptr; h->d_fr_bscan = nullptr; h->d_fr_btile = nullptr; h->fr_raw_cap = 0;
+    uint64_t bmax = cap / CK_LZ_BLOCK + (uint64_t)h->fr_max + 2;
+    if (bmax > 0xffffffffull) return fail(h, "lz_grow: more than 2^32 LZ4 blocks");
+    if (!h->d_fr_zoff) CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_zoff, sizeof(long long) * ((size_t)h->fr_max + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_raw, 2 * (cap + CK_PAD)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_bsize, sizeof(u32) * bmax));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_bscan, sizeof(long long) * (bmax + 1)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_btile, sizeof(unsigned long long) * (bmax / CK_SCAN_TILE + 2)));
+    h->fr_raw_cap = cap; h->fr_bmax = (u32)bmax;
+    return 0;
+}
 static int fr_alloc(ck_handle* h) {
     if (h->d_fr_items) return 0;
     size_t m = (size_t)h->max_pubs;
@@ -800,7 +825,7 @@ static int fr_alloc(ck_handle* h) {
     CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_table, sizeof(ck_frame_ent) * m));
     CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o1, sizeof(u32) * (m + 1)));
     CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o2, sizeof(u32) * (m + 1)));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_fr_info, sizeof(long long) * 2));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_fr_info, sizeof(long long) * 3));
     // first size of the frame buffer: every payload framed twice (a payload slot carries at most two publishes) plus the
     // record and frame overhead of a publish with an id of up to 40 bytes.  A pass that needs more grows it (ck_frames_size)
     return fr_grow(h, 2 * h->max_out + 160ull * m + 4096);
@@ -809,9 +834,11 @@ static int fr_alloc(ck_handle* h) {
 // group -> split -> size -> table + headers -> write -> CRC over items[0..n) that a source kernel built (gkey: group keys of
 // 6 * passes bits, all ones = not framed; passes 0: one group in the given order).  Queued only.
 static int frame_write(ck_handle* h);
+static int lz_compress(ck_handle* h);
 static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long long window, long long base_offset, long long ts) {
-    h->fr_n = n; h->fr_info = false; h->fr_sized = false;
+    h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec;
     if (!n) return 0;
+    if (h->fr_pass_codec && !h->d_fr_raw && lz_grow(h, h->fr_cap)) return 1;
     const u32* order = nullptr;
     if (passes) {
         if (group_alloc(h)) return 1;
@@ -857,26 +884,74 @@ static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long l
 }
 
 // the half of the pass that writes into the frame buffer: table + headers, records, CRC.  Everything it reads stays on the
-// device until the next pass, so it runs again into a larger buffer when the frames did not fit
+// device until the next pass, so it runs again into a larger buffer when the frames did not fit.  An LZ4 pass writes the
+// uncompressed frames into the scratch buffer and compresses them into the frame buffer before the CRC
 static int frame_write(ck_handle* h) {
     u32 n = h->fr_n, nb = (n + 255) / 256;
     const u32* order = h->fr_order;
+    bool lz = h->fr_pass_codec != 0;
+    u8* dst = lz ? h->d_fr_raw : h->d_fr_frames;
+    uint64_t cap = lz ? h->fr_raw_cap : h->fr_cap;
     {
         KTimer t(h, CK_K_FRAME);   // chunk counts per frame go to d_fr_head (free again), their scan to d_fr_S
         CKL(h) ck_fr_table_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_ffirst, h->d_fr_F, h->d_fr_R, n, h->d_fr_nlive,
-                                                          h->fr_base, h->fr_ts, h->fr_cap, h->d_fr_table, h->d_fr_frames, h->d_fr_head);
+                                                          h->fr_base, h->fr_ts, cap, h->d_fr_table, dst, h->d_fr_head);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
+    if (!lz && run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
         CKL(h) ck_fr_write_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_fstart, h->d_fr_F, h->d_fr_ffirst, h->d_fr_R, n,
-                                                                   h->d_fr_nlive, h->fr_cap, h->d_fr_frames);
+                                                                   h->d_fr_nlive, cap, dst);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (lz && lz_compress(h)) return 1;
+    {
+        KTimer t(h, CK_K_FRAME);
         u32 cblocks = (n + 7) / 8; if (cblocks > h->num_sms * 8) cblocks = h->num_sms * 8;
         CKL(h) ck_fr_crc_chunks_kernel<<<cblocks, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_frames, h->d_fr_partial);
         CKL(h) ck_fr_crc_fold_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_partial, h->d_fr_frames);
         CUDA_TRY(h, cudaGetLastError());
     }
+    return 0;
+}
+
+// the LZ4 stage (csrc/ck_kafka.cuh): the uncompressed frames in d_fr_raw -> compressed frames in the frame buffer, their
+// table entries and CRC chunk counts (scan in d_fr_S); h_fr_info[2] = bytes of the compressed frames.  Block scan in
+// d_fr_gscan and frame lengths in d_fr_size: the first half of the pass is done with both
+static int lz_compress(ck_handle* h) {
+    u32 n = h->fr_n, nb = (n + 255) / 256;
+    u8* slots = h->d_fr_raw + h->fr_raw_cap + CK_PAD;
+    {
+        KTimer t(h, CK_K_LZ4);
+        CKL(h) ck_lz_blocks_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_F, n, h->fr_raw_cap, h->d_fr_head);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_head, n, h->d_fr_gscan, 0, h->d_fr_tile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    {
+        KTimer t(h, CK_K_LZ4);
+        u32 blocks = h->num_sms * 8;
+        CKL(h) ck_lz_compress_kernel<<<blocks, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table, h->d_fr_gscan, h->d_fr_F, n, h->d_fr_raw, slots,
+                                                                              h->fr_bmax, h->d_fr_bsize);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_bsize, h->fr_bmax, h->d_fr_bscan, 0, h->d_fr_btile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    {
+        KTimer t(h, CK_K_LZ4);
+        CKL(h) ck_lz_size_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_gscan, h->d_fr_bscan, n, h->d_fr_size);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_size, n, h->d_fr_zoff, 0, h->d_fr_tile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    {
+        KTimer t(h, CK_K_LZ4);
+        CKL(h) ck_lz_gather_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_gscan, h->d_fr_F, n, h->d_fr_bscan, h->d_fr_bsize,
+                                                                         h->d_fr_zoff, h->d_fr_size, h->d_fr_raw, slots, h->fr_cap, h->d_fr_frames);
+        CKL(h) ck_lz_head_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_F, n, h->d_fr_zoff, h->d_fr_size, h->d_fr_raw, h->fr_cap,
+                                                           h->d_fr_frames, h->d_fr_head);
+        CUDA_TRY(h, cudaGetLastError());
+    }
+    if (run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info + 2, h->d_fr_zoff + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 
@@ -949,19 +1024,28 @@ extern "C" int ck_encode_frames_records(ck_handle* h, int32_t topic_id, const ui
     return frame_pass(h, n, passes, (u32)((1ull << (6 * passes)) - 1), h->fr_window, 0, timestamp_ms);
 }
 
-// frames and bytes of the last pass (waits for it).  Frames that did not fit the frame buffer are written again into a
-// buffer grown to their size (one more wait): a step is sized for whatever its ids and payloads need
+// bytes of the last pass's frames: uncompressed (as the table kernel lays them out) and as they go out
+static uint64_t fr_raw_bytes(ck_handle* h) { return h->fr_info ? (uint64_t)(h->h_fr_info[1] + (long long)CK_RB_HEADER * h->h_fr_info[0]) : 0; }
+static uint64_t fr_bytes(ck_handle* h) { return !h->fr_info ? 0 : h->fr_pass_codec ? (uint64_t)h->h_fr_info[2] : fr_raw_bytes(h); }
+
+// frames and bytes of the last pass (waits for it).  Frames that did not fit the frame buffer (or, compressed, the scratch
+// buffer of the uncompressed frames) are written again into buffers grown to their size (one more wait each): a step is
+// sized for whatever its ids and payloads need
 extern "C" int ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes) {
     cudaSetDevice(h->device);
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    long long nf = h->fr_info ? h->h_fr_info[0] : 0, nb = h->fr_info ? h->h_fr_info[1] + (long long)CK_RB_HEADER * nf : 0;
-    if ((uint64_t)nb > h->fr_cap) {
-        if (fr_grow(h, (uint64_t)nb + (uint64_t)nb / 8 + 4096) || frame_write(h)) return 1;
+    for (;;) {
+        uint64_t raw = fr_raw_bytes(h), nb = fr_bytes(h);
+        bool grow_raw = h->fr_pass_codec && raw > h->fr_raw_cap, grow = nb > h->fr_cap;
+        if (!grow_raw && !grow) break;
+        if (grow_raw && lz_grow(h, raw + raw / 8 + 4096)) return 1;
+        if (grow && fr_grow(h, nb + nb / 8 + 4096)) return 1;
+        if (frame_write(h)) return 1;
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     }
     h->fr_sized = true;
-    if (n_frames) *n_frames = (u32)nf;
-    if (nbytes) *nbytes = (uint64_t)nb;
+    if (n_frames) *n_frames = h->fr_info ? (u32)h->h_fr_info[0] : 0u;
+    if (nbytes) *nbytes = fr_bytes(h);
     return 0;
 }
 
@@ -970,9 +1054,9 @@ extern "C" int ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes
 extern "C" int ck_fetch_frames_async(ck_handle* h, ck_frame* host_table, uint32_t table_cap, uint8_t* host_frames, uint64_t cap) {
     cudaSetDevice(h->device);
     if (h->fr_info && !h->fr_sized) return fail(h, "ck_fetch_frames_async: call ck_frames_size after the frame pass first");
-    long long nf = h->fr_info ? h->h_fr_info[0] : 0, nb = h->fr_info ? h->h_fr_info[1] + (long long)CK_RB_HEADER * nf : 0;
-    if ((uint64_t)nb > h->fr_cap) return fail(h, "ck_fetch_frames_async: frames larger than the frame buffer");
-    if ((uint64_t)nf > table_cap || (uint64_t)nb > cap) return fail(h, "ck_fetch_frames_async: host buffers too small");
+    uint64_t nf = h->fr_info ? (uint64_t)h->h_fr_info[0] : 0, nb = fr_bytes(h);
+    if (nb > h->fr_cap) return fail(h, "ck_fetch_frames_async: frames larger than the frame buffer");
+    if (nf > table_cap || nb > cap) return fail(h, "ck_fetch_frames_async: host buffers too small");
     if (nf) CUDA_TRY(h, cudaMemcpyAsync(host_table, h->d_fr_table, sizeof(ck_frame) * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
     if (nb) CUDA_TRY(h, cudaMemcpyAsync(host_frames, h->d_fr_frames, (size_t)nb, cudaMemcpyDeviceToHost, h->stream));
     return 0;

@@ -465,4 +465,115 @@ ck_fr_crc_fold_kernel(const ck_frame_ent* __restrict__ table, const long long* _
     ck_put_be32(frames + e.offset + 17, c);
 }
 
+// ---- LZ4 compression of the frames (ck_set_option 3 = 3) ------------------------------------------------------------------
+// With the option on, the table and write kernels above build the uncompressed frames in a scratch buffer, and this stage
+// turns each into a batch with attributes 3 (LZ4): header | 7-byte LZ4 frame header | blocks | end mark 00000000, where
+// the records section [61, end) of the uncompressed frame is cut into independent blocks of 64 KB (the last one shorter):
+//   blocks   thread per frame: block count; its scan gives every frame its first block
+//   lz4      warp per block (ck_lz4_block): compressed bytes into a slot at the block's own offset in a second scratch
+//            region, or none when they would not be smaller (the block is then stored raw, bit 31 of its size set)
+//   size     block sizes -> scan; frame lengths -> scan -> offsets of the compressed frames
+//   gather   warp per block: size word + bytes into the frame buffer; then thread per frame: header (attributes 3,
+//            batchLength), LZ4 frame header, end mark, the frame table's offset / length and the CRC chunk count
+// The CRC kernels above then run over the compressed frames.
+// LZ4 frame descriptor as liblz4's LZ4F_compressFrame writes it with default preferences: magic 0x184D2204, FLG 0x60
+// (version 01, independent blocks, no checksums, no content size), BD 0x40 (64 KB blocks), HC = (xxh32(FLG BD) >> 8) & 0xFF
+#include "ck_lz4.cuh"
+#define CK_LZ_FRAME_HDR 7u
+#define CK_LZ_OVERHEAD (CK_LZ_FRAME_HDR + 4u)   // frame header + end mark
+
+// frame holding block b: the last frame whose first block is <= b (B = exclusive scan of the block counts)
+__device__ __forceinline__ u32 ck_lz_frame_of(const long long* __restrict__ B, u32 nf, unsigned long long b) {
+    u32 lo = 0, hi = nf;
+    while (hi - lo > 1) { u32 mid = (lo + hi) >> 1; if ((unsigned long long)B[mid] <= b) lo = mid; else hi = mid; }
+    return lo;
+}
+// thread per frame of the uncompressed frames (raw_cap: their buffer; frames that did not fit it get no block)
+__global__ void __launch_bounds__(256)
+ck_lz_blocks_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ F, u32 n, unsigned long long raw_cap,
+                    u32* __restrict__ nblk) {
+    u32 f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    u32 k = 0;
+    if (f < (u32)F[n]) {
+        ck_frame_ent e = table[f];
+        if ((unsigned long long)(e.offset + e.length) <= raw_cap) k = (u32)((e.length - CK_RB_HEADER + CK_LZ_BLOCK - 1) / CK_LZ_BLOCK);
+    }
+    nblk[f] = k;
+}
+// warps stride over the block slots 0 .. bmax: bsize[b] = 4 + bytes of block b as it goes out (0 past the last block)
+__global__ void __launch_bounds__(CK_LZ_WARPS * 32)
+ck_lz_compress_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B, const long long* __restrict__ F, u32 n,
+                      const u8* __restrict__ raw, u8* __restrict__ slots, u32 bmax, u32* __restrict__ bsize) {
+    __shared__ uint16_t tabs[CK_LZ_WARPS][1u << CK_LZ_HBITS];
+    u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = gridDim.x * CK_LZ_WARPS;
+    u32 nf = (u32)F[n];
+    unsigned long long total = (unsigned long long)B[n];
+    for (u32 b = blockIdx.x * CK_LZ_WARPS + wid; b < bmax; b += nw) {
+        if (b >= total) { if (lane == 0) bsize[b] = 0; continue; }
+        u32 f = ck_lz_frame_of(B, nf, b);
+        ck_frame_ent e = table[f];
+        unsigned long long at = (unsigned long long)e.offset + CK_RB_HEADER + (b - (unsigned long long)B[f]) * CK_LZ_BLOCK;
+        u32 len = (u32)min((unsigned long long)CK_LZ_BLOCK, (unsigned long long)(e.offset + e.length) - at);
+        u32 z = ck_lz4_block(raw + at, len, slots + at, tabs[wid], lane);
+        if (lane == 0) bsize[b] = 4u + (z ? z : len);
+    }
+}
+// thread per frame: compressed length (0: the frame has no blocks, it did not fit the scratch buffer); S = scan of bsize
+__global__ void __launch_bounds__(256)
+ck_lz_size_kernel(const long long* __restrict__ B, const long long* __restrict__ S, u32 n, u32* __restrict__ clen) {
+    u32 f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    clen[f] = B[f + 1] > B[f] ? CK_RB_HEADER + CK_LZ_OVERHEAD + (u32)(S[B[f + 1]] - S[B[f]]) : 0u;
+}
+// warp per block: its size word and bytes at their place in the compressed frame (Z = scan of clen)
+__global__ void __launch_bounds__(256)
+ck_lz_gather_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B, const long long* __restrict__ F, u32 n,
+                    const long long* __restrict__ S, const u32* __restrict__ bsize, const long long* __restrict__ Z,
+                    const u32* __restrict__ clen, const u8* __restrict__ raw, const u8* __restrict__ slots, unsigned long long cap,
+                    u8* __restrict__ frames) {
+    u32 lane = threadIdx.x & 31, nw = (gridDim.x * blockDim.x) >> 5;
+    u32 nf = (u32)F[n];
+    unsigned long long total = (unsigned long long)B[n];
+    for (unsigned long long b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < total; b += nw) {
+        u32 f = ck_lz_frame_of(B, nf, b);
+        if ((unsigned long long)Z[f] + clen[f] > cap) continue;
+        ck_frame_ent e = table[f];
+        unsigned long long at = (unsigned long long)e.offset + CK_RB_HEADER + (b - (unsigned long long)B[f]) * CK_LZ_BLOCK;
+        u32 len = (u32)min((unsigned long long)CK_LZ_BLOCK, (unsigned long long)(e.offset + e.length) - at);
+        u32 z = bsize[b] - 4u;
+        bool stored = z == len;
+        u8* d = frames + Z[f] + CK_RB_HEADER + CK_LZ_FRAME_HDR + (S[b] - S[B[f]]);
+        if (lane == 0) { u32 w = stored ? (z | 0x80000000u) : z; d[0] = (u8)w; d[1] = (u8)(w >> 8); d[2] = (u8)(w >> 16); d[3] = (u8)(w >> 24); }
+        ck_warp_copy(d + 4, (stored ? raw : slots) + at, z, lane);
+    }
+}
+// thread per frame: batch header (attributes 3, batchLength of the compressed frame), LZ4 frame header and end mark; the
+// table entry moves to the compressed frame; CRC chunk count as ck_fr_table_kernel gives it (0: not written)
+__global__ void __launch_bounds__(256)
+ck_lz_head_kernel(ck_frame_ent* __restrict__ table, const long long* __restrict__ F, u32 n, const long long* __restrict__ Z,
+                  const u32* __restrict__ clen, const u8* __restrict__ raw, unsigned long long cap, u8* __restrict__ frames,
+                  u32* __restrict__ chunks) {
+    u32 f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    if (f >= (u32)F[n]) { chunks[f] = 0; return; }
+    ck_frame_ent e = table[f];
+    u32 len = clen[f];
+    bool fits = len && (unsigned long long)Z[f] + len <= cap;
+    chunks[f] = fits ? (len - CK_RB_CRC_FROM + CK_RB_CRC_CHUNK - 1) / CK_RB_CRC_CHUNK : 0u;
+    if (fits) {
+        u8* d = frames + Z[f];
+        const u8* s = raw + e.offset;
+#pragma unroll 1
+        for (u32 i = 0; i < CK_RB_HEADER; i++) d[i] = s[i];
+        ck_put_be32(d + 8, len - 12u);
+        d[22] = 3;                                           // attributes: LZ4, CreateTime
+        ck_put_be32(d + CK_RB_HEADER, 0x04224D18u);          // magic 0x184D2204, little-endian
+        d[CK_RB_HEADER + 4] = 0x60; d[CK_RB_HEADER + 5] = 0x40; d[CK_RB_HEADER + 6] = 0x82;   // FLG, BD, HC
+        ck_put_be32(d + len - 4, 0u);
+    }
+    e.offset = Z[f]; e.length = len;
+    table[f] = e;
+}
+
 #endif  // CK_KAFKA_CUH

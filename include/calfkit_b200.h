@@ -83,7 +83,13 @@ int  ck_submit_device(ck_handle* h, const uint8_t* dev_in, const int64_t* dev_of
  * the record indices on the device) before the thread-per-record walk, so that the lanes of a warp walk records of one size
  * class; for topics with mixed sizes / shapes (reference analogue: none — the reference handles one record at a time).
  * option 2 (frame_bytes): the window W of the frame split of ck_encode_frames; a frame holds at most 61 + W + one record
- * bytes (default 1 MiB) */
+ * bytes (default 1 MiB)
+ * option 3 (frame codec): Kafka's compression codec id of the frames ck_encode_frames, ck_encode_frames_records and
+ * ck_encode_recordbatch build: 0 = none (default), 3 = LZ4; any other value is refused.  With LZ4 every frame is a batch with
+ * attributes 3 whose records section is one LZ4 frame (descriptor 04224D18 60 40 82: independent 64 KB blocks, no
+ * checksums), compressed on the device; a block that would not shrink is stored raw.  The split rule and the frame table
+ * keep their meaning (W applies to the uncompressed records); ck_frames_size, ck_fetch_frames_async and the frame table
+ * report the compressed frames, each at most its uncompressed length + 4 bytes per 64 KB block + 11 */
 int  ck_set_option(ck_handle* h, uint32_t option, uint64_t value);
 
 /* group the publish table of the current plan by destination topic on the device (stable two-pass radix sort over 12-bit
@@ -255,7 +261,7 @@ int  ck_device_buffers2(ck_handle* h, void** pubs, void** pay_len, void** descs)
 int  ck_profile(ck_handle* h, int enable);         /* record (asynchronous) CUDA events around every kernel */
 int  ck_profile_read(ck_handle* h, float* ms /* CK_NUM_KERNELS */, uint32_t* launches /* CK_NUM_KERNELS */, int reset);
 
-enum { CK_K_WALK = 0, CK_K_PLAN, CK_K_SCAN, CK_K_EMIT, CK_K_ROUTE, CK_K_FANOUT, CK_K_CANON, CK_K_WALK_LONG, CK_K_WALK_ELEMS, CK_K_FRAME, CK_NUM_KERNELS };
+enum { CK_K_WALK = 0, CK_K_PLAN, CK_K_SCAN, CK_K_EMIT, CK_K_ROUTE, CK_K_FANOUT, CK_K_CANON, CK_K_WALK_LONG, CK_K_WALK_ELEMS, CK_K_FRAME, CK_K_LZ4, CK_NUM_KERNELS };
 
 #ifdef __cplusplus
 }

@@ -1,10 +1,12 @@
 """Cost of the frame pass on a config-2 step (device-template tool node, 1M events), engine level.
 
-Two legs, alternating, two runs each:
-  sink    submit + plan + the copies a producer reads today (payload arena, offsets, lengths, publish table)
-  frames  the same + the frame pass over both output topics + the copy of the frames and their table
+Three legs, alternating, two runs each:
+  sink        submit + plan + the copies a producer reads today (payload arena, offsets, lengths, publish table)
+  frames      the same + the frame pass over both output topics + the copy of the frames and their table
+  frames_lz4  the same with LZ4 frames (ck_set_option 3 = 3): the frames are compressed on the device before the copy
 Per leg: step time (CUDA events around the whole step, copies included), the frame pass's kernel time (profile timer
-"frame"), events/s and D2H bytes per step.  Prints one JSON line with the card name and power limit read in the same run.
+"frame") and the compressor's ("lz4"), events/s, frame bytes and D2H bytes per step, and the compression ratio
+(uncompressed / compressed frame bytes).  Prints one JSON line with the card name and power limit read in the same run.
 
     python scripts/quick_frames.py [events]
 """
@@ -40,46 +42,51 @@ b_fr, b_tab = PinnedBuffer(2 * e.max_out + 160 * 2 * n), PinnedBuffer(FRAME_DTYP
 st = torch.cuda.ExternalStream(e.stream_ptr())
 
 
-def step(frames: bool) -> int:
+def step(frames: bool) -> tuple[int, int]:
     e.submit_device(d_in, d_off, n)
     e.tool_plan()
     if frames:
         e.encode_frames(1767225600000)
     nb, npay, npub = e.out_size()
     e._check(e.lib.ck_fetch_output_async(e.h, ptr(b_out.array), b_out.nbytes, ptr(b_off.array), ptr(b_len.array), ptr(b_pubs.array)))
-    d2h = nb + 8 * (npay + 1) + 4 * npay + PUB_DTYPE.itemsize * npub
+    d2h, fb = nb + 8 * (npay + 1) + 4 * npay + PUB_DTYPE.itemsize * npub, 0
     if frames:
         nf, fb = e.frames_size()
         e._check(e.lib.ck_fetch_frames_async(e.h, ptr(b_tab.array), 2 * n, ptr(b_fr.array), b_fr.nbytes))
         d2h += fb + FRAME_DTYPE.itemsize * nf
     e.sync()
-    return d2h
+    return d2h, fb
 
 
-def leg(frames: bool, steps: int = 5) -> dict:
+def leg(name: str, steps: int = 5) -> dict:
+    frames = name != "sink"
+    e.set_frame_compression("lz4" if name == "frames_lz4" else None)
     step(frames)
     e.profile(True)
     e.profile_read()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record(st)
     for _ in range(steps):
-        d2h = step(frames)
+        d2h, fb = step(frames)
     ev1.record(st)
     torch.cuda.synchronize()
     prof = e.profile_read()
     e.profile(False)
     ms = ev0.elapsed_time(ev1) / steps
-    return {"step_ms": round(ms, 3), "frame_kernel_ms": round(prof["frame"][0] / steps, 3), "events_per_s": round(n / ms * 1e3),
-            "d2h_bytes_per_step": d2h}
+    return {"step_ms": round(ms, 3), "frame_kernel_ms": round(prof["frame"][0] / steps, 3),
+            "lz4_kernel_ms": round(prof["lz4"][0] / steps, 3), "events_per_s": round(n / ms * 1e3),
+            "frame_bytes_per_step": fb, "d2h_bytes_per_step": d2h}
 
 
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
 res = {"events": n, "gpu": q.stdout.strip(), "runs": []}
 t0 = time.time()
 for _ in range(2):
-    for frames in (False, True):
-        res["runs"].append({"leg": "frames" if frames else "sink", **leg(frames)})
+    for name in ("sink", "frames", "frames_lz4"):
+        res["runs"].append({"leg": name, **leg(name)})
 res["wall_s"] = round(time.time() - t0, 1)
-nf, fb = e.frames_size()
-res["frames_per_step"], res["frame_bytes_per_step"] = nf, fb
+raw = next(r["frame_bytes_per_step"] for r in res["runs"] if r["leg"] == "frames")
+comp = next(r["frame_bytes_per_step"] for r in res["runs"] if r["leg"] == "frames_lz4")
+res["frames_per_step"] = e.frames_size()[0]
+res["compression_ratio"] = round(raw / comp, 2)
 print(json.dumps(res))
