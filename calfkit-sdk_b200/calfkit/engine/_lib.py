@@ -46,7 +46,7 @@ EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_registe
            "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_reset", "ck_submit_recordbatch",
            "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option",
            "ck_set_frame_topics", "ck_encode_frames", "ck_encode_frames_records", "ck_frames_size", "ck_fetch_frames_async",
-           "ck_fetch_rb_index_async"]
+           "ck_fetch_rb_index_async", "ck_fetch_rb_decoded_async"]
 
 _lib = None
 
@@ -107,6 +107,7 @@ def load() -> C.CDLL:
         "ck_submit_recordbatch": (C.c_int, [vp, u8p, C.c_uint64, C.POINTER(C.c_uint32)]),
         "ck_fetch_rb_index": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
         "ck_fetch_rb_index_async": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
+        "ck_fetch_rb_decoded_async": (C.c_int, [vp, u8p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
         "ck_encode_recordbatch": (C.c_int, [vp, u32p, C.c_uint32, C.c_int64, C.c_int64, u8p, C.c_uint64, C.POINTER(C.c_uint64)]),
         "ck_set_frame_topics": (C.c_int, [vp, i32p, C.c_uint32]),
         "ck_encode_frames": (C.c_int, [vp, C.c_int64]),

@@ -77,6 +77,25 @@ class _SpanOffsets:
         return len(self.off) + 1
 
 
+class FetchBytes:
+    """the bytes value offsets of a fetch response index: offsets below len(raw) lie in the raw response, offsets from
+    `base` on in the LZ4 batches' decoded records sections, `decoded` (ck_fetch_rb_decoded_async).  Sliced like an array"""
+    def __init__(self, raw: np.ndarray, base: int, decoded: np.ndarray):
+        self.raw, self.base, self.decoded = raw, int(base), decoded
+
+    def __getitem__(self, s: slice) -> np.ndarray:
+        a, b = int(s.start or 0), int(s.stop)
+        if a >= self.base:
+            return self.decoded[a - self.base:b - self.base]
+        if b > len(self.raw):
+            raise IndexError(f"span [{a}, {b}) runs past the raw bytes ({len(self.raw)}) and starts before the decoded ones ({self.base})")
+        return self.raw[a:b]
+
+    @property
+    def nbytes(self) -> int:
+        return int(self.raw.nbytes + self.decoded.nbytes)
+
+
 class BatchOutput:
     """Result of one plan+emit: unique payloads + the publish table that references them."""
 
@@ -211,7 +230,7 @@ class BatchEngine:
         self.topic_ids: dict[str, int] = {}
         self.num_partitions = 0
         self.n = 0
-        self._in_data = self._in_off = None
+        self._in_data = self._in_off = self._rb_raw = None
         self.frame_topics: list[str] = []
 
     # ------------------------------------------------------------------------------------------
@@ -326,26 +345,37 @@ class BatchEngine:
         self._check(self.lib.ck_submit(self.h, ptr(data), ptr(offsets), self.n))
 
     def submit_recordbatch(self, buf: np.ndarray) -> int:
-        """H2D + CRC32C check + record split + field decode + walk of a fetch response's record set (concatenated Kafka
-        RecordBatch v2 frames, uncompressed); returns the number of records.  Column spans are relative to each VALUE."""
+        """H2D + CRC32C check + (LZ4 batches) decode + record split + field decode + walk of a fetch response's record set
+        (concatenated Kafka RecordBatch v2 frames, uncompressed or LZ4); returns the number of records.  Column spans are
+        relative to each VALUE."""
         assert buf.dtype == np.uint8
         n = C.c_uint32(0)
         self._check(self.lib.ck_submit_recordbatch(self.h, ptr(buf), buf.nbytes, C.byref(n)))
         self.n = n.value
+        self._rb_raw = buf
         idx = self.rb_index()
-        # the host-side view of the batch for result decoding: record i = buf[val_off[i] : val_off[i] + val_len[i]]
-        self._in_data, self._in_off = buf, _SpanOffsets(idx["val_off"], idx["val_len"])
+        # the host-side view of the batch for result decoding: record i = data[val_off[i] : val_off[i] + val_len[i]]
+        self._in_data, self._in_off = idx["data"], _SpanOffsets(idx["val_off"], idx["val_len"])
         self._rb = idx
         return self.n
 
     def rb_index(self) -> dict[str, np.ndarray]:
-        """where value / key / the correlation_id header of every record lie in the submitted buffer (len -1 = absent)"""
+        """where value / key / the correlation_id header of every record lie (len -1 = absent), and under "data" the bytes
+        those offsets index: the submitted buffer, or a FetchBytes when the fetch held LZ4 batches"""
         n = self.n
         out = {"val_off": np.zeros(n, np.int64), "val_len": np.zeros(n, np.uint32), "key_off": np.zeros(n, np.int64),
                "key_len": np.zeros(n, np.int32), "corr_off": np.zeros(n, np.int64), "corr_len": np.zeros(n, np.int32),
                "bad": np.zeros(n, np.uint32)}
         if n:
             self._check(self.lib.ck_fetch_rb_index(self.h, *[ptr(out[k]) for k in ("val_off", "val_len", "key_off", "key_len", "corr_off", "corr_len", "bad")]))
+        base, nbytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.ck_fetch_rb_decoded_async(self.h, None, 0, C.byref(base), C.byref(nbytes)))
+        out["data"] = self._rb_raw
+        if nbytes.value:
+            dec = np.empty(nbytes.value, dtype=np.uint8)
+            self._check(self.lib.ck_fetch_rb_decoded_async(self.h, ptr(dec), dec.nbytes, None, None))
+            self.sync()
+            out["data"] = FetchBytes(self._rb_raw, base.value, dec)
         return out
 
     def encode_recordbatch(self, pub_indices: np.ndarray, base_offset: int = 0, timestamp_ms: int = 0) -> np.ndarray:

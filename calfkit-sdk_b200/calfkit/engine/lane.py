@@ -7,7 +7,7 @@ table).  No Python object is created per record anywhere on this path.
 
   Arena          inbound batch: pinned uint8 bytes + int64 offsets[n+1]
   FetchArena     inbound batch as a Kafka fetch response carries it: the record set (RecordBatch v2 frames) in one pinned
-                 buffer; CRC check, record split and field decode run on the device (ck_submit_recordbatch)
+                 buffer; CRC check, LZ4 decode, record split and field decode run on the device (ck_submit_recordbatch)
   PublishBatch   outbound batch: pinned payload arena + the ck_publish table; resolves topic names / keys lazily,
                  per topic, vectorised
   PinnedPool     recycles page-locked buffers (cudaHostAlloc costs milliseconds; the steady state allocates nothing)
@@ -26,7 +26,7 @@ import numpy as np
 
 from calfkit.engine import _lib
 from calfkit.engine._lib import COL, FRAME_DTYPE, PUB_DTYPE, ptr
-from calfkit.engine.batch import BatchEngine, Frames, ToolTemplate, _SpanOffsets
+from calfkit.engine.batch import BatchEngine, FetchBytes, Frames, ToolTemplate, _SpanOffsets
 from calfkit.exceptions import EngineError
 
 NO_PAYLOAD = 0xFFFFFFFF
@@ -179,9 +179,12 @@ class FetchArena:
 
 
 class FetchRecords:
-    """the records of a submitted FetchArena as the device split them: record i = its value, where it lies in the frame"""
-    def __init__(self, arena: FetchArena, val_off: np.ndarray, val_len: np.ndarray, bad: np.ndarray):
-        self.arena, self.data, self.offsets, self.bad = arena, arena.data, _SpanOffsets(val_off, val_len), bad
+    """the records of a submitted FetchArena as the device split them: record i = its value, where it lies in the frame —
+    in the arena, or for an LZ4 batch in its decoded records section (`decoded` = (value offset of decoded[0], decoded))"""
+    def __init__(self, arena: FetchArena, val_off: np.ndarray, val_len: np.ndarray, bad: np.ndarray,
+                 decoded: tuple[int, np.ndarray] | None = None):
+        data = arena.data if decoded is None else FetchBytes(arena.data, decoded[0], decoded[1])
+        self.arena, self.data, self.offsets, self.bad = arena, data, _SpanOffsets(val_off, val_len), bad
 
     @property
     def n(self) -> int:
@@ -387,13 +390,20 @@ class Lane:
         eng._check(eng.lib.ck_fetch_groups(eng.h, ptr(order), ptr(key_counts), 0))
         self._views = (b_out.array[:nb], off, ln, pubs, rows, order, key_counts)
         # a fetch response: where every record's value lies in it, and whether its frame failed the check
-        self._b_rb = self._rb = None
+        # (and, when it held LZ4 batches, their decoded records sections, which those offsets point into)
+        self._b_rb = self._rb = self._b_dec = self._dec = None
         if isinstance(self.arena, FetchArena):
             self._b_rb = b_rb = pool.take(16 * n + 64)
             val_off, val_len, bad = b_rb.view(np.int64, n), b_rb.view(np.uint32, n, 8 * n), b_rb.view(np.uint32, n, 12 * n)
             if n:
                 eng._check(eng.lib.ck_fetch_rb_index_async(eng.h, ptr(val_off), ptr(val_len), None, None, None, None, ptr(bad)))
             self._rb = (val_off, val_len, bad)
+            base, nbytes = C.c_uint64(0), C.c_uint64(0)
+            eng._check(eng.lib.ck_fetch_rb_decoded_async(eng.h, None, 0, C.byref(base), C.byref(nbytes)))
+            if nbytes.value:
+                self._b_dec = b_dec = pool.take(nbytes.value + 64)
+                eng._check(eng.lib.ck_fetch_rb_decoded_async(eng.h, ptr(b_dec.array), b_dec.nbytes, None, None))
+                self._dec = (base.value, b_dec.array[:nbytes.value])
         # the frame pass's frames and table (the stream was just synchronised for the sizes above)
         self._b_fr = self._fr = None
         if eng.frame_topics:
@@ -435,12 +445,17 @@ class Lane:
             self.d2h_bytes += int(frames.data.nbytes + frames.table.nbytes)
         if self._rb is not None:
             self.d2h_bytes += int(sum(a.nbytes for a in self._rb))
+        if self._dec is not None:
+            self.d2h_bytes += int(self._dec[1].nbytes)
         listed = C.c_uint32(0)
         eng._check(eng.lib.ck_canon_stats(eng.h, C.byref(listed), None))
         overlay = eng.overlay() if listed.value else None       # rare: some records arrived in a non-canonical spelling
         arena, self.arena, self.busy, self.collecting = self.arena, None, False, False
-        source = FetchRecords(arena, *self._rb) if self._rb is not None else arena
-        self._views = self._b_out = self._b_meta = self._b_fr = self._fr = self._b_rb = self._rb = None
+        source = FetchRecords(arena, *self._rb, decoded=self._dec) if self._rb is not None else arena
+        b_rb = (b_rb,) if b_rb is not None else ()
+        if self._b_dec is not None:
+            b_rb += (self._b_dec,)
+        self._views = self._b_out = self._b_meta = self._b_fr = self._fr = self._b_rb = self._rb = self._b_dec = self._dec = None
         self.received = []
         for meta, data, b_m, b_d in self._recv:
             self.received.append(received_batch(meta, data, eng.topic_names, on_release=lambda b_m=b_m, b_d=b_d: (pool.give(b_m), pool.give(b_d))))
@@ -449,7 +464,7 @@ class Lane:
         def done():
             pool.give(b_out)
             pool.give(b_meta)
-            for b in (b_fr or ()) + ((b_rb,) if b_rb is not None else ()):
+            for b in (b_fr or ()) + b_rb:
                 pool.give(b)
             arena.release()
         return PublishBatch(out, off, ln, pubs, eng.topic_names, source, rows[2:4], rows[0], rows[1], on_release=done, overlay=overlay,

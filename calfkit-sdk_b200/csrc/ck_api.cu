@@ -50,6 +50,10 @@ struct ck_handle {
     u32 *d_rb_rec_base = nullptr, *d_rb_batch_bad = nullptr, *d_rb_rec_batch = nullptr, *d_rb_val_len = nullptr, *d_rb_rec_bad = nullptr;
     int *d_rb_key_len = nullptr, *d_rb_corr_len = nullptr; uint32_t rb_n = 0;
     long long* h_rb_boff = nullptr; u32* h_rb_rbase = nullptr; cudaEvent_t rb_ev = nullptr;   // pinned frame index staging
+    // fetches holding LZ4 batches (allocated on the first one): the raw bytes, then every LZ4 batch's decoded records
+    // section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
+    u8* d_rb_fetch = nullptr; uint64_t rb_fetch_cap = 0; long long *d_rb_dec_off = nullptr, *h_rb_doff = nullptr; u32* d_rb_dec_len = nullptr;
+    uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: it held no LZ4 batch)
     // frame pass (allocated on first use): per slot, then per record in group order; the frames and their table
     ck_fitem* d_fr_items = nullptr; u32 *d_fr_gkey = nullptr, *d_fr_idx = nullptr, *d_fr_head = nullptr, *d_fr_fstart = nullptr, *d_fr_gfirst = nullptr;
     u32 *d_fr_ffirst = nullptr, *d_fr_size = nullptr, *d_fr_nlive = nullptr, *d_fr_partial = nullptr;
@@ -199,8 +203,9 @@ extern "C" void ck_destroy(ck_handle* h) {
                      h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
                      h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
                      h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
-                     h->d_fr_zoff, h->d_fr_btile};
+                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len};
     for (void* p : gptrs) if (p) cudaFree(p);
+    if (h->h_rb_doff) cudaFreeHost(h->h_rb_doff);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
     if (h->d_recv) cudaFree(h->d_recv);
     if (h->d_x_overflow) cudaFree(h->d_x_overflow);
@@ -705,9 +710,30 @@ static int rb_alloc(ck_handle* h) {
 }
 static inline uint32_t host_be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
 
+// the per-batch arrays of fetches holding LZ4 batches, on the first such fetch
+static int rb_lz_alloc(ck_handle* h) {
+    if (h->d_rb_dec_off) return 0;
+    size_t mr = (size_t)h->max_records + 1;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_dec_off, sizeof(long long) * mr));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_dec_len, sizeof(u32) * mr));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_doff, sizeof(long long) * mr));
+    return 0;
+}
+// the fetch buffer: raw bytes, then the decoded slots.  Grown as fr_grow grows the frame buffer (waits for the stream once)
+static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
+    if (h->d_rb_fetch) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_rb_fetch); }
+    h->d_rb_fetch = nullptr; h->rb_fetch_cap = 0;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_fetch, cap + CK_PAD));
+    h->rb_fetch_cap = cap;
+    return 0;
+}
+
 // A fetch response's record set (concatenated RecordBatch v2 frames, as it came off the socket) goes to HBM in one copy;
 // CRC32C check, record split and varint field decode run on the device and the walker reads every value where it lies.
-// The host only chains through the frame headers (12 + batchLength bytes each) to index the frames.
+// The host only chains through the frame headers (12 + batchLength bytes each) to index the frames, and through the LZ4
+// block chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to.  A fetch holding an LZ4 batch goes to the fetch
+// buffer instead of d_in, with a slot per LZ4 batch behind the raw bytes that the decode kernel fills; a fetch without one
+// takes the path it always took
 extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint32_t* n_records) {
     cudaSetDevice(h->device);
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
@@ -717,34 +743,62 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
     long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
+    bool lz = false; uint64_t dbytes = 0;             // slot bytes so far (the LZ4 batches' bounds)
     while (pos + 12 <= nbytes) {
         uint32_t blen = host_be32(host_buf + pos + 8);
         uint64_t end = pos + 12 + (uint64_t)blen;
         if ((int32_t)blen < (int32_t)(CK_RB_HEADER - 12) || end > nbytes) break;         // truncated trailing frame: legal in a fetch response
         uint32_t cnt = host_be32(host_buf + pos + 57);
         if (total + cnt > h->max_records || nb >= h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
+        if ((host_buf[pos + 22] & 7u) == CK_RB_LZ4) {
+            if (!lz) {                                 // the batches before the first LZ4 one have empty slots
+                if (rb_lz_alloc(h)) return 1;
+                for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
+                lz = true;
+            }
+            // the slot: what the block chain decodes to at most; 0 (the device marks the batch bad) when the chain cannot
+            // be walked or the decoded batch would not fit the 32-bit lengths of the record split
+            ck_lz_desc d; u32 k = 0; unsigned long long bound = 0;
+            const u8* z = host_buf + pos + CK_RB_HEADER;
+            if (!ck_lz_parse_desc(z, end - pos - CK_RB_HEADER, d) || !ck_lz_walk(z, end - pos - CK_RB_HEADER, d, &k, &bound) ||
+                CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
+            h->h_rb_doff[nb] = (long long)dbytes;
+            dbytes += bound;
+        } else if (lz) h->h_rb_doff[nb] = (long long)dbytes;
         boff[nb] = (long long)pos; rbase[nb] = (u32)total; nb++;
         total += cnt; pos = end;
     }
     boff[nb] = (long long)pos; rbase[nb] = (u32)total;
     u32 n = (u32)total;
     if (n_records) *n_records = n;
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_in, host_buf, pos, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_in + pos, 0, 16, h->stream));
+    u8* buf = h->d_in;
+    uint64_t base = 0, used = pos;
+    if (lz) {                                          // slots in value-offset space: behind the raw bytes, 16-byte aligned
+        base = (pos + 15) & ~15ull; used = base + dbytes;
+        for (u32 b = 0; b < nb; b++) h->h_rb_doff[b] += (long long)base;
+        h->h_rb_doff[nb] = (long long)used;
+        if (used > h->rb_fetch_cap && rb_fetch_grow(h, used + used / 8 + 4096)) return 1;
+        buf = h->d_rb_fetch;
+    }
+    CUDA_TRY(h, cudaMemcpyAsync(buf, host_buf, pos, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(buf + pos, 0, lz ? used - pos + 16 : 16, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    if (lz) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_dec_off, h->h_rb_doff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaEventRecord(h->rb_ev, h->stream));
-    h->rb_n = n;
+    h->rb_n = n; h->rb_dec_base = lz ? base : 0; h->rb_dec_bytes = lz ? dbytes : 0;
     if (nb) {
         KTimer t(h, CK_K_WALK);
-        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(h->d_in, h->d_rb_batch_off, nb, h->d_rb_batch_bad);
-        CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(h->d_in, h->d_rb_batch_off, h->d_rb_rec_base, nb, h->d_rb_batch_bad,
-                                                                        h->d_rb_rec_pos, h->d_rb_rec_batch);
-        if (n) CKL(h) ck_rb_fields_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(h->d_in, (long long)pos, h->d_rb_rec_pos, h->d_rb_rec_batch, h->d_rb_batch_bad, n,
+        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, nb, h->d_rb_batch_bad);
+        if (lz) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
+        CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off, lz ? h->d_rb_dec_off : nullptr,
+                                                                        lz ? h->d_rb_dec_len : nullptr, h->d_rb_rec_base, nb,
+                                                                        h->d_rb_batch_bad, h->d_rb_rec_pos, h->d_rb_rec_batch);
+        if (n) CKL(h) ck_rb_fields_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(buf, (long long)used, h->d_rb_rec_pos, h->d_rb_rec_batch, h->d_rb_batch_bad, n,
             h->d_in_off, h->d_rb_val_len, h->d_rb_key_off, h->d_rb_key_len, h->d_rb_corr_off, h->d_rb_corr_len, h->d_rb_rec_bad);
         CUDA_TRY(h, cudaGetLastError());
     }
-    h->cur_in = h->d_in; h->cur_in_off = h->d_in_off; h->cur_len = h->d_rb_val_len; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
+    h->cur_in = buf; h->cur_in_off = h->d_in_off; h->cur_len = h->d_rb_val_len; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
     if (launch_decode(h)) return 1;
     if (n) { CKL(h) ck_rb_mark_bad_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_rb_rec_bad, n, h->d_cols, n); CUDA_TRY(h, cudaGetLastError()); }
     return 0;
@@ -776,6 +830,18 @@ static int fetch_rb_index_impl(ck_handle* h, int64_t* val_off, uint32_t* val_len
     if (corr_len) CUDA_TRY(h, cudaMemcpyAsync(corr_len, h->d_rb_corr_len, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
     if (bad) CUDA_TRY(h, cudaMemcpyAsync(bad, h->d_rb_rec_bad, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
     if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// the decoded slots of the last ck_submit_recordbatch: value offsets from *base on index them.  Known on the host as soon
+// as the call returns; dst NULL asks for the size only
+extern "C" int ck_fetch_rb_decoded_async(ck_handle* h, uint8_t* dst, uint64_t cap, uint64_t* base, uint64_t* nbytes) {
+    cudaSetDevice(h->device);
+    if (base) *base = h->rb_dec_base;
+    if (nbytes) *nbytes = h->rb_dec_bytes;
+    if (!dst || !h->rb_dec_bytes) return 0;
+    if (cap < h->rb_dec_bytes) return fail(h, "ck_fetch_rb_decoded_async: host buffer too small");
+    CUDA_TRY(h, cudaMemcpyAsync(dst, h->d_rb_fetch + h->rb_dec_base, h->rb_dec_bytes, cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 

@@ -8,18 +8,24 @@
 //   ck_rb_crc_kernel     warp per batch: CRC32C (Castagnoli) of the covered bytes [21, end) — every lane runs a
 //                        slicing-by-4 table CRC over its own contiguous chunk, the 32 partial CRCs are folded with
 //                        GF(2) polynomial arithmetic (crc(A||B) = crc(A) * x^(8|B|) mod P  xor  crc(B));
+//   ck_rb_lz4_kernel     (a fetch holding LZ4 batches only) warp per LZ4 batch: its records section, one LZ4 frame, decoded
+//                        into the batch's slot behind the raw bytes (ck_lz4.cuh)
 //   ck_rb_split_kernel   thread per batch: hop from record to record (each starts with its own varint length)
 //   ck_rb_fields_kernel  thread per record: zig-zag varints -> key span, value span, the `correlation_id` header span
-// The walker then reads every value where it lies inside the raw buffer (ck_view.len): no per-record slicing on the host.
+// The walker then reads every value where it lies inside the buffer (ck_view.len): the raw bytes, or an LZ4 batch's decoded
+// slot.  No per-record slicing on the host.
 //
 // encode (produce): the publishes of a step to the frame topics, grouped by (topic, partition), become frames in one
 // asynchronous pass (ck_fr_*_kernel, below); ck_encode_recordbatch is its one-group case
 #ifndef CK_KAFKA_CUH
 #define CK_KAFKA_CUH
 
+#include "ck_lz4.cuh"
+
 #define CK_CRC_POLY 0x82F63B78u
 #define CK_RB_HEADER 61u
 #define CK_RB_CRC_FROM 21u
+#define CK_RB_LZ4 3u                 // attributes & 7: Kafka's codec id of LZ4
 
 // ---- CRC32C -----------------------------------------------------------------------------------------------------------
 // four 256-entry tables (slicing-by-4) built in shared memory by the block itself
@@ -102,7 +108,8 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
     const u8* f = buf + batch_off[w];
     u32 flen = (u32)(batch_off[w + 1] - batch_off[w]);
     u32 bad = 0;
-    if (flen < CK_RB_HEADER || f[16] != 2 || ((f[21] << 8 | f[22]) & 7)) bad = 1;      // not magic 2 / compressed: not handled here
+    u32 codec = flen >= CK_RB_HEADER ? f[22] & 7u : 0u;
+    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_LZ4)) bad = 1;   // not magic 2 / gzip, snappy, zstd
     else {
         u32 c = ck_crc32c_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
         if (c != ck_be32(f + 17)) bad = 1;
@@ -123,23 +130,74 @@ __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u3
     return true;
 }
 
+__device__ __forceinline__ bool ck_rb_is_lz4(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
+    return (buf[batch_off[b] + 22] & 7u) == CK_RB_LZ4;
+}
+
+// warp per batch of a fetch that holds LZ4 batches; the uncompressed ones and those the CRC check refused are skipped.
+// dec_off[b] .. dec_off[b+1]: the slot of batch b in buf, behind the raw bytes, sized by the host's walk of its block chain
+// (ck_lz_walk; an empty slot: a chain the host could not walk).  The records section of the batch is one LZ4 frame; its
+// blocks decode in order into the slot (linked blocks reach back into the frame's earlier output there), with the header
+// checksum, block checksums, content checksum and content size verified where the frame carries them.  dec_len[b] = the
+// decoded length; a frame that is malformed in any way, or does not fit its slot, marks its batch bad
+__global__ void __launch_bounds__(256)
+ck_rb_lz4_kernel(u8* __restrict__ buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off, u32 nb,
+                 u32* __restrict__ batch_bad, u32* __restrict__ dec_len) {
+    u32 w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (w >= nb || batch_bad[w] || !ck_rb_is_lz4(buf, batch_off, w)) return;
+    const u8* z = buf + batch_off[w] + CK_RB_HEADER;
+    unsigned long long zn = (unsigned long long)(batch_off[w + 1] - batch_off[w]) - CK_RB_HEADER;
+    u8* out = buf + dec_off[w];
+    unsigned long long cap = (unsigned long long)(dec_off[w + 1] - dec_off[w]), bound = 0, op = 0;
+    ck_lz_desc d;
+    u32 nblk;
+    bool ok = cap && ck_lz_parse_desc(z, zn, d) && ck_lz_walk(z, zn, d, &nblk, &bound) && bound <= cap;
+    unsigned long long pos = ok ? d.hdr_len : 0;
+    while (ok) {                                               // the walk checked the chain: every size word lies in the frame
+        u32 word = ck_lz_le32(z + pos), sz = word & 0x7FFFFFFFu;
+        pos += 4;
+        if (!word) break;
+        const u8* blk = z + pos;
+        if (d.block_sum && ck_xxh32_warp(blk, sz, 0, lane) != ck_lz_le32(blk + sz)) { ok = false; break; }
+        if (word >> 31) {                                      // stored raw
+            if (op + sz > cap) { ok = false; break; }
+            for (u32 i = lane; i < sz; i += 32) out[op + i] = blk[i];
+            op += sz;
+        } else {
+            long long r = ck_lz4_decode_block(blk, sz, out, op, d.linked ? 0ull : op, cap, d.block_max, lane);
+            if (r < 0) { ok = false; break; }
+            op += (unsigned long long)r;
+        }
+        __syncwarp();
+        pos += sz + (d.block_sum ? 4u : 0u);
+    }
+    __syncwarp();
+    if (ok && d.content_sum) ok = ck_xxh32_warp(out, (u32)op, 0, lane) == ck_lz_le32(z + pos);
+    if (ok && d.has_size) ok = d.content_size == op;
+    if (lane == 0) { dec_len[w] = ok ? (u32)op : 0u; if (!ok) batch_bad[w] = 1; }
+}
+
 // thread per batch: where does each record start.  rec_base[b] = records in the batches before b (host prefix sum of
-// the recordsCount header fields); a batch whose records do not add up to its length is marked bad
+// the recordsCount header fields); a batch whose records do not add up to its records section is marked bad.  The records
+// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for an LZ4 batch (dec_off given) its decoded slot
+// [dec_off[b], dec_off[b] + dec_len[b])
 __global__ void __launch_bounds__(128)
-ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const u32* __restrict__ rec_base, u32 nb,
+ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off,
+                   const u32* __restrict__ dec_len, const u32* __restrict__ rec_base, u32 nb,
                    u32* __restrict__ batch_bad, long long* __restrict__ rec_pos, u32* __restrict__ rec_batch) {
     u32 b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
     u32 r0 = rec_base[b], cnt = rec_base[b + 1] - r0;
-    long long base = batch_off[b];
-    const u8* f = buf + base;
-    u32 flen = (u32)(batch_off[b + 1] - base);
-    u32 pos = CK_RB_HEADER;
     bool ok = !batch_bad[b];
+    long long lo = batch_off[b] + CK_RB_HEADER, hi = batch_off[b + 1];
+    if (ok && dec_off && ck_rb_is_lz4(buf, batch_off, b)) { lo = dec_off[b]; hi = lo + dec_len[b]; }
+    const u8* f = buf + lo;
+    u32 flen = (u32)(hi - lo);
+    u32 pos = 0;
     for (u32 k = 0; k < cnt; k++) {
         rec_batch[r0 + k] = b;
         if (!ok) { rec_pos[r0 + k] = -1; continue; }
-        rec_pos[r0 + k] = base + pos;
+        rec_pos[r0 + k] = lo + pos;
         long long len;
         if (!ck_varint(f, pos, flen, len) || len < 0 || pos + (u32)len > flen) { ok = false; rec_pos[r0 + k] = -1; continue; }
         pos += (u32)len;
@@ -478,7 +536,6 @@ ck_fr_crc_fold_kernel(const ck_frame_ent* __restrict__ table, const long long* _
 // The CRC kernels above then run over the compressed frames.
 // LZ4 frame descriptor as liblz4's LZ4F_compressFrame writes it with default preferences: magic 0x184D2204, FLG 0x60
 // (version 01, independent blocks, no checksums, no content size), BD 0x40 (64 KB blocks), HC = (xxh32(FLG BD) >> 8) & 0xFF
-#include "ck_lz4.cuh"
 #define CK_LZ_FRAME_HDR 7u
 #define CK_LZ_OVERHEAD (CK_LZ_FRAME_HDR + 4u)   // frame header + end mark
 

@@ -94,4 +94,155 @@ __device__ __forceinline__ u32 ck_lz4_block(const u8* __restrict__ src, u32 len,
     return op;
 }
 
+// ---- decoding (lz4's doc/lz4_Frame_format.md and doc/lz4_Block_format.md) ------------------------------------------------
+// The one parse of the LZ4 frame format: the host walks a frame's block chain to size its output (ck_submit_recordbatch),
+// the device parses it again and decodes it (ck_lz_decode_kernel, ck_kafka.cuh).  Every read is checked against the
+// frame's end and every write against the output's capacity: the frames are outside input.
+#define CK_HD __host__ __device__ __forceinline__
+#define CK_LZ_MAGIC 0x184D2204u
+
+CK_HD u32 ck_lz_le32(const u8* p) { return (u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16) | ((u32)p[3] << 24); }
+CK_HD u32 ck_xxh_rotl(u32 x, u32 r) { return (x << r) | (x >> (32u - r)); }
+#define CK_XXH_P1 2654435761u
+#define CK_XXH_P2 2246822519u
+#define CK_XXH_P3 3266489917u
+#define CK_XXH_P4 668265263u
+#define CK_XXH_P5 374761393u
+// the tail of XXH32: h = the merged accumulators (or seed + P5) + n, then the bytes past the last 16-byte stripe
+CK_HD u32 ck_xxh32_tail(u32 h, const u8* p, u32 n) {
+    u32 i = n & ~15u;
+    for (; i + 4 <= n; i += 4) h = ck_xxh_rotl(h + ck_lz_le32(p + i) * CK_XXH_P3, 17) * CK_XXH_P4;
+    for (; i < n; i++) h = ck_xxh_rotl(h + p[i] * CK_XXH_P5, 11) * CK_XXH_P1;
+    h ^= h >> 15; h *= CK_XXH_P2; h ^= h >> 13; h *= CK_XXH_P3; h ^= h >> 16;
+    return h;
+}
+CK_HD u32 ck_xxh32_acc0(u32 k, u32 seed) {
+    return k == 0 ? seed + CK_XXH_P1 + CK_XXH_P2 : k == 1 ? seed + CK_XXH_P2 : k == 2 ? seed : seed - CK_XXH_P1;
+}
+// XXH32 of p[0, n) (the xxHash specification), one thread
+CK_HD u32 ck_xxh32(const u8* p, u32 n, u32 seed) {
+    u32 h = seed + CK_XXH_P5;
+    if (n >= 16) {
+        u32 v[4];
+        for (u32 k = 0; k < 4; k++) v[k] = ck_xxh32_acc0(k, seed);
+        for (u32 s = 0; s + 16 <= n; s += 16)
+            for (u32 k = 0; k < 4; k++) v[k] = ck_xxh_rotl(v[k] + ck_lz_le32(p + s + 4 * k) * CK_XXH_P2, 13) * CK_XXH_P1;
+        h = ck_xxh_rotl(v[0], 1) + ck_xxh_rotl(v[1], 7) + ck_xxh_rotl(v[2], 12) + ck_xxh_rotl(v[3], 18);
+    }
+    return ck_xxh32_tail(h + n, p, n);
+}
+// the same by one warp (every lane returns it): lanes 0-3 run the four accumulators over the stripes side by side
+__device__ __forceinline__ u32 ck_xxh32_warp(const u8* p, u32 n, u32 seed, u32 lane) {
+    u32 v = ck_xxh32_acc0(lane & 3u, seed);
+    if (n >= 16 && lane < 4)
+        for (u32 s = 0; s + 16 <= n; s += 16) v = ck_xxh_rotl(v + ck_lz_le32(p + s + 4 * lane) * CK_XXH_P2, 13) * CK_XXH_P1;
+    u32 v0 = __shfl_sync(0xffffffffu, v, 0), v1 = __shfl_sync(0xffffffffu, v, 1), v2 = __shfl_sync(0xffffffffu, v, 2), v3 = __shfl_sync(0xffffffffu, v, 3);
+    u32 h = n >= 16 ? ck_xxh_rotl(v0, 1) + ck_xxh_rotl(v1, 7) + ck_xxh_rotl(v2, 12) + ck_xxh_rotl(v3, 18) : seed + CK_XXH_P5;
+    return ck_xxh32_tail(h + n, p, n);
+}
+
+// frame descriptor: magic | FLG | BD | [content size u64 LE] | [dictionary id u32 LE] | HC
+struct ck_lz_desc {
+    u32 hdr_len;                       // bytes up to and including HC
+    u32 block_max;                     // BD's block maximum: 64 KB, 256 KB, 1 MB or 4 MB
+    bool linked, block_sum, content_sum, has_size;
+    unsigned long long content_size;
+};
+// the descriptor of the frame p[0, n): false when it is not one this decoder takes (bad magic, version, reserved bits,
+// block maximum or HC, a dictionary id — Kafka never sets one — or a frame that ends inside its descriptor)
+CK_HD bool ck_lz_parse_desc(const u8* p, unsigned long long n, ck_lz_desc& d) {
+    if (n < 7 || ck_lz_le32(p) != CK_LZ_MAGIC) return false;
+    u32 flg = p[4], bd = p[5];
+    if ((flg >> 6) != 1u || (flg & 2u) || (flg & 1u) || (bd & 0x8Fu)) return false;
+    u32 id = (bd >> 4) & 7u;
+    if (id < 4) return false;
+    d.block_max = 1u << (2 * id + 8);                          // 4: 64 KB, 5: 256 KB, 6: 1 MB, 7: 4 MB
+    d.linked = !(flg & 0x20u); d.block_sum = (flg & 0x10u) != 0; d.has_size = (flg & 8u) != 0; d.content_sum = (flg & 4u) != 0;
+    u32 pos = 6;
+    d.content_size = 0;
+    if (d.has_size) {
+        if (n < 15) return false;
+        d.content_size = (unsigned long long)ck_lz_le32(p + 6) | ((unsigned long long)ck_lz_le32(p + 10) << 32);
+        pos += 8;
+    }
+    if (pos >= n || p[pos] != ((ck_xxh32(p + 4, pos - 4, 0) >> 8) & 0xFFu)) return false;
+    d.hdr_len = pos + 1;
+    return true;
+}
+// the block chain of the frame p[0, n) after its descriptor: every size word to the end mark, block checksums and the
+// content checksum stepped over, and nothing after them.  *nblocks = blocks, *bound = the most the blocks decode to (the
+// block maximum per compressed block, the size of a stored block; at most the content size when the frame states it).
+// false: the chain leaves the frame, a block is larger than the block maximum, or bytes follow the frame
+CK_HD bool ck_lz_walk(const u8* p, unsigned long long n, const ck_lz_desc& d, u32* nblocks, unsigned long long* bound) {
+    unsigned long long pos = d.hdr_len, b = 0;
+    u32 k = 0;
+    for (;;) {
+        if (pos + 4 > n) return false;
+        u32 w = ck_lz_le32(p + pos);
+        pos += 4;
+        if (!w) break;
+        u32 sz = w & 0x7FFFFFFFu;
+        if (sz > d.block_max) return false;
+        pos += sz + (d.block_sum ? 4u : 0u);
+        if (pos > n) return false;
+        b += (w >> 31) ? sz : d.block_max;
+        k++;
+    }
+    if (d.content_sum) pos += 4;
+    if (pos != n) return false;
+    if (d.has_size && d.content_size < b) b = d.content_size;
+    *nblocks = k; *bound = b;
+    return true;
+}
+
+// LZ4 length continuation: 255 ... 255, last (< 255).  Every lane reads the same bytes; false when the block ends inside it
+__device__ __forceinline__ bool ck_lz_get_len(const u8* __restrict__ src, u32& ip, u32 n, unsigned long long& len) {
+    for (;;) {
+        if (ip >= n) return false;
+        u32 b = src[ip++];
+        len += b;
+        if (b != 255u) return true;
+    }
+}
+// One LZ4 block src[0, n) decoded by one warp into out[op, ...): out holds the frame's output so far, and a match may
+// reach back to out[lo] (lo = 0 for linked blocks, op for an independent block).  The block decodes to at most block_max
+// bytes and out to at most cap.  Every lane parses the same sequences; the warp copies the literals and the match of each.
+// A match copies out[pos - off + (i mod off)]: bytes that lie before it, so overlapping matches need no ordering.
+// Returns the decoded size, or -1 for a malformed block: a missing literals-only last sequence, lengths or literals past
+// the block, offset 0 or reaching before out[lo], output past block_max or cap, or a last match nearer than 12 bytes to
+// the end of the block (or ending inside its last 5 bytes)
+__device__ __forceinline__ long long ck_lz4_decode_block(const u8* __restrict__ src, u32 n, u8* __restrict__ out,
+                                                         unsigned long long op, unsigned long long lo, unsigned long long cap,
+                                                         u32 block_max, u32 lane) {
+    const unsigned long long start = op, lim = min(cap, start + block_max);
+    unsigned long long m_start = ~0ull, m_end = 0;             // the last match, relative to the block
+    u32 ip = 0;
+    for (;;) {
+        if (ip >= n) return -1;
+        u32 token = src[ip++];
+        unsigned long long ll = token >> 4;
+        if (ll == 15u && !ck_lz_get_len(src, ip, n, ll)) return -1;
+        if (ll > n - ip || op + ll > lim) return -1;
+        for (u32 i = lane; i < ll; i += 32) out[op + i] = src[ip + i];
+        ip += (u32)ll; op += ll;
+        if (ip == n) break;                                    // the last sequence: literals only
+        if (ip + 2 > n) return -1;
+        u32 off = src[ip] | ((u32)src[ip + 1] << 8);
+        ip += 2;
+        unsigned long long ml = token & 15u;
+        if (ml == 15u && !ck_lz_get_len(src, ip, n, ml)) return -1;
+        ml += 4;
+        if (off == 0 || off > op - lo || op + ml > lim) return -1;
+        __syncwarp();                                          // the literals (and earlier matches) before they are read
+        const u8* m = out + (op - off);
+        for (u32 i = lane; i < ml; i += 32) out[op + i] = m[i % off];
+        m_start = op - start; op += ml; m_end = op - start;
+        __syncwarp();
+    }
+    __syncwarp();
+    unsigned long long len = op - start;
+    if (m_start != ~0ull && (m_start + 12 > len || m_end + 5 > len)) return -1;
+    return (long long)len;
+}
+
 #endif  // CK_LZ4_CUH

@@ -1,0 +1,116 @@
+"""Cost of consuming LZ4 fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
+
+The step's tool events are framed once by the record form of the frame pass (ck_encode_frames_records), uncompressed and
+with LZ4 (ck_set_option 3 = 3), as a producer would write them to the tool's input topic.  Two legs, alternating, two
+runs each, consume one of those fetch responses per step:
+  plain  ck_submit_recordbatch over the uncompressed frames + plan + the copies a Lane makes (results, record index)
+  lz4    the same over the LZ4 frames: their records sections are decoded on the device, and the decoded region is
+         copied back with the results (ck_fetch_rb_decoded_async)
+Per leg: step time (CUDA events around the whole step, copies included), the fetch and walk kernels (profile timer
+"walk": CRC, LZ4 decode, split, fields and the walker), the LZ4 decode alone (walk of lz4 minus walk of plain), events/s,
+and H2D / D2H bytes per step.  Prints one JSON line with the card name and power limit read in the same run.
+
+    python scripts/quick_fetch.py [events]
+"""
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "calfkit-sdk_b200"))
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+from calfkit import synth  # noqa: E402
+from calfkit.engine import BatchEngine, ToolTemplate  # noqa: E402
+from calfkit.engine._lib import PUB_DTYPE, ptr  # noqa: E402
+from calfkit.engine.lane import PinnedBuffer  # noqa: E402
+
+TOPICS = ["tool.get_weather.input", "tool.get_weather.output", "weather_agent.input"]
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 1_000_000
+recs = synth.tool_events(n, seed=0)
+
+
+def corr_of(r: bytes) -> str:
+    k = r.index(b'"correlation_id":"') + 18
+    return r[k:r.index(b'"', k)].decode()
+
+
+items = [(r, c.encode(), c) for r, c in ((r, corr_of(r)) for r in recs)]
+fetch = {}
+fr = BatchEngine(0, max_records=n, max_in_bytes=sum(len(r) for r in recs) + 64 * n + 4096)
+fr.register_topics(TOPICS, num_partitions=8)
+for codec in (None, "lz4"):
+    fr.set_frame_compression(codec)
+    fr.encode_frames_records("tool.get_weather.input", items, 1767225600000)
+    frames = fr.fetch_frames()
+    fetch["lz4" if codec else "plain"] = b"".join(frames.frame(i).tobytes() for i in range(len(frames)))
+fr.close()
+del items
+
+e = BatchEngine(0, max_records=n, max_in_bytes=len(fetch["plain"]) + 4096)
+e.register_topics(TOPICS, num_partitions=8)
+e.set_tool_node("tool.get_weather.output", ToolTemplate.from_format("It's sunny in {location}"))
+pinned = {}
+for k, v in fetch.items():
+    pinned[k] = PinnedBuffer(len(v))
+    pinned[k].array[:len(v)] = np.frombuffer(v, dtype=np.uint8)
+b_out = PinnedBuffer(e.max_out + 64)
+b_off, b_len = PinnedBuffer(8 * (n + 1)), PinnedBuffer(4 * n)
+b_pubs = PinnedBuffer(PUB_DTYPE.itemsize * 2 * n)
+b_rb = PinnedBuffer(16 * n + 64)
+b_dec = [None]
+st = torch.cuda.ExternalStream(e.stream_ptr())
+
+
+def step(name: str) -> tuple[int, int]:
+    buf = pinned[name]
+    nrec = C.c_uint32(0)
+    e._check(e.lib.ck_submit_recordbatch(e.h, ptr(buf.array), buf.nbytes, C.byref(nrec)))
+    e.n = m = nrec.value
+    e.tool_plan()
+    nb, npay, npub = e.out_size()
+    e._check(e.lib.ck_fetch_output_async(e.h, ptr(b_out.array), b_out.nbytes, ptr(b_off.array), ptr(b_len.array), ptr(b_pubs.array)))
+    e._check(e.lib.ck_fetch_rb_index_async(e.h, ptr(b_rb.array), ptr(b_rb.array[8 * m:]), None, None, None, None, ptr(b_rb.array[12 * m:])))
+    d2h = nb + 8 * (npay + 1) + 4 * npay + PUB_DTYPE.itemsize * npub + 16 * m
+    base, dn = C.c_uint64(0), C.c_uint64(0)
+    e._check(e.lib.ck_fetch_rb_decoded_async(e.h, None, 0, C.byref(base), C.byref(dn)))
+    if dn.value:
+        if b_dec[0] is None or b_dec[0].nbytes < dn.value:
+            b_dec[0] = PinnedBuffer(dn.value)
+        e._check(e.lib.ck_fetch_rb_decoded_async(e.h, ptr(b_dec[0].array), b_dec[0].nbytes, None, None))
+        d2h += dn.value
+    e.sync()
+    return buf.nbytes, d2h
+
+
+def leg(name: str, steps: int = 5) -> dict:
+    step(name)
+    e.profile(True)
+    e.profile_read()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record(st)
+    for _ in range(steps):
+        h2d, d2h = step(name)
+    ev1.record(st)
+    torch.cuda.synchronize()
+    prof = e.profile_read()
+    e.profile(False)
+    ms = ev0.elapsed_time(ev1) / steps
+    return {"step_ms": round(ms, 3), "walk_kernel_ms": round(prof["walk"][0] / steps, 3), "events_per_s": round(n / ms * 1e3),
+            "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h}
+
+
+q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+res = {"events": n, "gpu": q.stdout.strip(), "fetch_bytes": {k: len(v) for k, v in fetch.items()}, "runs": []}
+t0 = time.time()
+for _ in range(2):
+    for name in ("plain", "lz4"):
+        res["runs"].append({"leg": name, **leg(name)})
+res["wall_s"] = round(time.time() - t0, 1)
+walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k in ("plain", "lz4")}
+res["lz4_decode_ms"] = round(walk["lz4"] - walk["plain"], 3)
+res["decoded_bytes"] = int(b_dec[0].nbytes) if b_dec[0] is not None else 0
+print(json.dumps(res))
