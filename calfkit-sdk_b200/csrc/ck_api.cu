@@ -50,10 +50,10 @@ struct ck_handle {
     u32 *d_rb_rec_base = nullptr, *d_rb_batch_bad = nullptr, *d_rb_rec_batch = nullptr, *d_rb_val_len = nullptr, *d_rb_rec_bad = nullptr;
     int *d_rb_key_len = nullptr, *d_rb_corr_len = nullptr; uint32_t rb_n = 0;
     long long* h_rb_boff = nullptr; u32* h_rb_rbase = nullptr; cudaEvent_t rb_ev = nullptr;   // pinned frame index staging
-    // fetches holding LZ4 batches (allocated on the first one): the raw bytes, then every LZ4 batch's decoded records
-    // section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
+    // fetches holding gzip or LZ4 batches (allocated on the first one): the raw bytes, then every such batch's decoded
+    // records section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
     u8* d_rb_fetch = nullptr; uint64_t rb_fetch_cap = 0; long long *d_rb_dec_off = nullptr, *h_rb_doff = nullptr; u32* d_rb_dec_len = nullptr;
-    uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: it held no LZ4 batch)
+    uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: no gzip / LZ4 batch)
     // frame pass (allocated on first use): per slot, then per record in group order; the frames and their table
     ck_fitem* d_fr_items = nullptr; u32 *d_fr_gkey = nullptr, *d_fr_idx = nullptr, *d_fr_head = nullptr, *d_fr_fstart = nullptr, *d_fr_gfirst = nullptr;
     u32 *d_fr_ffirst = nullptr, *d_fr_size = nullptr, *d_fr_nlive = nullptr, *d_fr_partial = nullptr;
@@ -710,7 +710,7 @@ static int rb_alloc(ck_handle* h) {
 }
 static inline uint32_t host_be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
 
-// the per-batch arrays of fetches holding LZ4 batches, on the first such fetch
+// the per-batch arrays of fetches holding gzip or LZ4 batches, on the first such fetch
 static int rb_lz_alloc(ck_handle* h) {
     if (h->d_rb_dec_off) return 0;
     size_t mr = (size_t)h->max_records + 1;
@@ -730,10 +730,11 @@ static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
 
 // A fetch response's record set (concatenated RecordBatch v2 frames, as it came off the socket) goes to HBM in one copy;
 // CRC32C check, record split and varint field decode run on the device and the walker reads every value where it lies.
-// The host only chains through the frame headers (12 + batchLength bytes each) to index the frames, and through the LZ4
-// block chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to.  A fetch holding an LZ4 batch goes to the fetch
-// buffer instead of d_in, with a slot per LZ4 batch behind the raw bytes that the decode kernel fills; a fetch without one
-// takes the path it always took
+// The host only chains through the frame headers (12 + batchLength bytes each) to index the frames, through the LZ4 block
+// chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to, and through the member header of a gzip batch to read
+// its ISIZE (ck_gz_member).  A fetch holding a gzip or LZ4 batch goes to the fetch buffer instead of d_in, with a slot per
+// such batch behind the raw bytes that the decode kernel of its codec fills (one launch per codec present); a fetch
+// without one takes the path it always took
 extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint32_t* n_records) {
     cudaSetDevice(h->device);
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
@@ -743,25 +744,36 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
     long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
-    bool lz = false; uint64_t dbytes = 0;             // slot bytes so far (the LZ4 batches' bounds)
+    bool lz = false, has_lz4 = false, has_gz = false; // lz: the fetch holds a decoded batch (gzip or LZ4)
+    uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 batches' bounds, the gzip ISIZEs)
     while (pos + 12 <= nbytes) {
         uint32_t blen = host_be32(host_buf + pos + 8);
         uint64_t end = pos + 12 + (uint64_t)blen;
         if ((int32_t)blen < (int32_t)(CK_RB_HEADER - 12) || end > nbytes) break;         // truncated trailing frame: legal in a fetch response
         uint32_t cnt = host_be32(host_buf + pos + 57);
         if (total + cnt > h->max_records || nb >= h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
-        if ((host_buf[pos + 22] & 7u) == CK_RB_LZ4) {
-            if (!lz) {                                 // the batches before the first LZ4 one have empty slots
+        u32 codec = host_buf[pos + 22] & 7u;
+        if (codec == CK_RB_LZ4 || codec == CK_RB_GZIP) {
+            if (!lz) {                                 // the batches before the first decoded one have empty slots
                 if (rb_lz_alloc(h)) return 1;
                 for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
                 lz = true;
             }
-            // the slot: what the block chain decodes to at most; 0 (the device marks the batch bad) when the chain cannot
-            // be walked or the decoded batch would not fit the 32-bit lengths of the record split
-            ck_lz_desc d; u32 k = 0; unsigned long long bound = 0;
+            // the slot: LZ4, what the block chain decodes to at most; gzip, the member's ISIZE.  0 (the device marks the
+            // batch bad) when the chain cannot be walked or the member header parsed, or the decoded batch would not fit
+            // the 32-bit lengths of the record split
+            unsigned long long bound = 0;
             const u8* z = host_buf + pos + CK_RB_HEADER;
-            if (!ck_lz_parse_desc(z, end - pos - CK_RB_HEADER, d) || !ck_lz_walk(z, end - pos - CK_RB_HEADER, d, &k, &bound) ||
-                CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
+            if (codec == CK_RB_LZ4) {
+                ck_lz_desc d; u32 k = 0;
+                if (!ck_lz_parse_desc(z, end - pos - CK_RB_HEADER, d) || !ck_lz_walk(z, end - pos - CK_RB_HEADER, d, &k, &bound) ||
+                    CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
+                has_lz4 = true;
+            } else {
+                u32 hdr = 0, isize = 0;
+                if (ck_gz_member(z, end - pos - CK_RB_HEADER, &hdr, &isize) && CK_RB_HEADER + (unsigned long long)isize <= 0x7fffffffull) bound = isize;
+                has_gz = true;
+            }
             h->h_rb_doff[nb] = (long long)dbytes;
             dbytes += bound;
         } else if (lz) h->h_rb_doff[nb] = (long long)dbytes;
@@ -790,7 +802,9 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     if (nb) {
         KTimer t(h, CK_K_WALK);
         CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, nb, h->d_rb_batch_bad);
-        if (lz) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
+        if (has_lz4) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
+        if (has_gz) CKL(h) ck_rb_gzip_kernel<<<(nb + CK_GZ_WARPS - 1) / CK_GZ_WARPS, 32 * CK_GZ_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
+                                                                                                          h->d_rb_batch_bad, h->d_rb_dec_len);
         CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off, lz ? h->d_rb_dec_off : nullptr,
                                                                         lz ? h->d_rb_dec_len : nullptr, h->d_rb_rec_base, nb,
                                                                         h->d_rb_batch_bad, h->d_rb_rec_pos, h->d_rb_rec_batch);

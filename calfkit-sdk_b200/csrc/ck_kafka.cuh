@@ -10,10 +10,12 @@
 //                        GF(2) polynomial arithmetic (crc(A||B) = crc(A) * x^(8|B|) mod P  xor  crc(B));
 //   ck_rb_lz4_kernel     (a fetch holding LZ4 batches only) warp per LZ4 batch: its records section, one LZ4 frame, decoded
 //                        into the batch's slot behind the raw bytes (ck_lz4.cuh)
+//   ck_rb_gzip_kernel    (a fetch holding gzip batches only) warp per gzip batch: its records section, one gzip member,
+//                        inflated into the batch's slot (ck_inflate.cuh) and checked against the trailer's CRC32
 //   ck_rb_split_kernel   thread per batch: hop from record to record (each starts with its own varint length)
 //   ck_rb_fields_kernel  thread per record: zig-zag varints -> key span, value span, the `correlation_id` header span
-// The walker then reads every value where it lies inside the buffer (ck_view.len): the raw bytes, or an LZ4 batch's decoded
-// slot.  No per-record slicing on the host.
+// The walker then reads every value where it lies inside the buffer (ck_view.len): the raw bytes, or a compressed batch's
+// decoded slot.  No per-record slicing on the host.
 //
 // encode (produce): the publishes of a step to the frame topics, grouped by (topic, partition), become frames in one
 // asynchronous pass (ck_fr_*_kernel, below); ck_encode_recordbatch is its one-group case
@@ -21,19 +23,24 @@
 #define CK_KAFKA_CUH
 
 #include "ck_lz4.cuh"
+#include "ck_inflate.cuh"
 
-#define CK_CRC_POLY 0x82F63B78u
+#define CK_CRC_POLY 0x82F63B78u      // CRC32C (Castagnoli), reflected
+#define CK_CRC32_POLY 0xEDB88320u    // CRC32 (IEEE), reflected: gzip's
 #define CK_RB_HEADER 61u
 #define CK_RB_CRC_FROM 21u
-#define CK_RB_LZ4 3u                 // attributes & 7: Kafka's codec id of LZ4
+#define CK_RB_GZIP 1u                // attributes & 7: Kafka's codec ids of gzip
+#define CK_RB_LZ4 3u                 // and LZ4
 
-// ---- CRC32C -----------------------------------------------------------------------------------------------------------
-// four 256-entry tables (slicing-by-4) built in shared memory by the block itself
+// ---- CRC32 ------------------------------------------------------------------------------------------------------------
+// Generic over the reflected polynomial P: CRC32C (Castagnoli, the batch CRC) by default, CRC32 (IEEE, the gzip trailer)
+// for the gzip decode.  Four 256-entry tables (slicing-by-4) built in shared memory by the block itself
+template <u32 P = CK_CRC_POLY>
 __device__ __forceinline__ void ck_crc_tables(u32* t /* [4][256] */) {
     for (u32 i = threadIdx.x; i < 256; i += blockDim.x) {
         u32 c = i;
 #pragma unroll
-        for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((c & 1u) ? CK_CRC_POLY : 0u);
+        for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((c & 1u) ? P : 0u);
         t[i] = c;
     }
     __syncthreads();
@@ -44,13 +51,15 @@ __device__ __forceinline__ void ck_crc_tables(u32* t /* [4][256] */) {
     }
     __syncthreads();
 }
-// finalised CRC32C of p[0..n) (init / xor-out all ones)
-__device__ __forceinline__ u32 ck_crc32c_span(const u32* __restrict__ t, const u8* __restrict__ p, u32 n) {
+// finalised CRC of p[0..n) (init / xor-out all ones) with the tables of its polynomial.  LDG: words read through the
+// read-only cache; false for bytes the same kernel wrote
+template <bool LDG = true>
+__device__ __forceinline__ u32 ck_crc_span(const u32* __restrict__ t, const u8* __restrict__ p, u32 n) {
     u32 c = 0xffffffffu;
     while (n && ((uintptr_t)p & 3u)) { c = t[(c ^ *p++) & 0xffu] ^ (c >> 8); n--; }
     const u32* w = (const u32*)p;
     for (; n >= 4; n -= 4) {
-        c ^= __ldg(w++);
+        c ^= LDG ? __ldg(w++) : *w++;
         c = t[768 + (c & 0xffu)] ^ t[512 + ((c >> 8) & 0xffu)] ^ t[256 + ((c >> 16) & 0xffu)] ^ t[c >> 24];
     }
     p = (const u8*)w;
@@ -58,37 +67,41 @@ __device__ __forceinline__ u32 ck_crc32c_span(const u32* __restrict__ t, const u
     return ~c;
 }
 // a(x) * b(x) mod P(x), reflected representation (bit 31 = x^0)
+template <u32 P = CK_CRC_POLY>
 __device__ __forceinline__ u32 ck_gf_mul(u32 a, u32 b) {
     u32 p = 0;
 #pragma unroll 4
     for (u32 m = 0x80000000u; m; m >>= 1) {
         if (a & m) p ^= b;
-        b = (b & 1u) ? (b >> 1) ^ CK_CRC_POLY : b >> 1;
+        b = (b & 1u) ? (b >> 1) ^ P : b >> 1;
     }
     return p;
 }
 // x^(8 n) mod P
+template <u32 P = CK_CRC_POLY>
 __device__ __forceinline__ u32 ck_gf_xpow8(unsigned long long n) {
     u32 p = 0x80000000u;                       // x^0
     u32 sq = 0x00800000u;                      // x^8
-    while (n) { if (n & 1ull) p = ck_gf_mul(sq, p); sq = ck_gf_mul(sq, sq); n >>= 1; }
+    while (n) { if (n & 1ull) p = ck_gf_mul<P>(sq, p); sq = ck_gf_mul<P>(sq, sq); n >>= 1; }
     return p;
 }
-__device__ __forceinline__ u32 ck_crc_combine(u32 crc_a, u32 crc_b, u32 xpow_len_b) { return ck_gf_mul(xpow_len_b, crc_a) ^ crc_b; }
+template <u32 P = CK_CRC_POLY>
+__device__ __forceinline__ u32 ck_crc_combine(u32 crc_a, u32 crc_b, u32 xpow_len_b) { return ck_gf_mul<P>(xpow_len_b, crc_a) ^ crc_b; }
 
-// CRC32C of one span by one warp (all lanes return it): lane 0 takes the odd-sized head so that every other lane holds
+// the CRC of one span by one warp (all lanes return it): lane 0 takes the odd-sized head so that every other lane holds
 // exactly `chunk` bytes and the tree fold shifts by multiples of one precomputed power
-__device__ __forceinline__ u32 ck_crc32c_warp(const u32* __restrict__ t, const u8* __restrict__ p, u32 n, u32 lane) {
+template <u32 P = CK_CRC_POLY, bool LDG = true>
+__device__ __forceinline__ u32 ck_crc_warp(const u32* __restrict__ t, const u8* __restrict__ p, u32 n, u32 lane) {
     u32 chunk = (n >> 5) & ~3u;
     u32 head = n - 31u * chunk;
-    u32 c = lane == 0 ? ck_crc32c_span(t, p, head) : (chunk ? ck_crc32c_span(t, p + head + (lane - 1) * chunk, chunk) : 0u);
+    u32 c = lane == 0 ? ck_crc_span<LDG>(t, p, head) : (chunk ? ck_crc_span<LDG>(t, p + head + (lane - 1) * chunk, chunk) : 0u);
     if (!chunk) return __shfl_sync(0xffffffffu, c, 0);
-    u32 xp = ck_gf_xpow8(chunk);               // x^(8 chunk); squared at every level: right blocks hold 1, 2, 4, 8, 16 chunks
+    u32 xp = ck_gf_xpow8<P>(chunk);            // x^(8 chunk); squared at every level: right blocks hold 1, 2, 4, 8, 16 chunks
 #pragma unroll
     for (u32 s = 1; s < 32; s <<= 1) {
         u32 right = __shfl_down_sync(0xffffffffu, c, s);
-        if ((lane & (2 * s - 1)) == 0) c = ck_crc_combine(c, right, xp);
-        xp = ck_gf_mul(xp, xp);
+        if ((lane & (2 * s - 1)) == 0) c = ck_crc_combine<P>(c, right, xp);
+        xp = ck_gf_mul<P>(xp, xp);
     }
     return __shfl_sync(0xffffffffu, c, 0);
 }
@@ -109,9 +122,9 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
     u32 flen = (u32)(batch_off[w + 1] - batch_off[w]);
     u32 bad = 0;
     u32 codec = flen >= CK_RB_HEADER ? f[22] & 7u : 0u;
-    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_LZ4)) bad = 1;   // not magic 2 / gzip, snappy, zstd
+    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_GZIP && codec != CK_RB_LZ4)) bad = 1;   // not magic 2 / snappy, zstd
     else {
-        u32 c = ck_crc32c_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
+        u32 c = ck_crc_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
         if (c != ck_be32(f + 17)) bad = 1;
     }
     if (lane == 0) batch_bad[w] = bad;
@@ -132,6 +145,11 @@ __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u3
 
 __device__ __forceinline__ bool ck_rb_is_lz4(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
     return (buf[batch_off[b] + 22] & 7u) == CK_RB_LZ4;
+}
+// a batch whose records section is decoded into a slot: gzip or LZ4
+__device__ __forceinline__ bool ck_rb_is_decoded(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
+    u32 codec = buf[batch_off[b] + 22] & 7u;
+    return codec == CK_RB_GZIP || codec == CK_RB_LZ4;
 }
 
 // warp per batch of a fetch that holds LZ4 batches; the uncompressed ones and those the CRC check refused are skipped.
@@ -177,10 +195,36 @@ ck_rb_lz4_kernel(u8* __restrict__ buf, const long long* __restrict__ batch_off, 
     if (lane == 0) { dec_len[w] = ok ? (u32)op : 0u; if (!ok) batch_bad[w] = 1; }
 }
 
+// warp per batch of a fetch that holds gzip batches (CK_GZ_WARPS per block, each with its Huffman tables in shared memory);
+// the others and those the CRC check refused are skipped.  dec_off[b] .. dec_off[b+1]: the slot of batch b, as many bytes
+// as the member's ISIZE says (ck_gz_member on the host).  The records section is one gzip member: its header parsed again,
+// its deflate stream inflated into the slot (ck_gz_decode: zlib's verdict on every block), the trailer right behind the
+// final block and ending at the batch's end, the output exactly ISIZE bytes, and the CRC32 of the output (the warp fold
+// over the IEEE tables) equal to the trailer's.  The host refuses a member by giving it an empty slot; a member of
+// ISIZE 0 gets one too, so the slot's size is no verdict: the decode parses the member itself and refuses unless the slot
+// is exactly ISIZE bytes.  dec_len[b] = the inflated length; anything else marks the batch bad
+#define CK_GZ_WARPS 4u
+__global__ void __launch_bounds__(32 * CK_GZ_WARPS)
+ck_rb_gzip_kernel(u8* buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off, u32 nb,
+                  u32* __restrict__ batch_bad, u32* __restrict__ dec_len) {
+    __shared__ u32 t[1024];
+    __shared__ ck_gz_ws ws[CK_GZ_WARPS];
+    ck_crc_tables<CK_CRC32_POLY>(t);
+    u32 wi = threadIdx.x >> 5, w = blockIdx.x * CK_GZ_WARPS + wi, lane = threadIdx.x & 31;
+    if (w >= nb || batch_bad[w] || (buf[batch_off[w] + 22] & 7u) != CK_RB_GZIP) return;
+    const u8* z = buf + batch_off[w] + CK_RB_HEADER;
+    unsigned long long zn = (unsigned long long)(batch_off[w + 1] - batch_off[w]) - CK_RB_HEADER;
+    u8* out = buf + dec_off[w];
+    long long r = ck_gz_decode(z, zn, out, (unsigned long long)(dec_off[w + 1] - dec_off[w]), ws[wi], lane);
+    __syncwarp();
+    bool ok = r >= 0 && ck_crc_warp<CK_CRC32_POLY, false>(t, out, (u32)r, lane) == ck_gz_le32(z + zn - 8);
+    if (lane == 0) { dec_len[w] = ok ? (u32)r : 0u; if (!ok) batch_bad[w] = 1; }
+}
+
 // thread per batch: where does each record start.  rec_base[b] = records in the batches before b (host prefix sum of
 // the recordsCount header fields); a batch whose records do not add up to its records section is marked bad.  The records
-// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for an LZ4 batch (dec_off given) its decoded slot
-// [dec_off[b], dec_off[b] + dec_len[b])
+// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for a gzip or LZ4 batch (dec_off given) its decoded
+// slot [dec_off[b], dec_off[b] + dec_len[b])
 __global__ void __launch_bounds__(128)
 ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off,
                    const u32* __restrict__ dec_len, const u32* __restrict__ rec_base, u32 nb,
@@ -190,7 +234,7 @@ ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ bat
     u32 r0 = rec_base[b], cnt = rec_base[b + 1] - r0;
     bool ok = !batch_bad[b];
     long long lo = batch_off[b] + CK_RB_HEADER, hi = batch_off[b + 1];
-    if (ok && dec_off && ck_rb_is_lz4(buf, batch_off, b)) { lo = dec_off[b]; hi = lo + dec_len[b]; }
+    if (ok && dec_off && ck_rb_is_decoded(buf, batch_off, b)) { lo = dec_off[b]; hi = lo + dec_len[b]; }
     const u8* f = buf + lo;
     u32 flen = (u32)(hi - lo);
     u32 pos = 0;
@@ -500,7 +544,7 @@ ck_fr_crc_chunks_kernel(const ck_frame_ent* __restrict__ table, const long long*
         ck_frame_ent e = table[lo];
         unsigned long long start = (c - (unsigned long long)C[lo]) * CK_RB_CRC_CHUNK, covered = (unsigned long long)e.length - CK_RB_CRC_FROM;
         u32 len = (u32)min((unsigned long long)CK_RB_CRC_CHUNK, covered - start);
-        u32 crc = ck_crc32c_warp(t, frames + e.offset + CK_RB_CRC_FROM + start, len, lane);
+        u32 crc = ck_crc_warp(t, frames + e.offset + CK_RB_CRC_FROM + start, len, lane);
         if (lane == 0) partial[c] = crc;
     }
 }

@@ -1,13 +1,16 @@
-"""Cost of consuming LZ4 fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
+"""Cost of consuming LZ4 and gzip fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
 
 The step's tool events are framed once by the record form of the frame pass (ck_encode_frames_records), uncompressed and
-with LZ4 (ck_set_option 3 = 3), as a producer would write them to the tool's input topic.  Two legs, alternating, two
-runs each, consume one of those fetch responses per step:
+with LZ4 (ck_set_option 3 = 3), as a producer would write them to the tool's input topic; the gzip fetch is the same
+step's uncompressed frames with every records section recompressed on the host by zlib at level 6 (the level Java's
+GZIPOutputStream uses), one member per batch.  Three legs, alternating, two runs each, consume one of those fetch
+responses per step:
   plain  ck_submit_recordbatch over the uncompressed frames + plan + the copies a Lane makes (results, record index)
   lz4    the same over the LZ4 frames: their records sections are decoded on the device, and the decoded region is
          copied back with the results (ck_fetch_rb_decoded_async)
+  gzip   the same over the gzip frames (inflated on the device)
 Per leg: step time (CUDA events around the whole step, copies included), the fetch and walk kernels (profile timer
-"walk": CRC, LZ4 decode, split, fields and the walker), the LZ4 decode alone (walk of lz4 minus walk of plain), events/s,
+"walk": CRC, decode, split, fields and the walker), each decode alone (walk of the leg minus walk of plain), events/s,
 and H2D / D2H bytes per step.  Prints one JSON line with the card name and power limit read in the same run.
 
     python scripts/quick_fetch.py [events]
@@ -15,9 +18,11 @@ and H2D / D2H bytes per step.  Prints one JSON line with the card name and power
 import ctypes as C
 import json
 import os
+import struct
 import subprocess
 import sys
 import time
+import zlib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "calfkit-sdk_b200"))
@@ -50,6 +55,25 @@ for codec in (None, "lz4"):
 fr.close()
 del items
 
+
+def gzip_frames(buf: bytes) -> bytes:
+    """every frame's records section [61, end) as one gzip member (zlib level 6), attributes codec 1, CRC32C recomputed"""
+    from oracle import kafka_batch as kb
+    out, pos = [], 0
+    while pos + 12 <= len(buf):
+        end = pos + 12 + int.from_bytes(buf[pos + 8:pos + 12], "big")
+        f = buf[pos:end]
+        c = zlib.compressobj(6, zlib.DEFLATED, 31)
+        sec = c.compress(f[61:]) + c.flush()
+        covered = struct.pack(">h", (struct.unpack_from(">h", f, 21)[0] & ~7) | 1) + f[23:61] + sec
+        out.append(f[:8] + struct.pack(">i", len(covered) + 9) + f[12:17] + struct.pack(">I", kb.crc32c(covered)) + covered)
+        pos = end
+    return b"".join(out)
+
+
+sys.path.insert(0, ROOT)
+fetch["gzip"] = gzip_frames(fetch["plain"])
+
 e = BatchEngine(0, max_records=n, max_in_bytes=len(fetch["plain"]) + 4096)
 e.register_topics(TOPICS, num_partitions=8)
 e.set_tool_node("tool.get_weather.output", ToolTemplate.from_format("It's sunny in {location}"))
@@ -61,7 +85,7 @@ b_out = PinnedBuffer(e.max_out + 64)
 b_off, b_len = PinnedBuffer(8 * (n + 1)), PinnedBuffer(4 * n)
 b_pubs = PinnedBuffer(PUB_DTYPE.itemsize * 2 * n)
 b_rb = PinnedBuffer(16 * n + 64)
-b_dec = [None]
+b_dec = {}
 st = torch.cuda.ExternalStream(e.stream_ptr())
 
 
@@ -78,9 +102,9 @@ def step(name: str) -> tuple[int, int]:
     base, dn = C.c_uint64(0), C.c_uint64(0)
     e._check(e.lib.ck_fetch_rb_decoded_async(e.h, None, 0, C.byref(base), C.byref(dn)))
     if dn.value:
-        if b_dec[0] is None or b_dec[0].nbytes < dn.value:
-            b_dec[0] = PinnedBuffer(dn.value)
-        e._check(e.lib.ck_fetch_rb_decoded_async(e.h, ptr(b_dec[0].array), b_dec[0].nbytes, None, None))
+        if name not in b_dec or b_dec[name].nbytes < dn.value:
+            b_dec[name] = PinnedBuffer(dn.value)
+        e._check(e.lib.ck_fetch_rb_decoded_async(e.h, ptr(b_dec[name].array), b_dec[name].nbytes, None, None))
         d2h += dn.value
     e.sync()
     return buf.nbytes, d2h
@@ -88,6 +112,8 @@ def step(name: str) -> tuple[int, int]:
 
 def leg(name: str, steps: int = 5) -> dict:
     step(name)
+    m = e.n
+    bad = int(b_rb.array[12 * m:16 * m].view(np.uint32).sum())
     e.profile(True)
     e.profile_read()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -100,17 +126,18 @@ def leg(name: str, steps: int = 5) -> dict:
     e.profile(False)
     ms = ev0.elapsed_time(ev1) / steps
     return {"step_ms": round(ms, 3), "walk_kernel_ms": round(prof["walk"][0] / steps, 3), "events_per_s": round(n / ms * 1e3),
-            "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h}
+            "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "bad_records": bad}
 
 
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
 res = {"events": n, "gpu": q.stdout.strip(), "fetch_bytes": {k: len(v) for k, v in fetch.items()}, "runs": []}
 t0 = time.time()
 for _ in range(2):
-    for name in ("plain", "lz4"):
+    for name in ("plain", "lz4", "gzip"):
         res["runs"].append({"leg": name, **leg(name)})
 res["wall_s"] = round(time.time() - t0, 1)
-walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k in ("plain", "lz4")}
+walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k in ("plain", "lz4", "gzip")}
 res["lz4_decode_ms"] = round(walk["lz4"] - walk["plain"], 3)
-res["decoded_bytes"] = int(b_dec[0].nbytes) if b_dec[0] is not None else 0
+res["gzip_decode_ms"] = round(walk["gzip"] - walk["plain"], 3)
+res["decoded_bytes"] = {k: int(b.nbytes) for k, b in b_dec.items()}
 print(json.dumps(res))
