@@ -731,10 +731,11 @@ static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
 // A fetch response's record set (concatenated RecordBatch v2 frames, as it came off the socket) goes to HBM in one copy;
 // CRC32C check, record split and varint field decode run on the device and the walker reads every value where it lies.
 // The host only chains through the frame headers (12 + batchLength bytes each) to index the frames, through the LZ4 block
-// chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to, and through the member header of a gzip batch to read
-// its ISIZE (ck_gz_member).  A fetch holding a gzip or LZ4 batch goes to the fetch buffer instead of d_in, with a slot per
-// such batch behind the raw bytes that the decode kernel of its codec fills (one launch per codec present); a fetch
-// without one takes the path it always took
+// chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to, through the member header of a gzip batch to read its
+// ISIZE (ck_gz_member), and through the frame header and block headers of a zstd batch to bound what it decodes to
+// (ck_zs_header, ck_zs_walk).  A fetch holding a gzip, LZ4 or zstd batch goes to the fetch buffer instead of d_in, with a
+// slot per such batch behind the raw bytes that the decode kernel of its codec fills (one launch per codec present); a
+// fetch without one takes the path it always took
 extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint32_t* n_records) {
     cudaSetDevice(h->device);
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
@@ -744,8 +745,8 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
     long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
-    bool lz = false, has_lz4 = false, has_gz = false; // lz: the fetch holds a decoded batch (gzip or LZ4)
-    uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 batches' bounds, the gzip ISIZEs)
+    bool lz = false, has_lz4 = false, has_gz = false, has_zs = false;   // lz: the fetch holds a decoded batch
+    uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 and zstd bounds, the gzip ISIZEs)
     while (pos + 12 <= nbytes) {
         uint32_t blen = host_be32(host_buf + pos + 8);
         uint64_t end = pos + 12 + (uint64_t)blen;
@@ -753,15 +754,17 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
         uint32_t cnt = host_be32(host_buf + pos + 57);
         if (total + cnt > h->max_records || nb >= h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
         u32 codec = host_buf[pos + 22] & 7u;
-        if (codec == CK_RB_LZ4 || codec == CK_RB_GZIP) {
+        if (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD) {
             if (!lz) {                                 // the batches before the first decoded one have empty slots
                 if (rb_lz_alloc(h)) return 1;
                 for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
                 lz = true;
             }
-            // the slot: LZ4, what the block chain decodes to at most; gzip, the member's ISIZE.  0 (the device marks the
-            // batch bad) when the chain cannot be walked or the member header parsed, or the decoded batch would not fit
-            // the 32-bit lengths of the record split
+            // the slot: LZ4, what the block chain decodes to at most; gzip, the member's ISIZE; zstd, what the blocks
+            // decode to at most (compressed ones Block_Maximum_Size, even when Frame_Content_Size says less: their literals
+            // are decoded into the end of that room).  0 (the device marks the batch bad) when the chain or the blocks
+            // cannot be walked or the member header parsed, or the decoded batch would not fit the 32-bit lengths of the
+            // record split
             unsigned long long bound = 0;
             const u8* z = host_buf + pos + CK_RB_HEADER;
             if (codec == CK_RB_LZ4) {
@@ -769,6 +772,11 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
                 if (!ck_lz_parse_desc(z, end - pos - CK_RB_HEADER, d) || !ck_lz_walk(z, end - pos - CK_RB_HEADER, d, &k, &bound) ||
                     CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
                 has_lz4 = true;
+            } else if (codec == CK_RB_ZSTD) {
+                ck_zs_frame f;
+                if (!ck_zs_header(z, end - pos - CK_RB_HEADER, f) || !ck_zs_walk(z, end - pos - CK_RB_HEADER, f, &bound) ||
+                    CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
+                has_zs = true;
             } else {
                 u32 hdr = 0, isize = 0;
                 if (ck_gz_member(z, end - pos - CK_RB_HEADER, &hdr, &isize) && CK_RB_HEADER + (unsigned long long)isize <= 0x7fffffffull) bound = isize;
@@ -804,6 +812,8 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
         CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, nb, h->d_rb_batch_bad);
         if (has_lz4) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
         if (has_gz) CKL(h) ck_rb_gzip_kernel<<<(nb + CK_GZ_WARPS - 1) / CK_GZ_WARPS, 32 * CK_GZ_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
+                                                                                                          h->d_rb_batch_bad, h->d_rb_dec_len);
+        if (has_zs) CKL(h) ck_rb_zstd_kernel<<<(nb + CK_ZS_WARPS - 1) / CK_ZS_WARPS, 32 * CK_ZS_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
                                                                                                           h->d_rb_batch_bad, h->d_rb_dec_len);
         CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off, lz ? h->d_rb_dec_off : nullptr,
                                                                         lz ? h->d_rb_dec_len : nullptr, h->d_rb_rec_base, nb,

@@ -12,6 +12,8 @@
 //                        into the batch's slot behind the raw bytes (ck_lz4.cuh)
 //   ck_rb_gzip_kernel    (a fetch holding gzip batches only) warp per gzip batch: its records section, one gzip member,
 //                        inflated into the batch's slot (ck_inflate.cuh) and checked against the trailer's CRC32
+//   ck_rb_zstd_kernel    (a fetch holding zstd batches only) warp per zstd batch: its records section, one zstd frame,
+//                        decoded into the batch's slot (ck_zstd.cuh)
 //   ck_rb_split_kernel   thread per batch: hop from record to record (each starts with its own varint length)
 //   ck_rb_fields_kernel  thread per record: zig-zag varints -> key span, value span, the `correlation_id` header span
 // The walker then reads every value where it lies inside the buffer (ck_view.len): the raw bytes, or a compressed batch's
@@ -24,13 +26,15 @@
 
 #include "ck_lz4.cuh"
 #include "ck_inflate.cuh"
+#include "ck_zstd.cuh"
 
 #define CK_CRC_POLY 0x82F63B78u      // CRC32C (Castagnoli), reflected
 #define CK_CRC32_POLY 0xEDB88320u    // CRC32 (IEEE), reflected: gzip's
 #define CK_RB_HEADER 61u
 #define CK_RB_CRC_FROM 21u
 #define CK_RB_GZIP 1u                // attributes & 7: Kafka's codec ids of gzip
-#define CK_RB_LZ4 3u                 // and LZ4
+#define CK_RB_LZ4 3u                 // LZ4
+#define CK_RB_ZSTD 4u                // and zstd
 
 // ---- CRC32 ------------------------------------------------------------------------------------------------------------
 // Generic over the reflected polynomial P: CRC32C (Castagnoli, the batch CRC) by default, CRC32 (IEEE, the gzip trailer)
@@ -122,7 +126,7 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
     u32 flen = (u32)(batch_off[w + 1] - batch_off[w]);
     u32 bad = 0;
     u32 codec = flen >= CK_RB_HEADER ? f[22] & 7u : 0u;
-    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_GZIP && codec != CK_RB_LZ4)) bad = 1;   // not magic 2 / snappy, zstd
+    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_GZIP && codec != CK_RB_LZ4 && codec != CK_RB_ZSTD)) bad = 1;   // not magic 2 / snappy
     else {
         u32 c = ck_crc_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
         if (c != ck_be32(f + 17)) bad = 1;
@@ -146,10 +150,10 @@ __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u3
 __device__ __forceinline__ bool ck_rb_is_lz4(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
     return (buf[batch_off[b] + 22] & 7u) == CK_RB_LZ4;
 }
-// a batch whose records section is decoded into a slot: gzip or LZ4
+// a batch whose records section is decoded into a slot: gzip, LZ4 or zstd
 __device__ __forceinline__ bool ck_rb_is_decoded(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
     u32 codec = buf[batch_off[b] + 22] & 7u;
-    return codec == CK_RB_GZIP || codec == CK_RB_LZ4;
+    return codec == CK_RB_GZIP || codec == CK_RB_LZ4 || codec == CK_RB_ZSTD;
 }
 
 // warp per batch of a fetch that holds LZ4 batches; the uncompressed ones and those the CRC check refused are skipped.
@@ -221,9 +225,31 @@ ck_rb_gzip_kernel(u8* buf, const long long* __restrict__ batch_off, const long l
     if (lane == 0) { dec_len[w] = ok ? (u32)r : 0u; if (!ok) batch_bad[w] = 1; }
 }
 
+// warp per batch of a fetch that holds zstd batches (CK_ZS_WARPS per block, each with its Huffman and sequence tables in
+// shared memory); the others and those the CRC check refused are skipped.  dec_off[b] .. dec_off[b+1]: the slot of batch
+// b, sized by the host's walk of the frame's blocks (ck_zs_walk: raw and RLE blocks their size, compressed blocks
+// Block_Maximum_Size), so that every compressed block has room for its literals at the end of its reservation.  The
+// records section is one zstd frame: its header parsed and its blocks walked again, and refused unless the walk's bound is
+// the slot's size (the host gives an empty slot to a frame it refuses, and a valid frame of empty blocks has one too),
+// then decoded into the slot (ck_zs_decode: libzstd's verdict on every block), its output equal to Frame_Content_Size
+// when the frame carries one and its XXH64 (four lanes, one accumulator each) to the checksum when present, the frame
+// ending exactly at the batch's end.  dec_len[b] = the decoded length; anything else marks the batch bad
+#define CK_ZS_WARPS 3u
+__global__ void __launch_bounds__(32 * CK_ZS_WARPS)
+ck_rb_zstd_kernel(u8* buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off, u32 nb,
+                  u32* __restrict__ batch_bad, u32* __restrict__ dec_len) {
+    __shared__ ck_zs_ws ws[CK_ZS_WARPS];
+    u32 wi = threadIdx.x >> 5, w = blockIdx.x * CK_ZS_WARPS + wi, lane = threadIdx.x & 31;
+    if (w >= nb || batch_bad[w] || (buf[batch_off[w] + 22] & 7u) != CK_RB_ZSTD) return;
+    const u8* z = buf + batch_off[w] + CK_RB_HEADER;
+    unsigned long long zn = (unsigned long long)(batch_off[w + 1] - batch_off[w]) - CK_RB_HEADER;
+    long long r = ck_zs_decode(z, zn, buf + dec_off[w], (unsigned long long)(dec_off[w + 1] - dec_off[w]), ws[wi], lane);
+    if (lane == 0) { dec_len[w] = r >= 0 ? (u32)r : 0u; if (r < 0) batch_bad[w] = 1; }
+}
+
 // thread per batch: where does each record start.  rec_base[b] = records in the batches before b (host prefix sum of
 // the recordsCount header fields); a batch whose records do not add up to its records section is marked bad.  The records
-// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for a gzip or LZ4 batch (dec_off given) its decoded
+// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for a gzip, LZ4 or zstd batch (dec_off given) its decoded
 // slot [dec_off[b], dec_off[b] + dec_len[b])
 __global__ void __launch_bounds__(128)
 ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off,

@@ -102,7 +102,7 @@ int  ck_fetch_groups(ck_handle* h, uint32_t* host_order, uint32_t* host_key_coun
 
 /* Kafka RecordBatch v2 framing on the device (reference: aiokafka under broker.subscriber / broker.publish,
  * calfkit/worker/worker.py:45-53, calfkit/nodes/base.py:82-87).  ck_submit_recordbatch takes a fetch response's record set
- * (concatenated v2 frames, uncompressed, gzip or LZ4, below) as it came off the socket: one H2D copy (the frame index goes through page-locked
+ * (concatenated v2 frames, uncompressed, gzip, LZ4 or zstd, below) as it came off the socket: one H2D copy (the frame index goes through page-locked
  * staging the handle owns: nothing waits for the stream), then CRC32C verification, record split and
  * zig-zag varint field decode on the device; the walker reads each value where it lies.  Records of a frame that fails the
  * CRC / framing check get status 6 (bad frame); a truncated trailing frame is ignored.  *n_records = records decoded.
@@ -123,10 +123,15 @@ int  ck_fetch_rb_index_async(ck_handle* h, int64_t* val_off, uint32_t* val_len, 
  * point there.  A frame that is malformed in any way, or whose block chain runs past the batch, gets status 6 like a CRC
  * failure.  gzip batches (attributes & 7 = 1) are inflated the same way: the records section is one gzip member (RFC 1952
  * / 1951, exactly what zlib's inflate accepts, FHCRC and the trailer's CRC32 and ISIZE checked) inflated into a slot of
- * its ISIZE; a malformed member, or anything after it (a second member included), gets status 6.  Snappy and zstd
- * batches always do.
+ * its ISIZE; a malformed member, or anything after it (a second member included), gets status 6.  zstd batches
+ * (attributes & 7 = 4) are decoded the same way: the records section is one zstd frame (RFC 8878, what libzstd 1.5.5
+ * accepts with default parameters: window up to 2^27 + 1, no dictionary, content size and XXH64 checksum verified when
+ * present) decoded into a slot of the bound the host's walk of its block headers gives (raw and RLE blocks their size,
+ * compressed blocks the block maximum, even when the frame states a smaller content size: the literals are decoded into
+ * the end of that room); a malformed frame, a skippable or second frame, or anything after the frame gets status 6.
+ * Snappy batches always do.
  * ck_fetch_rb_decoded_async: where those slots start in value-offset space (*base) and their bytes (*nbytes; 0 for a fetch
- * without a gzip or LZ4 batch), known as soon as ck_submit_recordbatch returns; with dst given (page-locked, cap >= *nbytes) their
+ * without a gzip, LZ4 or zstd batch), known as soon as ck_submit_recordbatch returns; with dst given (page-locked, cap >= *nbytes) their
  * D2H copy is queued: value offset v >= *base lies at dst[v - *base] after ck_sync. */
 int  ck_fetch_rb_decoded_async(ck_handle* h, uint8_t* dst, uint64_t cap, uint64_t* base, uint64_t* nbytes);
 int  ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uint32_t n, int64_t base_offset, int64_t timestamp_ms,

@@ -1,14 +1,17 @@
-"""Cost of consuming LZ4 and gzip fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
+"""Cost of consuming LZ4, gzip and zstd fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
 
 The step's tool events are framed once by the record form of the frame pass (ck_encode_frames_records), uncompressed and
 with LZ4 (ck_set_option 3 = 3), as a producer would write them to the tool's input topic; the gzip fetch is the same
 step's uncompressed frames with every records section recompressed on the host by zlib at level 6 (the level Java's
-GZIPOutputStream uses), one member per batch.  Three legs, alternating, two runs each, consume one of those fetch
-responses per step:
+GZIPOutputStream uses), one member per batch; the zstd fetch is the same with every records section recompressed by
+libzstd at level 3 (Kafka's default zstd level) and fed to it in 64 KB pieces, so that its frames carry no content size
+(the zstd leg is left out, and reported as not measured, when libzstd.so.1 cannot be loaded).  Four legs, alternating,
+two runs each, consume one of those fetch responses per step:
   plain  ck_submit_recordbatch over the uncompressed frames + plan + the copies a Lane makes (results, record index)
   lz4    the same over the LZ4 frames: their records sections are decoded on the device, and the decoded region is
          copied back with the results (ck_fetch_rb_decoded_async)
   gzip   the same over the gzip frames (inflated on the device)
+  zstd   the same over the zstd frames (decoded on the device)
 Per leg: step time (CUDA events around the whole step, copies included), the fetch and walk kernels (profile timer
 "walk": CRC, decode, split, fields and the walker), each decode alone (walk of the leg minus walk of plain), events/s,
 and H2D / D2H bytes per step.  Prints one JSON line with the card name and power limit read in the same run.
@@ -73,6 +76,27 @@ def gzip_frames(buf: bytes) -> bytes:
 
 sys.path.insert(0, ROOT)
 fetch["gzip"] = gzip_frames(fetch["plain"])
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import zstd_ref  # noqa: E402
+
+
+def zstd_frames(buf: bytes) -> bytes:
+    """every frame's records section as one zstd frame (libzstd level 3, streamed in 64 KB pieces), attributes codec 4"""
+    from oracle import kafka_batch as kb
+    out, pos = [], 0
+    while pos + 12 <= len(buf):
+        end = pos + 12 + int.from_bytes(buf[pos + 8:pos + 12], "big")
+        f = buf[pos:end]
+        sec = zstd_ref.stream(f[61:], piece=64 << 10, level=3)
+        covered = struct.pack(">h", (struct.unpack_from(">h", f, 21)[0] & ~7) | 4) + f[23:61] + sec
+        out.append(f[:8] + struct.pack(">i", len(covered) + 9) + f[12:17] + struct.pack(">I", kb.crc32c(covered)) + covered)
+        pos = end
+    return b"".join(out)
+
+
+if zstd_ref.lib() is not None:
+    fetch["zstd"] = zstd_frames(fetch["plain"])
+LEGS = [k for k in ("plain", "lz4", "gzip", "zstd") if k in fetch]
 
 e = BatchEngine(0, max_records=n, max_in_bytes=len(fetch["plain"]) + 4096)
 e.register_topics(TOPICS, num_partitions=8)
@@ -130,14 +154,16 @@ def leg(name: str, steps: int = 5) -> dict:
 
 
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
-res = {"events": n, "gpu": q.stdout.strip(), "fetch_bytes": {k: len(v) for k, v in fetch.items()}, "runs": []}
+res = {"events": n, "gpu": q.stdout.strip(), "libzstd": zstd_ref.version() if "zstd" in fetch else None,
+       "fetch_bytes": {k: len(v) for k, v in fetch.items()}, "runs": []}
 t0 = time.time()
 for _ in range(2):
-    for name in ("plain", "lz4", "gzip"):
+    for name in LEGS:
         res["runs"].append({"leg": name, **leg(name)})
 res["wall_s"] = round(time.time() - t0, 1)
-walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k in ("plain", "lz4", "gzip")}
+walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k in LEGS}
 res["lz4_decode_ms"] = round(walk["lz4"] - walk["plain"], 3)
 res["gzip_decode_ms"] = round(walk["gzip"] - walk["plain"], 3)
+res["zstd_decode_ms"] = round(walk["zstd"] - walk["plain"], 3) if "zstd" in walk else "not measured"
 res["decoded_bytes"] = {k: int(b.nbytes) for k, b in b_dec.items()}
 print(json.dumps(res))
