@@ -43,7 +43,7 @@ EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_registe
            "ck_sync", "ck_out_size", "ck_fetch_columns", "ck_fetch_output", "ck_fetch_overlay", "ck_fetch_topic_hist", "ck_stream",
            "ck_device_buffers", "ck_device_buffers2", "ck_profile", "ck_profile_read", "ck_fetch_cols",
            "ck_host_alloc", "ck_host_free", "ck_canon_stats", "ck_fetch_output_async",
-           "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_reset", "ck_submit_recordbatch",
+           "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_compact", "ck_gate_reset", "ck_submit_recordbatch",
            "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option",
            "ck_set_frame_topics", "ck_encode_frames", "ck_encode_frames_records", "ck_frames_size", "ck_fetch_frames_async",
            "ck_fetch_rb_index_async", "ck_fetch_rb_decoded_async"]
@@ -118,6 +118,7 @@ def load() -> C.CDLL:
         "ck_gate_register": (C.c_int, [vp, C.c_uint32]),
         "ck_gate_arrive": (C.c_int, [vp, C.c_uint64]),
         "ck_gate_stats": (C.c_int, [vp, vp]),
+        "ck_gate_compact": (C.c_int, [vp]),
         "ck_gate_reset": (C.c_int, [vp]),
         "ck_fetch_overlay": (C.c_int, [vp, u8p, C.c_uint64, i64p, u32p, C.POINTER(C.c_uint64)]),
         "ck_fetch_topic_hist": (C.c_int, [vp, u32p, C.c_uint32]),

@@ -313,9 +313,11 @@ class BatchEngine:
         self._check(self.lib.ck_set_option(self.h, 1, 1 if on else 0))
 
     # ---- aggregation gate on the device (csrc/ck_gate.cuh; reference nodes/agent.py:57-68) ---------------------------
-    def gate_create(self, max_entries: int = 1 << 14, max_slots: int | None = None, arena_bytes: int = 256 << 20) -> None:
-        self._check(self.lib.ck_gate_create(self.h, max_entries, max_slots if max_slots is not None else 16 * max_entries, arena_bytes))
-        self.gate_arena_bytes = arena_bytes
+    def gate_create(self, max_entries: int = 1 << 14, max_slots: int | None = None, arena_bytes: int = 128 << 20) -> None:
+        """the device holds two arenas of arena_bytes (and two entry and slot arrays): gate_compact moves between them"""
+        max_slots = max_slots if max_slots is not None else 16 * max_entries
+        self._check(self.lib.ck_gate_create(self.h, max_entries, max_slots, arena_bytes))
+        self.gate_max_entries, self.gate_max_slots, self.gate_arena_bytes = max_entries, max_slots, arena_bytes
 
     def gate_register(self, min_pending: int = 2) -> None:
         """after fanout_plan: every record that went out as list[Call] becomes a pending entry of the gate"""
@@ -326,12 +328,22 @@ class BatchEngine:
         self._check(self.lib.ck_gate_arrive(self.h, stamp_base))
 
     def gate_stats(self) -> dict[str, int]:
+        """`failures`: fan-outs the last gate_register could not hold, and tool returns or merges of the last gate_arrive
+        the arena could not hold (those records are declined); the next register / arrive call starts again from 0"""
         out = np.zeros(5, dtype=np.uint64)
         self._check(self.lib.ck_gate_stats(self.h, ptr(out)))
-        st = dict(zip(["entries_used", "slots_used", "arena_used", "live", "failures"], (int(x) for x in out)))
-        if st["failures"]:
-            raise EngineError(f"aggregation gate out of capacity ({st}): raise max_entries / max_slots / arena_bytes")
-        return st
+        return dict(zip(["entries_used", "slots_used", "arena_used", "live", "failures"], (int(x) for x in out)))
+
+    def gate_compact(self, room: int = 0, force: bool = False) -> bool:
+        """give back what finished fan-outs used once entries, slots or arena bytes in use pass half of what the gate
+        holds, or once fewer than `room` entries are left (the records of a batch about to be registered); always with
+        force.  Returns whether it compacted"""
+        st = self.gate_stats()
+        if not (force or 2 * st["entries_used"] > self.gate_max_entries or 2 * st["slots_used"] > self.gate_max_slots
+                or 2 * st["arena_used"] > self.gate_arena_bytes or st["entries_used"] + room > self.gate_max_entries):
+            return False
+        self._check(self.lib.ck_gate_compact(self.h))
+        return True
 
     def gate_reset(self) -> None:
         self._check(self.lib.ck_gate_reset(self.h))

@@ -188,12 +188,13 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
         if gated:
             # the aggregation gate runs on the device: of the N tool returns of a fan-out N-1 end here as Silent without ever
             # becoming Python objects; the completing one comes back as the envelope carrying base_state + collected results
+            engine.gate_compact()           # gives back what finished fan-outs used once the gate is half full
             engine.gate_arrive(self._gate_stamp)
             self._gate_stamp += len(records)
             merged_env = engine.fetch()
-            st = engine.gate_stats()
-            if st["live"] == 0 and st["arena_used"] > engine.gate_arena_bytes // 2:
-                engine.gate_reset()
+            failed = engine.gate_stats()["failures"]
+            if failed:
+                logger.error("aggregation gate: %d tool results found no room in the arena; their fan-outs are declined", failed)
         cols = merged_env.cols if merged_env is not None else engine.columns()
         mv = memoryview(data)
         ovl = engine.overlay()          # records that arrived in another spelling: their canonical re-emission (the columns refer to it)
@@ -255,6 +256,8 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
             d2, o2 = pack_records(recs2)
             saved_topics = self._use_registry(engine, override_registry) if override_registry is not None else None
             try:
+                if kind == "fanout" and gated:
+                    engine.gate_compact(room=len(items))        # every record of the batch may register a fan-out
                 engine.submit(d2, o2)                                                        # re-validated on the device
                 seed = int(np.random.SeedSequence().entropy) & ((1 << 63) - 1)
                 if kind == "fanout":
@@ -266,6 +269,8 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
                 else:
                     engine.tailcall_plan(now_ms, seed)
                 out = engine.fetch()
+                if kind == "fanout" and gated and (failed := engine.gate_stats()["failures"]):
+                    logger.error("aggregation gate full: %d fan-outs were not registered; their tool returns will pass through", failed)
                 publishes = list(out.publishes())                 # topic ids are resolved against the registry in force
             finally:
                 if saved_topics is not None:

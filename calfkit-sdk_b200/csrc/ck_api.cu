@@ -39,6 +39,9 @@ struct ck_handle {
     u32* d_topic_hist = nullptr;
     // aggregation gate (allocated by ck_gate_create)
     ck_gate gate{}; bool gate_set = false; u32* d_rec_entry = nullptr;
+    ck_gate gate_spare{};               // the entries, slots and arena ck_gate_compact moves the live fan-outs into
+    u32* d_gate_src = nullptr;          // [max_entries] compaction: old index of every new entry
+    unsigned long long gate_reg_seq = 0;    // records registered so far: registration order of the entries
     // peer exchange (ck_comm_create)
     u8* d_recv = nullptr; ck_xpeers peers{}; void* peer_opened[CK_X_MAXWORLD] = {nullptr}; u32 comm_rank = 0, comm_world = 0, max_fwd = 0, x_nb = 0;
     unsigned long long region_stride = 0, region_data_cap = 0; u32* d_x_overflow = nullptr; bool comm_ready = false;
@@ -196,7 +199,8 @@ extern "C" void ck_destroy(ck_handle* h) {
                     h->d_tab_len, h->d_tab_id, h->d_tab_names, h->d_x_hist, h->d_x_base, h->d_x_nbytes, h->d_x_src_off, h->d_x_len, h->d_x_dst_off,
                     h->d_x_len32, h->d_x_pub, h->d_x_tile, h->d_x_grand, h->d_x_grand2};
     for (void* p : ptrs) if (p) cudaFree(p);
-    void* gptrs[] = {h->gate.keys, h->gate.vals, h->gate.entries, h->gate.slots, h->gate.arena, h->gate.ctr, h->d_rec_entry,
+    void* gptrs[] = {h->gate.keys, h->gate.entries, h->gate.slots, h->gate.arena, h->gate.ctr, h->d_rec_entry,
+                     h->gate_spare.entries, h->gate_spare.slots, h->gate_spare.arena, h->d_gate_src,
                      h->d_rb_batch_off, h->d_rb_rec_pos, h->d_rb_key_off, h->d_rb_corr_off, h->d_rb_rec_base, h->d_rb_batch_bad,
                      h->d_g_hist, h->d_g_o1, h->d_g_o2, h->d_g_keys, h->d_g_base, h->d_g_tile, h->d_g_grand,
                      h->d_rb_rec_batch, h->d_rb_val_len, h->d_rb_rec_bad, h->d_rb_key_len, h->d_rb_corr_len,
@@ -1182,20 +1186,27 @@ extern "C" int ck_gate_create(ck_handle* h, uint32_t max_entries, uint32_t max_s
     cudaSetDevice(h->device);
     if (h->gate_set) return fail(h, "ck_gate_create: already created");
     if (arena_bytes >= (1ull << 32)) return fail(h, "ck_gate_create: arena must be smaller than 4 GiB (32-bit segment offsets)");
+    if (max_entries == 0 || max_entries > (1u << 28)) return fail(h, "ck_gate_create: max_entries must be in [1, 2^28]");
     ck_gate g{};
     u32 cap = 64; while (cap < 4 * (uint64_t)max_entries) cap <<= 1;
     g.cap = cap; g.max_entries = max_entries; g.max_slots = max_slots; g.arena_cap = arena_bytes;
+    ck_gate s = g;
     CUDA_TRY(h, cudaMalloc((void**)&g.keys, sizeof(unsigned long long) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&g.vals, sizeof(u32) * cap));
     CUDA_TRY(h, cudaMalloc((void**)&g.entries, sizeof(ck_gate_entry) * (size_t)max_entries));
     CUDA_TRY(h, cudaMalloc((void**)&g.slots, sizeof(ck_gate_slot) * (size_t)max_slots));
     CUDA_TRY(h, cudaMalloc((void**)&g.arena, arena_bytes + CK_PAD));
     CUDA_TRY(h, cudaMalloc((void**)&g.ctr, sizeof(unsigned long long) * 8));
+    // the second set of buffers for ck_gate_compact: the gate holds twice the entries, slots and arena it is sized for
+    CUDA_TRY(h, cudaMalloc((void**)&s.entries, sizeof(ck_gate_entry) * (size_t)max_entries));
+    CUDA_TRY(h, cudaMalloc((void**)&s.slots, sizeof(ck_gate_slot) * (size_t)max_slots));
+    CUDA_TRY(h, cudaMalloc((void**)&s.arena, arena_bytes + CK_PAD));
+    s.keys = g.keys; s.ctr = g.ctr;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_gate_src, sizeof(u32) * (size_t)max_entries));
     CUDA_TRY(h, cudaMalloc((void**)&h->d_rec_entry, sizeof(u32) * (size_t)h->max_records));
     CUDA_TRY(h, cudaMemsetAsync(g.keys, 0, sizeof(unsigned long long) * cap, h->stream));
     CUDA_TRY(h, cudaMemsetAsync(g.ctr, 0, sizeof(unsigned long long) * 8, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    h->gate = g; h->gate_set = true;
+    h->gate = g; h->gate_spare = s; h->gate_set = true;
     return 0;
 }
 
@@ -1204,6 +1215,21 @@ extern "C" int ck_gate_reset(ck_handle* h) {
     if (!h->gate_set) return fail(h, "ck_gate_reset: call ck_gate_create first");
     CUDA_TRY(h, cudaMemsetAsync(h->gate.keys, 0, sizeof(unsigned long long) * h->gate.cap, h->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->gate.ctr, 0, sizeof(unsigned long long) * 8, h->stream));
+    return 0;
+}
+
+// give back what finished fan-outs used: the live entries (with their slots, blobs and collected values) move to the
+// spare buffers, which become the gate's, and the key table is rebuilt from them.  Asynchronous; the pending state
+// and every later result are exactly what they would have been without it.
+extern "C" int ck_gate_compact(ck_handle* h) {
+    cudaSetDevice(h->device);
+    if (!h->gate_set) return fail(h, "ck_gate_compact: call ck_gate_create first");
+    ck_gate g = h->gate, d = h->gate_spare;
+    CUDA_TRY(h, cudaMemsetAsync(g.keys, 0, sizeof(unsigned long long) * g.cap, h->stream));
+    CKL(h) ck_gate_compact_plan_kernel<<<1, 1024, 0, h->stream>>>(g, d, h->d_gate_src);
+    CKL(h) ck_gate_compact_move_kernel<<<(g.max_entries + 7) / 8, 256, 0, h->stream>>>(g, d, h->d_gate_src);
+    CUDA_TRY(h, cudaGetLastError());
+    h->gate = d; h->gate_spare = g;
     return 0;
 }
 
@@ -1220,9 +1246,12 @@ extern "C" int ck_gate_register(ck_handle* h, uint32_t min_pending) {
     cudaSetDevice(h->device);
     if (!h->gate_set) return fail(h, "ck_gate_register: call ck_gate_create first");
     u32 n = h->n;
+    CUDA_TRY(h, cudaMemsetAsync(h->gate.ctr + 4, 0, sizeof(unsigned long long), h->stream));   // failures of this call
     if (!n) return 0;
     KTimer t(h, CK_K_FANOUT);
-    CKL(h) ck_gate_register_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, min_pending, h->d_rec_entry);
+    CKL(h) ck_gate_register_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, min_pending,
+                                                                              h->gate_reg_seq, h->d_rec_entry);
+    h->gate_reg_seq += n;
     CKL(h) ck_gate_copy_base_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(view_of(h), n, h->gate, h->d_rec_entry);
     CUDA_TRY(h, cudaGetLastError());
     return 0;
@@ -1236,6 +1265,7 @@ extern "C" int ck_gate_arrive(ck_handle* h, uint64_t stamp_base) {
     if (!h->gate_set) return fail(h, "ck_gate_arrive: call ck_gate_create first");
     if (!h->tool_set) return fail(h, "ck_gate_arrive: call ck_set_tool_node (publish topic) first");
     u32 n = h->n;
+    CUDA_TRY(h, cudaMemsetAsync(h->gate.ctr + 4, 0, sizeof(unsigned long long), h->stream));   // failures of this call
     {
         KTimer t(h, CK_K_PLAN);
         if (n) {

@@ -7,9 +7,11 @@
 // of the arriving state; N-1 of the N arrivals end in Silent, the one that completes the set continues with
 // `base_state` + the collected results (dict insertion order = order of collection) and the entry is deleted.
 //
-// Here the pending table lives in HBM: an open-addressing hash table keyed by the 64-bit FNV-1a of the correlation id
-// (bytes verified on a hit), one entry per pending fan-out (base-state blob + expected-id slots) and a bump-allocated
-// byte arena for the blobs.  A whole batch of arrivals is processed at once and still reproduces the reference's
+// Here the pending table lives in HBM: an open-addressing hash table over the 64-bit FNV-1a of the correlation id, one
+// 64-bit word per key slot that holds the hash's high 32 bits and the entry index together (bytes verified on a hit), one
+// entry per pending fan-out (base-state blob + expected-id slots) and a bump-allocated byte arena for the blobs.
+// Entries, slots and arena bytes are only ever appended; ck_gate_compact moves the live ones to a second set of buffers
+// and rebuilds the key table, which gives back everything finished fan-outs used.  A whole batch of arrivals is processed at once and still reproduces the reference's
 // one-at-a-time semantics exactly, through arrival stamps (stamp = records consumed before this batch + index in it):
 //   probe    every arrival finds its entry and does atomicMin(slot.stamp, own stamp) on the slots of the expected ids
 //            it carries: after the kernel each slot holds the stamp of the FIRST arrival that carried it — the one the
@@ -37,6 +39,7 @@ struct ck_gate_slot {               // one expected tool_call_id of a pending fa
 struct ck_gate_entry {
     unsigned long long base_off;    // base-state blob in the arena
     unsigned long long corr_off;    // correlation id bytes in the arena
+    unsigned long long reg;         // registration order (records registered before its batch + index in it): the later wins
     u32 base_len, corr_len;
     u32 tr_close;                   // offset inside the blob of the closing '}' of tool_results
     u32 tr_empty;                   // tool_results was {} at fan-out
@@ -44,16 +47,17 @@ struct ck_gate_entry {
     u32 live, pad;
 };
 struct ck_gate {
-    unsigned long long* keys;       // [cap] 64-bit correlation hashes, 0 = empty
-    u32* vals;                      // [cap] entry index
+    unsigned long long* keys;       // [cap] (hash >> 32) << 32 | (entry index + 1), 0 = empty
     u32 cap;                        // power of two
     ck_gate_entry* entries; u32 max_entries;
     ck_gate_slot* slots; u32 max_slots;
     u8* arena; unsigned long long arena_cap;
-    // counters: [0] entries used, [1] slots used, [2] arena bytes used, [3] live entries, [4] capacity failures
+    // counters: [0] entries used, [1] slots used, [2] arena bytes used, [3] live entries,
+    // [4] capacity failures of the last register / arrive call
     unsigned long long* ctr;
 };
 
+#define CK_GATE_TAG(h) ((h) >> 32)
 __device__ __forceinline__ unsigned long long ck_fnv64(Rd& r, u32 off, u32 len) {
     unsigned long long h = 14695981039346656037ull;
     for (u32 i = 0; i < len; i++) h = (h ^ r.at(off + i)) * 1099511628211ull;
@@ -63,26 +67,37 @@ __device__ __forceinline__ bool ck_bytes_eq(Rd& r, u32 off, const u8* __restrict
     for (u32 i = 0; i < len; i++) if (r.at(off + i) != q[i]) return false;
     return true;
 }
+// the entry a key word names holds this correlation id; L2 reads: in the register kernel another SM may have published
+// the entry a moment ago
+__device__ __forceinline__ bool ck_gate_same_corr(const ck_gate& g, u32 e, Rd& r, u32 coff, u32 clen) {
+    const ck_gate_entry* en = g.entries + e;
+    if (__ldcg(&en->corr_len) != clen) return false;
+    const u8* q = g.arena + __ldcg(&en->corr_off);
+    for (u32 i = 0; i < clen; i++) if (r.at(coff + i) != __ldcg(q + i)) return false;
+    return true;
+}
 __device__ __forceinline__ int ck_gate_find(const ck_gate& g, Rd& r, u32 coff, u32 clen, unsigned long long h) {
     u32 s = (u32)h & (g.cap - 1);
     for (u32 p = 0; p < g.cap; p++) {
         unsigned long long k = g.keys[s];
         if (k == 0) return -1;
-        if (k == h) {
-            u32 e = g.vals[s];
+        if (CK_GATE_TAG(k) == CK_GATE_TAG(h)) {
+            u32 e = (u32)k - 1;
             const ck_gate_entry& en = g.entries[e];
-            if (en.live && en.corr_len == clen && ck_bytes_eq(r, coff, g.arena + en.corr_off, clen)) return (int)e;
+            if (en.corr_len == clen && ck_bytes_eq(r, coff, g.arena + en.corr_off, clen)) return en.live ? (int)e : -1;   // one key per id
         }
         s = (s + 1) & (g.cap - 1);
     }
     return -1;
 }
+__device__ __forceinline__ unsigned long long ck_pad16(unsigned long long x) { return (x + 15u) & ~15ull; }
 
 // ---- registration: after the fan-out plan of a batch of post-LLM envelopes, every record that went out as list[Call]
 // (ACTION == FANOUT) becomes a pending entry: base_state = its `state` object, expected ids = its pending tool calls.
 // (a) thread per record: allocate entry, slots and arena space, insert into the table, fill the slots
 __global__ void __launch_bounds__(128)
-ck_gate_register_kernel(ck_view v, u32 n, const u32* __restrict__ cols, u32 stride, ck_gate g, u32 min_pending, u32* __restrict__ rec_entry) {
+ck_gate_register_kernel(ck_view v, u32 n, const u32* __restrict__ cols, u32 stride, ck_gate g, u32 min_pending,
+                        unsigned long long reg_base, u32* __restrict__ rec_entry) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
 #define COL(k) cols[(size_t)(k) * stride + i]
@@ -104,11 +119,15 @@ ck_gate_register_kernel(ck_view v, u32 n, const u32* __restrict__ cols, u32 stri
     if (pending < min_pending || pending == 0) return;
     u32 e = (u32)atomicAdd(&g.ctr[0], 1ull);
     u32 s0 = (u32)atomicAdd(&g.ctr[1], (unsigned long long)pending);
-    unsigned long long need = (unsigned long long)((base_len + 15u) & ~15u) + ((clen + 15u) & ~15u);
+    unsigned long long need = ck_pad16(base_len) + ck_pad16(clen);
     unsigned long long a0 = atomicAdd(&g.ctr[2], need);
-    if (e >= g.max_entries || s0 + pending > g.max_slots || a0 + need > g.arena_cap) { atomicAdd(&g.ctr[4], 1ull); return; }
+    if (e >= g.max_entries || (unsigned long long)s0 + pending > g.max_slots || a0 + need > g.arena_cap) {
+        if (e < g.max_entries) g.entries[e].live = 0;       // allocated but never filled: compaction must not read it as live
+        atomicAdd(&g.ctr[4], 1ull);
+        return;
+    }
     ck_gate_entry en;
-    en.base_off = a0; en.base_len = base_len; en.corr_off = a0 + ((base_len + 15u) & ~15u); en.corr_len = clen;
+    en.base_off = a0; en.base_len = base_len; en.corr_off = a0 + ck_pad16(base_len); en.corr_len = clen; en.reg = reg_base + i;
     en.tr_close = tr + trl - 1 - CK_STATE_OFF; en.tr_empty = (trl == 2); en.n_expected = pending; en.first_slot = s0; en.live = 1; en.pad = 0;
     for (u32 b = 0; b < clen; b++) g.arena[en.corr_off + b] = r.at(coff + b);
     u32 pos = tc + 1, j = 0;
@@ -123,20 +142,35 @@ ck_gate_register_kernel(ck_view v, u32 n, const u32* __restrict__ cols, u32 stri
     }
     g.entries[e] = en;
     __threadfence();
-    // insert: claim an empty key slot, or take over the slot of a (stale) entry with the same correlation id
-    // (dict assignment in the reference: a new PendingToolBatch replaces the old one)
+    // insert: claim an empty key slot, or take over the key slot of the same correlation id from an earlier registration
+    // (dict assignment in the reference: a new PendingToolBatch replaces the old one; within a batch the highest record
+    // index is the later one).  A key word names its entry in the same 64-bit store, so whoever reads the word finds the
+    // entry already written.  An id keeps its key slot for good, and the key table is only rebuilt by ck_gate_compact.
     unsigned long long h = ck_fnv64(r, coff, clen);
+    unsigned long long mine = (CK_GATE_TAG(h) << 32) | (e + 1ull);
     u32 s = (u32)h & (g.cap - 1);
-    for (u32 p = 0; p < g.cap; p++) {
-        unsigned long long prev = atomicCAS(&g.keys[s], 0ull, h);
-        if (prev == 0) { g.vals[s] = e; break; }
-        if (prev == h) {
-            u32 old = g.vals[s];
-            const ck_gate_entry& oe = g.entries[old];
-            bool same = oe.corr_len == clen && ck_bytes_eq(r, coff, g.arena + oe.corr_off, clen);
-            if (same || !oe.live) { if (same && oe.live) { g.entries[old].live = 0; atomicAdd(&g.ctr[3], (unsigned long long)-1ll); } g.vals[s] = e; break; }
+    int won = -1;                                            // -1 still probing, 0 a later registration holds the id, 1 inserted
+    for (u32 p = 0; p < g.cap && won < 0; p++, s = (s + 1) & (g.cap - 1)) {
+        unsigned long long cur = atomicCAS(&g.keys[s], 0ull, mine);
+        if (cur == 0) { won = 1; break; }
+        // the word of a key slot only ever changes to the word of an entry with the same correlation id
+        if (CK_GATE_TAG(cur) != CK_GATE_TAG(h) || !ck_gate_same_corr(g, (u32)cur - 1, r, coff, clen)) continue;
+        while (won < 0) {
+            u32 old = (u32)cur - 1;
+            if (__ldcg(&g.entries[old].reg) > en.reg) { won = 0; break; }
+            unsigned long long prev = atomicCAS(&g.keys[s], cur, mine);
+            if (prev == cur) {
+                won = 1;
+                if (atomicExch(&g.entries[old].live, 0u)) atomicAdd(&g.ctr[3], (unsigned long long)-1ll);
+            } else {
+                cur = prev;
+            }
         }
-        s = (s + 1) & (g.cap - 1);
+    }
+    if (won != 1) {                                          // replaced by a later record of this batch (or no key slot left)
+        g.entries[e].live = 0;
+        if (won < 0) atomicAdd(&g.ctr[4], 1ull);
+        return;
     }
     atomicAdd(&g.ctr[3], 1ull);
     rec_entry[i] = e;
@@ -211,9 +245,9 @@ ck_gate_resolve_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, ck_
     // the first arrival that carried an id is the one the reference collects from: it copies the value into the arena
     ck_gate_each_match(g, en, r, COL(CK_COL_TR_OFF), [&](ck_gate_slot& sl, u32 v0, u32 vl) {
         if (sl.stamp != my) return;
-        unsigned long long need = (vl + 15u) & ~15u;
+        unsigned long long need = ck_pad16(vl);
         unsigned long long a0 = atomicAdd(&g.ctr[2], need);
-        if (a0 + need > g.arena_cap) { atomicAdd(&g.ctr[4], 1ull); return; }
+        if (a0 + need > g.arena_cap) { atomicAdd(&g.ctr[4], 1ull); return; }     // val_len stays 0: the merge declines
         for (u32 b = 0; b < vl; b++) g.arena[a0 + b] = r.at(v0 + b);
         sl.val_off = a0; sl.val_len = vl;
     });
@@ -250,24 +284,35 @@ ck_gate_merge_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, ck_ga
     // piece q = ["," if not first] "id":value ; its rank = number of slots with a smaller stamp; offsets by rank
     // pass 1: every lane handles slots lane, lane+32, ...: rank + length
     u32 total = 0;
-    bool lead_comma = !en.tr_empty;
+    bool lead_comma = !en.tr_empty, missing = false;
     for (u32 base = 0; base < nexp; base += 32) {
         u32 q = base + lane;
         u32 len = 0;
         if (q < nexp) len = 1 + sl[q].id_len + 2 + sl[q].val_len;          // "id": value
+        missing |= __any_sync(0xffffffffu, q < nexp && sl[q].val_len == 0);  // a JSON value is never empty: its copy found no room
         // sum of lengths is order independent
         for (int o = 16; o; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
         total += len;
     }
     total += nexp - 1 + (lead_comma ? 1u : 0u);                            // commas
-    unsigned long long blob = 0;
-    if (lane == 0) {
-        unsigned long long need = (total + 15u) & ~15u;
+    unsigned long long blob = CK_GATE_INF;
+    if (lane == 0 && !missing) {
+        unsigned long long need = ck_pad16(total);
         blob = atomicAdd(&g.ctr[2], need);
-        if (blob + need > g.arena_cap) { atomicAdd(&g.ctr[4], 1ull); blob = CK_GATE_INF; }
+        if (blob + need > g.arena_cap) blob = CK_GATE_INF;
     }
     blob = __shfl_sync(0xffffffffu, blob, 0);
-    if (blob == CK_GATE_INF) { if (lane == 0) { cols[(size_t)CK_COL_STATUS * stride + w] = CK_UNSUPPORTED; cols[(size_t)CK_COL_ACTION * stride + w] = CK_ACT_RAISES; } return; }
+    if (blob == CK_GATE_INF) {
+        // the arena could not hold a collected value or the merged pieces: the record is declined and the fan-out is
+        // given up, so no envelope with a hole in it ever leaves the device
+        if (lane == 0) {
+            if (!missing) atomicAdd(&g.ctr[4], 1ull);                       // a missing value was counted by its copy
+            cols[(size_t)CK_COL_STATUS * stride + w] = CK_UNSUPPORTED; cols[(size_t)CK_COL_ACTION * stride + w] = CK_ACT_RAISES;
+            en.live = 0;
+            atomicAdd(&g.ctr[3], (unsigned long long)-1ll);
+        }
+        return;
+    }
     // pass 2: for every slot, its start = sum of the lengths of all pieces with a smaller stamp (+ commas)
     for (u32 q = 0; q < nexp; q++) {
         unsigned long long sq = sl[q].stamp;
@@ -303,6 +348,86 @@ ck_gate_merge_kernel(ck_view v, u32 n, u32* __restrict__ cols, u32 stride, ck_ga
         else pay_len[w] = sw.total;
         en.live = 0;                                                          // del self._pending_batches[correlation_id]
         atomicAdd(&g.ctr[3], (unsigned long long)-1ll);
+    }
+}
+
+// ---- compaction: the live entries, their slots, base blobs, correlation bytes and collected values move to the other
+// set of buffers `d` (same capacities, same counters and key table), in index order; stamps and values are unchanged.
+// The host clears the key table first and swaps the buffers afterwards.
+__device__ __forceinline__ unsigned long long ck_gate_live_bytes(const ck_gate& g, const ck_gate_entry& en) {
+    unsigned long long b = ck_pad16(en.base_len) + ck_pad16(en.corr_len);
+    for (u32 q = 0; q < en.n_expected; q++) { u32 vl = g.slots[en.first_slot + q].val_len; if (vl) b += ck_pad16(vl); }
+    return b;
+}
+// (a) one block: new entry index, first slot and arena offset of every live entry (block scan); src[new] = old index
+__global__ void __launch_bounds__(1024)
+ck_gate_compact_plan_kernel(ck_gate g, ck_gate d, u32* __restrict__ src) {
+    __shared__ u32 s_e[32], s_s[32];
+    __shared__ unsigned long long s_a[32];
+    u32 t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    unsigned long long used = g.ctr[0];
+    u32 ne = used < g.max_entries ? (u32)used : g.max_entries;
+    u32 per = (ne + blockDim.x - 1) / blockDim.x, lo = min(t * per, ne), hi = min(lo + per, ne);
+    u32 ce = 0, cs = 0; unsigned long long ca = 0;
+    for (u32 e = lo; e < hi; e++) {
+        const ck_gate_entry& en = g.entries[e];
+        if (!en.live) continue;
+        ce++; cs += en.n_expected; ca += ck_gate_live_bytes(g, en);
+    }
+    u32 ie = ce, is = cs; unsigned long long ia = ca;                      // inclusive scan in the warp
+    for (int o = 1; o < 32; o <<= 1) {
+        u32 x = __shfl_up_sync(0xffffffffu, ie, o), y = __shfl_up_sync(0xffffffffu, is, o);
+        unsigned long long z = __shfl_up_sync(0xffffffffu, ia, o);
+        if (lane >= (u32)o) { ie += x; is += y; ia += z; }
+    }
+    if (lane == 31) { s_e[wid] = ie; s_s[wid] = is; s_a[wid] = ia; }
+    __syncthreads();                                                       // every thread has read ctr[0] by now
+    if (wid == 0) {
+        u32 nw = blockDim.x >> 5;
+        u32 x = lane < nw ? s_e[lane] : 0, y = lane < nw ? s_s[lane] : 0; unsigned long long z = lane < nw ? s_a[lane] : 0;
+        for (int o = 1; o < 32; o <<= 1) {
+            u32 x2 = __shfl_up_sync(0xffffffffu, x, o), y2 = __shfl_up_sync(0xffffffffu, y, o);
+            unsigned long long z2 = __shfl_up_sync(0xffffffffu, z, o);
+            if (lane >= (u32)o) { x += x2; y += y2; z += z2; }
+        }
+        if (lane < nw) { s_e[lane] = x; s_s[lane] = y; s_a[lane] = z; }
+    }
+    __syncthreads();
+    u32 oe = ie - ce + (wid ? s_e[wid - 1] : 0u), os = is - cs + (wid ? s_s[wid - 1] : 0u);
+    unsigned long long oa = ia - ca + (wid ? s_a[wid - 1] : 0ull);
+    for (u32 e = lo; e < hi; e++) {
+        const ck_gate_entry& en = g.entries[e];
+        if (!en.live) continue;
+        ck_gate_entry m = en;
+        m.first_slot = os; m.base_off = oa; m.corr_off = oa + ck_pad16(en.base_len);
+        d.entries[oe] = m; src[oe] = e;
+        oe++; os += en.n_expected; oa += ck_gate_live_bytes(g, en);
+    }
+    if (t == blockDim.x - 1) { g.ctr[0] = oe; g.ctr[1] = os; g.ctr[2] = oa; g.ctr[3] = oe; }
+}
+// (b) warp per live entry: copy blobs, slots and collected values (laid out after the correlation bytes in slot order),
+// then insert its key into the cleared table
+__global__ void __launch_bounds__(256)
+ck_gate_compact_move_kernel(ck_gate g, ck_gate d, const u32* __restrict__ src) {
+    u32 w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (w >= d.ctr[0]) return;
+    const ck_gate_entry& ne = d.entries[w];
+    const ck_gate_entry& oe = g.entries[src[w]];
+    ck_warp_copy(d.arena + ne.base_off, g.arena + oe.base_off, ne.base_len, lane);
+    ck_warp_copy(d.arena + ne.corr_off, g.arena + oe.corr_off, ne.corr_len, lane);
+    unsigned long long vo = ne.corr_off + ck_pad16(ne.corr_len);
+    for (u32 q = 0; q < ne.n_expected; q++) {
+        ck_gate_slot sl = g.slots[oe.first_slot + q];
+        if (sl.val_len) { ck_warp_copy(d.arena + vo, g.arena + sl.val_off, sl.val_len, lane); sl.val_off = vo; vo += ck_pad16(sl.val_len); }
+        if (lane == 0) d.slots[ne.first_slot + q] = sl;
+    }
+    if (lane == 0) {
+        Rd r; r.init(g.arena + oe.corr_off, oe.corr_len);
+        unsigned long long h = ck_fnv64(r, 0, oe.corr_len);
+        unsigned long long word = (CK_GATE_TAG(h) << 32) | (w + 1ull);
+        u32 s = (u32)h & (d.cap - 1);
+        for (u32 p = 0; p < d.cap; p++, s = (s + 1) & (d.cap - 1))
+            if (atomicCAS(&d.keys[s], 0ull, word) == 0ull) break;
     }
 }
 

@@ -194,20 +194,29 @@ int  ck_tailcall_plan(ck_handle* h, uint64_t unix_ms, uint64_t seed);
 /* aggregation gate on the device (calfkit/nodes/agent.py:57-68 _parallel_state_aggregation, models/state.py:127-141
  * PendingToolBatch): an HBM-resident table keyed by correlation id holding, per pending fan-out, the state the agent fanned
  * out from and the expected tool_call_ids with the results collected so far.
- *   ck_gate_create    sizes the table (entries = concurrent fan-outs, slots = sum of their expected ids, arena < 4 GiB)
+ *   ck_gate_create    sizes the table (entries = concurrent fan-outs, slots = sum of their expected ids, arena < 4 GiB);
+ *                     entries, slots and arena are allocated twice (the second set is what ck_gate_compact moves into)
  *   ck_gate_register  after ck_fanout_plan on a batch of post-LLM envelopes: every record that went out as list[Call]
- *                     (ACTION == CK_ACT_FANOUT) becomes a pending entry (a new one replaces an old one for the same id)
+ *                     (ACTION == CK_ACT_FANOUT) becomes a pending entry (a new one replaces an old one for the same id;
+ *                     within one batch the highest record index wins).  A fan-out that finds no room is not registered
+ *                     and counted as a failure: its tool returns pass through
  *   ck_gate_arrive    on a submitted batch of records arriving at the agent's topic; stamp_base = records this node
  *                     consumed before this batch (arrival order across and inside batches).  Column ACTION afterwards:
  *                     CK_ACT_SILENT (collected, still incomplete; only the handler-return publish to publish_topic),
  *                     9 = complete (payload i = inbound envelope carrying base_state + the collected results in order
- *                     of collection; the entry is deleted), 10 = no pending fan-out (continue with the inbound state)
- *   ck_gate_stats     out5 = {entries used, slots used, arena bytes used, live entries, capacity failures}
- *   ck_gate_reset     forget everything (e.g. when live == 0 and the arena is mostly used) */
+ *                     of collection; the entry is deleted), 10 = no pending fan-out (continue with the inbound state).
+ *                     A completing record whose results found no room in the arena is declined (STATUS CK_UNSUPPORTED,
+ *                     ACTION CK_ACT_RAISES), counted as a failure, and its entry is deleted
+ *   ck_gate_stats     out5 = {entries used, slots used, arena bytes used, live entries, capacity failures of the last
+ *                     register / arrive call}
+ *   ck_gate_compact   moves the live entries to fresh space and rebuilds the key table: gives back what finished
+ *                     fan-outs used (run it when entries, slots or arena bytes used pass a threshold)
+ *   ck_gate_reset     forget everything */
 int  ck_gate_create(ck_handle* h, uint32_t max_entries, uint32_t max_slots, uint64_t arena_bytes);
 int  ck_gate_register(ck_handle* h, uint32_t min_pending /* 2 = the reference's rule; 1 also registers single Calls */);
 int  ck_gate_arrive(ck_handle* h, uint64_t stamp_base);
 int  ck_gate_stats(ck_handle* h, uint64_t* out5);
+int  ck_gate_compact(ck_handle* h);
 int  ck_gate_reset(ck_handle* h);
 /* cross-partition forward over NVLink peer memory (records shard by Kafka partition across the GPUs of a box; reference
  * analogue: producing to a topic-partition another worker process consumes, nodes/base.py:82-87 key=correlation_id).

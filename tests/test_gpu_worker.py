@@ -89,6 +89,59 @@ def test_parallel_fanout_three_tools_and_aggregation():
         assert len(calls[-1].tool_calls) == 3
 
 
+def test_parallel_fanout_many_conversations_small_gate(caplog):
+    """a long-lived agent Worker: 300 conversations, each fanning out to one device-template tool and two host tools,
+    through a Worker whose agent gate holds 16 fan-outs (batch_records=16), so ~300 fan-outs pass through a 16-entry
+    gate.  Every answer is right, and no record is dropped and no batch is retried."""
+    _skip_without_cuda()
+    import logging
+    from calfkit import Agent, Client, Worker, agent_tool
+    from calfkit.models import ToolContext
+    from calfkit.models.messages import ModelResponse, TextPart, ToolCallPart, ToolReturnPart
+    from calfkit.nodes import FunctionModelClient
+
+    @agent_tool
+    def tool_a(x: str) -> str:
+        """a"""
+        return f"A<{x}>"
+
+    @agent_tool(device_template="B<{x}>")
+    def tool_b(x: str) -> str:
+        """b"""
+        return f"B<{x}>"
+
+    @agent_tool
+    def tool_c(ctx: ToolContext, x: str) -> str:
+        """c: contextual tool reading provided deps"""
+        return f"C<{x}:{ctx.deps.provided_deps['tenant']}>"
+
+    def llm(messages, tools):
+        rets = [p for p in getattr(messages[-1], "parts", []) if isinstance(p, ToolReturnPart)]
+        if rets:
+            return ModelResponse(parts=[TextPart(content=" | ".join(str(r.content) for r in rets))])
+        return ModelResponse(parts=[ToolCallPart(tool_name=t.name, args={"x": "v"}) for t in tools])
+
+    async def go():
+        client = Client.connect()
+        agent = Agent("planner", subscribe_topics="planner.input", publish_topic="planner.output",
+                      model_client=FunctionModelClient(llm), tools=[tool_a, tool_b, tool_c])
+        worker = Worker(client, nodes=[agent, tool_a, tool_b, tool_c], batch_records=16)
+        res = []
+        for wave in range(30):                  # ten conversations at a time: at most 10 fan-outs pending at once
+            hs = [await client.invoke_node("go", "planner.input", deps={"tenant": f"t{10 * wave + i}"}) for i in range(10)]
+            await worker.run(until_idle=True)
+            res += [await h.result(timeout=5) for h in hs]
+        await client.close()
+        return res
+
+    with caplog.at_level(logging.WARNING):
+        res = asyncio.run(go())
+    for i, r in enumerate(res):
+        assert r.output == f"A<v> | B<v> | C<v:t{i}>"
+    bad = [rec.getMessage() for rec in caplog.records if rec.levelno >= logging.WARNING and rec.name.startswith("calfkit")]
+    assert not bad, bad[:5]
+
+
 def _three_tools():
     from calfkit import agent_tool
 
