@@ -17,7 +17,12 @@ Two granularities share the topics:
     when the entry is contiguous.
 Kafka's own granularity — record batches — at both ends:
   * `produce_fetch(topic, buf)` enqueues a fetch response's record set (engine.lane.FetchArena); `poll_arena` splits such
-    entries only at frame boundaries and the device checks, splits and decodes them;
+    entries only at frame boundaries and the device checks, splits and decodes them.  Transactions (KIP-98): a record set
+    holds the batches of one or more partitions back to back, `partitions=[(byte start, aborted), ...]` in byte order,
+    where `aborted` is that partition's AbortedTransactions from the fetch response, [(producer id, first offset), ...];
+    `aborted_transactions=aborted` alone is the one-partition case.  Control batches are skipped at every isolation level;
+    a consumer at isolation_level="read_committed" also skips the aborted transactions' batches.  The mask of those is
+    computed once over the whole entry (an aborted producer stays aborted across a split) and sliced with it;
   * `frame_sink(topic, fn)`: `fn(topic, partition_or_None, frame, n_records)` once per produce-ready RecordBatch v2 frame.
     A lane's frames are handed out as they are; per-record Records produced to such a topic are collected and framed by
     the engine's record form at `flush_frames` (the Worker calls it once per step and installs the `framer`).  There is no
@@ -163,10 +168,14 @@ class MemoryBroker:
         for r in records:
             self.produce(r)
 
-    def produce_fetch(self, topic: str, buf) -> None:
-        """a fetch response's record set for one topic (bytes, a uint8 array or an engine.lane.FetchArena)"""
+    def produce_fetch(self, topic: str, buf, aborted_transactions=None, partitions=None) -> None:
+        """a fetch response's record set for one topic (bytes, a uint8 array or an engine.lane.FetchArena), with the
+        AbortedTransactions of its one partition, [(producer id, first offset), ...], or its partitions (see above)"""
         from calfkit.engine.lane import FetchArena
-        fa = buf if isinstance(buf, FetchArena) else FetchArena.of(buf)
+        if isinstance(buf, FetchArena) and (aborted_transactions is not None or partitions is not None):
+            from calfkit.exceptions import EngineError
+            raise EngineError("a FetchArena carries its own partitions: give them to FetchArena.of")
+        fa = buf if isinstance(buf, FetchArena) else FetchArena.of(buf, aborted_transactions=aborted_transactions, partitions=partitions)
         self.arenas[topic].append(fa)
         self.produced += fa.n
 

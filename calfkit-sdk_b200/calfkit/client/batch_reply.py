@@ -17,7 +17,7 @@ from pydantic import TypeAdapter
 
 from calfkit.broker import Record
 from calfkit.client.deserialize import _UNSET
-from calfkit.engine._lib import CK_ACT_REPLY, CK_OK, COL, STATUS_NAMES
+from calfkit.engine._lib import CK_ACT_REPLY, CK_OK, CK_SKIPPED, COL, STATUS_NAMES
 from calfkit.exceptions import DeserializationError, RecordRejected
 from calfkit.nodes.base import pack_records
 
@@ -47,6 +47,8 @@ class BatchReplyDecoder:
         adapter = TypeAdapter(output_type) if mode == 2 else None
         res: list[ReplyOutput] = []
         for i, r in enumerate(recs):
+            if cols[COL["STATUS"], i] == CK_SKIPPED:          # not delivered to a consumer (a control / aborted batch)
+                continue
             if cols[COL["STATUS"], i] != CK_OK:
                 st = int(cols[COL["STATUS"], i])
                 res.append(ReplyOutput(r.correlation_id, error=RecordRejected(st, STATUS_NAMES[st], i)))

@@ -15,8 +15,8 @@ _PKG_ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__fi
 LIB_PATH = os.environ.get("CK_LIB") or os.path.join(_PKG_ROOT, "libcalfkit_b200.so")   # CK_LIB: kernel A/B builds during development
 
 # ---- constants mirrored from csrc/ck_common.h (checked against the header in tests/test_abi.py) ----
-CK_OK, CK_NOT_CANONICAL, CK_JSON_INVALID, CK_SCHEMA_INVALID, CK_UNSUPPORTED, CK_EMPTY, CK_BAD_FRAME = range(7)
-STATUS_NAMES = ["ok", "not_canonical", "json_invalid", "schema_invalid", "unsupported", "empty", "bad_frame"]
+CK_OK, CK_NOT_CANONICAL, CK_JSON_INVALID, CK_SCHEMA_INVALID, CK_UNSUPPORTED, CK_EMPTY, CK_BAD_FRAME, CK_SKIPPED = range(8)
+STATUS_NAMES = ["ok", "not_canonical", "json_invalid", "schema_invalid", "unsupported", "empty", "bad_frame", "skipped"]
 (CK_ACT_NONE, CK_ACT_RETURN, CK_ACT_SILENT, CK_ACT_RAISES, CK_ACT_CALL, CK_ACT_TAILCALL, CK_ACT_FANOUT,
  CK_ACT_HOST_TOOL, CK_ACT_REPLY, CK_ACT_GATE_COMPLETE, CK_ACT_GATE_PASS) = range(11)
 ACTION_NAMES = ["none", "return", "silent", "raises", "call", "tailcall", "fanout", "host_tool", "reply", "gate_complete", "gate_pass"]
@@ -46,7 +46,7 @@ EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_registe
            "ck_fetch_cols_async", "ck_gate_create", "ck_gate_register", "ck_gate_arrive", "ck_gate_stats", "ck_gate_compact", "ck_gate_reset", "ck_submit_recordbatch",
            "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option",
            "ck_set_frame_topics", "ck_encode_frames", "ck_encode_frames_records", "ck_frames_size", "ck_fetch_frames_async",
-           "ck_fetch_rb_index_async", "ck_fetch_rb_decoded_async"]
+           "ck_fetch_rb_index_async", "ck_fetch_rb_decoded_async", "ck_set_fetch_hidden", "ck_fetch_txn_mask"]
 
 _lib = None
 
@@ -108,6 +108,8 @@ def load() -> C.CDLL:
         "ck_fetch_rb_index": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
         "ck_fetch_rb_index_async": (C.c_int, [vp, i64p, u32p, i64p, i32p, i64p, i32p, u32p]),
         "ck_fetch_rb_decoded_async": (C.c_int, [vp, u8p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+        "ck_set_fetch_hidden": (C.c_int, [vp, u8p, C.c_uint32]),
+        "ck_fetch_txn_mask": (C.c_int, [u8p, C.c_uint64, vp, C.c_uint32, u32p, i64p, i64p, C.c_uint32, u8p, C.c_uint32, C.POINTER(C.c_uint32)]),
         "ck_encode_recordbatch": (C.c_int, [vp, u32p, C.c_uint32, C.c_int64, C.c_int64, u8p, C.c_uint64, C.POINTER(C.c_uint64)]),
         "ck_set_frame_topics": (C.c_int, [vp, i32p, C.c_uint32]),
         "ck_encode_frames": (C.c_int, [vp, C.c_int64]),

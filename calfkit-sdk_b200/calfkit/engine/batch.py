@@ -24,6 +24,35 @@ from calfkit.exceptions import EngineError
 # frame codecs the device builds, by the name Kafka clients use (KafkaBroker(compression_type=...)) -> Kafka's codec id
 FRAME_CODECS = {None: 0, "lz4": 3}
 
+# what a Kafka consumer's `isolation_level` takes: read_committed hides the records of aborted transactions (csrc/ck_txn.h)
+ISOLATION_LEVELS = ("read_uncommitted", "read_committed")
+
+
+def txn_partitions(aborted_transactions=None, partitions=None) -> list[tuple[int, list[tuple[int, int]]]]:
+    """the partition model of a fetch response's record set: [(byte start of the partition's batches, its AbortedTransactions
+    [(producer id, first offset), ...]), ...] in byte order; `aborted_transactions` alone: one partition, the whole record set"""
+    if aborted_transactions is not None and partitions is not None:
+        raise EngineError("give aborted_transactions (one partition) or partitions, not both")
+    if partitions is None:
+        partitions = [(0, aborted_transactions or [])]
+    return [(int(start), [(int(pid), int(first)) for pid, first in ab]) for start, ab in partitions]
+
+
+def fetch_txn_mask(buf: np.ndarray, partitions) -> np.ndarray:
+    """per complete batch of the record set `buf`: 1 where a read_committed consumer skips it, a transactional batch of an
+    aborted producer (ck_fetch_txn_mask; control batches are skipped by the engine itself)"""
+    lib = _lib.load()
+    starts = np.asarray([s for s, _ab in partitions], dtype=np.uint64)
+    runs = np.asarray([r for r, (_s, ab) in enumerate(partitions) for _e in ab], dtype=np.uint32)
+    pids = np.asarray([pid for _s, ab in partitions for pid, _f in ab], dtype=np.int64)
+    firsts = np.asarray([first for _s, ab in partitions for _p, first in ab], dtype=np.int64)
+    cap = buf.nbytes // 61 + 1
+    mask, nb = np.zeros(cap, dtype=np.uint8), C.c_uint32(0)
+    if lib.ck_fetch_txn_mask(ptr(buf), buf.nbytes, ptr(starts), len(starts), ptr(runs), ptr(pids), ptr(firsts), len(runs),
+                             ptr(mask), cap, C.byref(nb)):
+        raise EngineError(lib.ck_last_error(None).decode())
+    return mask[:nb.value]
+
 
 @dataclass
 class ToolTemplate:
@@ -232,6 +261,7 @@ class BatchEngine:
         self.n = 0
         self._in_data = self._in_off = self._rb_raw = None
         self.frame_topics: list[str] = []
+        self.read_committed = False
 
     # ------------------------------------------------------------------------------------------
     def close(self) -> None:
@@ -356,11 +386,28 @@ class BatchEngine:
         self._in_data, self._in_off = data, offsets
         self._check(self.lib.ck_submit(self.h, ptr(data), ptr(offsets), self.n))
 
-    def submit_recordbatch(self, buf: np.ndarray) -> int:
+    def set_isolation_level(self, level: str) -> None:
+        """what the fetches submitted from now on deliver, as a Kafka consumer's `isolation_level` says: "read_uncommitted"
+        (the default) every record but the control batches' markers, "read_committed" also not the records of aborted
+        transactions (those a fetch names in its AbortedTransactions).  Records not delivered get status CK_SKIPPED"""
+        if level not in ISOLATION_LEVELS:
+            raise EngineError(f"isolation_level {level!r}: expected one of {ISOLATION_LEVELS}")
+        self.read_committed = level == "read_committed"
+
+    def set_fetch_hidden(self, mask: np.ndarray) -> None:
+        """the read_committed mask (fetch_txn_mask, or its slice) of the next fetch submitted"""
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        self._check(self.lib.ck_set_fetch_hidden(self.h, ptr(mask), len(mask)))
+
+    def submit_recordbatch(self, buf: np.ndarray, aborted_transactions=None, partitions=None) -> int:
         """H2D + CRC32C check + (gzip / LZ4 / zstd batches) decode + record split + field decode + walk of a fetch response's record set
         (concatenated Kafka RecordBatch v2 frames, uncompressed, gzip, LZ4 or zstd); returns the number of records.  Column spans are
-        relative to each VALUE."""
+        relative to each VALUE.  Control batches are skipped; under read_committed so are the aborted transactions' batches, from
+        `aborted_transactions` [(producer id, first offset), ...] of a one-partition record set or `partitions` (txn_partitions)"""
         assert buf.dtype == np.uint8
+        parts = txn_partitions(aborted_transactions, partitions)
+        if self.read_committed and any(ab for _s, ab in parts):
+            self.set_fetch_hidden(fetch_txn_mask(buf, parts))
         n = C.c_uint32(0)
         self._check(self.lib.ck_submit_recordbatch(self.h, ptr(buf), buf.nbytes, C.byref(n)))
         self.n = n.value

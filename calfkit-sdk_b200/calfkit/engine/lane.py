@@ -26,7 +26,7 @@ import numpy as np
 
 from calfkit.engine import _lib
 from calfkit.engine._lib import COL, FRAME_DTYPE, PUB_DTYPE, ptr
-from calfkit.engine.batch import BatchEngine, FetchBytes, Frames, ToolTemplate, _SpanOffsets
+from calfkit.engine.batch import BatchEngine, FetchBytes, Frames, ToolTemplate, _SpanOffsets, fetch_txn_mask, txn_partitions
 from calfkit.exceptions import EngineError
 
 NO_PAYLOAD = 0xFFFFFFFF
@@ -129,20 +129,33 @@ class Arena:
 class FetchArena:
     """the record set of one fetch response — concatenated RecordBatch v2 frames as they came off the socket — in one
     buffer.  The host only chains through the 12-byte frame prefixes (baseOffset, batchLength) to count frames and records;
-    a truncated trailing frame (legal in a fetch response) is carried along and ignored by the device"""
-    def __init__(self, data: np.ndarray, on_release: Callable[[], None] | None = None):
+    a truncated trailing frame (legal in a fetch response) is carried along and ignored by the device.
+    `partitions` (engine.batch.txn_partitions): where each partition's batches start and its AbortedTransactions, from
+    which hidden() gives the read_committed mask; a slice carries its part of the mask instead"""
+    def __init__(self, data: np.ndarray, on_release: Callable[[], None] | None = None, partitions=None,
+                 hidden: np.ndarray | None = None):
         assert data.dtype == np.uint8
         self.data, self._on_release, self._index = data, on_release, None
+        self.partitions, self._hidden = partitions, hidden
 
     @classmethod
-    def of(cls, buf, pool: PinnedPool | None = None) -> "FetchArena":
-        """land a fetch response (bytes / uint8 array) in a page-locked buffer"""
+    def of(cls, buf, pool: PinnedPool | None = None, aborted_transactions=None, partitions=None) -> "FetchArena":
+        """land a fetch response (bytes / uint8 array) in a page-locked buffer; aborted_transactions [(producer id, first
+        offset), ...] of its one partition, or partitions [(byte start, [(producer id, first offset), ...]), ...]"""
+        parts = txn_partitions(aborted_transactions, partitions)
         src = np.frombuffer(bytes(buf), dtype=np.uint8) if not isinstance(buf, np.ndarray) else buf
         if pool is None:
-            return cls(src)
+            return cls(src, partitions=parts)
         b = pool.take(src.nbytes + 64)
         b.array[:src.nbytes] = src
-        return cls(b.array[:src.nbytes], on_release=lambda: pool.give(b))
+        return cls(b.array[:src.nbytes], on_release=lambda: pool.give(b), partitions=parts)
+
+    def hidden(self) -> np.ndarray | None:
+        """per complete frame, 1 where a read_committed consumer skips it; computed once over the whole fetch, since the
+        aborted producers carry from batch to batch across any split.  None: the fetch names no aborted transaction"""
+        if self._hidden is None and self.partitions and any(ab for _s, ab in self.partitions):
+            self._hidden = fetch_txn_mask(self.data, self.partitions)
+        return self._hidden
 
     def frames(self) -> tuple[np.ndarray, np.ndarray]:
         """(starts[k + 1], records[k]) of the k complete frames; starts[k] is where the truncated tail (if any) begins"""
@@ -169,8 +182,9 @@ class FetchArena:
 
     def slice_frames(self, a: int, b: int | None) -> "FetchArena":
         """frames [a, b) as a zero-copy view; b None: to the end of the buffer (the truncated tail included)"""
-        starts = self.frames()[0]
-        return FetchArena(self.data[int(starts[a]):(int(starts[b]) if b is not None else self.data.nbytes)])
+        starts, hidden = self.frames()[0], self.hidden()
+        return FetchArena(self.data[int(starts[a]):(int(starts[b]) if b is not None else self.data.nbytes)],
+                          hidden=None if hidden is None else hidden[a:b])
 
     def release(self) -> None:
         if self._on_release is not None:
@@ -349,11 +363,14 @@ class Lane:
 
     def submit(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None) -> None:
         """device-template tool node: decode + plan + encode + route (+ frame pass, + forward to the owning ranks), all
-        asynchronous.  A FetchArena goes to the device as it is (ck_submit_recordbatch).  With frame topics set on the engine,
+        asynchronous.  A FetchArena goes to the device as it is (ck_submit_recordbatch), with its read_committed mask when
+        the engine's isolation level is read_committed.  With frame topics set on the engine,
         their publishes are framed with baseTimestamp timestamp_ms (default: now)"""
         self.arena, self.busy = arena, True
         eng = self.eng
         if isinstance(arena, FetchArena):
+            if eng.read_committed and arena.hidden() is not None:
+                eng.set_fetch_hidden(arena.hidden())
             n = C.c_uint32(0)
             eng._check(eng.lib.ck_submit_recordbatch(eng.h, ptr(arena.data), arena.data.nbytes, C.byref(n)))
             eng.n = n.value

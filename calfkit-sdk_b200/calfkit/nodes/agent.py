@@ -26,7 +26,7 @@ import pydantic_core
 
 from calfkit._types import AgentOutputT
 from calfkit.broker import Record
-from calfkit.engine._lib import CK_ACT_FANOUT, CK_ACT_GATE_COMPLETE, CK_ACT_SILENT, CK_OK, COL, STATUS_NAMES
+from calfkit.engine._lib import CK_ACT_FANOUT, CK_ACT_GATE_COMPLETE, CK_ACT_SILENT, CK_OK, CK_SKIPPED, COL, STATUS_NAMES
 from calfkit.models import State
 from calfkit.models.messages import (ModelMessage, ModelRequest, ModelResponse, RetryPromptPart, ToolCallPart,
                                      ToolDefinition, ToolReturnPart)
@@ -203,7 +203,8 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
         silent_returns: list[Record] = []
         for i in range(len(records)):
             if cols[COL["STATUS"], i] != CK_OK:
-                logger.error("record %d rejected: %s", i, STATUS_NAMES[int(cols[COL["STATUS"], i])])
+                if cols[COL["STATUS"], i] != CK_SKIPPED:      # skipped: not delivered to a consumer (a control / aborted batch)
+                    logger.error("record %d rejected: %s", i, STATUS_NAMES[int(cols[COL["STATUS"], i])])
                 continue
             if gated and cols[COL["ACTION"], i] == CK_ACT_SILENT:
                 if self.publish_topic:          # handler return of a Silent: the inbound envelope (nodes/base.py:137-145, worker.py:52-53)
@@ -275,7 +276,7 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
             finally:
                 if saved_topics is not None:
                     self._restore_registry(engine, saved_topics)
-            for r in np.flatnonzero(out.cols[COL["STATUS"]] != CK_OK):
+            for r in np.flatnonzero((out.cols[COL["STATUS"]] != CK_OK) & (out.cols[COL["STATUS"]] != CK_SKIPPED)):
                 # e.g. more tool calls than the engine indexes per record (DESIGN.md §8): the conversation stops here
                 logger.error("record %d declined after the agent step: %s; nothing is published for it",
                              items[r][0], STATUS_NAMES[int(out.cols[COL["STATUS"], r])])

@@ -23,7 +23,7 @@ import pydantic_core
 from typing_extensions import Self
 
 from calfkit.broker import Record
-from calfkit.engine._lib import CK_ACT_HOST_TOOL, CK_ACT_RAISES, CK_OK, CK_UNSUPPORTED, COL, STATUS_NAMES
+from calfkit.engine._lib import CK_ACT_HOST_TOOL, CK_ACT_RAISES, CK_OK, CK_SKIPPED, CK_UNSUPPORTED, COL, STATUS_NAMES
 from calfkit.engine.batch import ToolTemplate
 from calfkit.models import SessionRunContext, State, ToolContext
 from calfkit.models.actions import NodeResult
@@ -297,6 +297,8 @@ class ToolNodeDef(BaseToolNodeDef):
         out = engine.fetch()
         declined = []
         for i in np.nonzero(out.cols[COL["STATUS"]] != CK_OK)[0]:
+            if out.cols[COL["STATUS"], i] == CK_SKIPPED:        # not delivered to a consumer (a control / aborted batch)
+                continue
             if out.cols[COL["STATUS"], i] == CK_UNSUPPORTED and out.cols[COL["ACTION"], i] == CK_ACT_RAISES and not force_host \
                     and self._template is not None:
                 declined.append(int(i))                      # the template declined it: the host-tool path below takes over

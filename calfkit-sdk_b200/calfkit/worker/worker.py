@@ -11,7 +11,9 @@ node.handler.  Here run() is the batch loop itself.  Two paths per node:
     (engine for decode / plan / encode, Python only for the user callable) -> `broker.produce_batch`.
 
 A poll is bounded by records AND bytes, an engine-level failure splits the batch and retries (dequeued records are never
-lost), and records the device declines as CK_UNSUPPORTED are re-run through the host-tool path.
+lost), and records the device declines as CK_UNSUPPORTED are re-run through the host-tool path.  Records of a fetch
+response that a consumer does not deliver (control batches; under the subscriber's isolation_level="read_committed" the
+aborted transactions' batches) come out CK_SKIPPED: counted in stats["skipped"], neither logged nor re-run.
 """
 from __future__ import annotations
 
@@ -26,8 +28,8 @@ import numpy as np
 from calfkit.broker import Record
 from calfkit.client import Client
 from calfkit.engine import BatchEngine
-from calfkit.engine.batch import FRAME_CODECS
-from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_UNSUPPORTED, STATUS_NAMES
+from calfkit.engine.batch import FRAME_CODECS, ISOLATION_LEVELS
+from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_SKIPPED, CK_UNSUPPORTED, STATUS_NAMES
 from calfkit.exceptions import EngineError
 from calfkit.engine.lane import LanePipeline, PublishBatch
 from calfkit.nodes import BaseNodeDef
@@ -96,7 +98,8 @@ class Worker:
         self._pipes: dict[int, LanePipeline] = {}
         self._framer_eng: BatchEngine | None = None
         self._frame_pool = None
-        self.stats = {"records": 0, "publishes": 0, "rejected": 0, "raises": 0, "host_fallback": 0, "steps": 0}
+        self._levels: dict[int, str] = {}          # node -> its subscription's isolation_level
+        self.stats = {"records": 0, "publishes": 0, "rejected": 0, "skipped": 0, "raises": 0, "host_fallback": 0, "steps": 0}
 
     def add_nodes(self, *nodes: BaseNodeDef) -> None:
         self._nodes.extend(nodes)
@@ -109,6 +112,11 @@ class Worker:
             logger.info("registering node=%s subscribe=%s publish=%s", node.name, node.subscribe_topics, node.publish_topic)
             subscriber = self._client._connection.subscriber(*node.subscribe_topics, group_id=group_id,
                                                              max_workers=self._max_workers, **self._extra_subscribe_kwargs)
+            # a FastStream KafkaBroker.subscriber takes isolation_level among its kwargs; here it goes to the node's lanes
+            level = subscriber.kwargs.get("isolation_level", "read_uncommitted")
+            if level not in ISOLATION_LEVELS:
+                raise EngineError(f"node {node.name}: isolation_level {level!r}, expected one of {ISOLATION_LEVELS}")
+            self._levels[id(node)] = level
             handler = subscriber(node.handler)
             if node.publish_topic:
                 self._client._connection.publisher(node.publish_topic, **self._extra_publish_kwargs)(handler)
@@ -123,10 +131,12 @@ class Worker:
             frame_topics = list(self._client._connection.frame_sinks)
             topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics + frame_topics
             codec = self._frame_codec() if frame_topics else None
+            level = self._levels.get(id(node), "read_uncommitted")
 
             def configure(eng: BatchEngine) -> None:
                 eng.register_topics(topics, num_partitions=getattr(self._client._connection, "num_partitions", 0))
                 node.configure_engine(eng)
+                eng.set_isolation_level(level)
                 if frame_topics:
                     eng.set_frame_topics(frame_topics)
                     eng.set_frame_compression(codec)
@@ -142,7 +152,9 @@ class Worker:
             batch.release()
             return
         self.stats["records"] += n
-        bad = batch.status != CK_OK
+        skipped = batch.status == CK_SKIPPED
+        self.stats["skipped"] += int(np.count_nonzero(skipped))
+        bad = (batch.status != CK_OK) & ~skipped
         nbad = int(np.count_nonzero(bad))
         if nbad:
             self.stats["rejected"] += nbad
@@ -155,7 +167,7 @@ class Worker:
                 self.stats["host_fallback"] += len(redo)
                 recs = [Record(node.subscribe_topics[0], batch.source.record(int(i))) for i in redo]
                 self._run_host(node, recs, force_host=True)
-        self.stats["raises"] += int(np.count_nonzero((batch.action == CK_ACT_RAISES) & ~bad))
+        self.stats["raises"] += int(np.count_nonzero((batch.action == CK_ACT_RAISES) & (batch.status == CK_OK)))
         self.stats["publishes"] += batch.n_publishes
         broker.produce_publishes(batch)
 

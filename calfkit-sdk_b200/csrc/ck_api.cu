@@ -8,6 +8,7 @@
 
 #include "../../include/calfkit_b200.h"
 #include "ck_kernels.cuh"
+#include "ck_txn.h"
 
 static_assert(sizeof(ck_publish) == sizeof(ck_pub), "ck_publish must mirror ck_pub");
 static_assert(sizeof(ck_frame) == sizeof(ck_frame_ent), "ck_frame must mirror ck_frame_ent");
@@ -57,6 +58,9 @@ struct ck_handle {
     // records section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
     u8* d_rb_fetch = nullptr; uint64_t rb_fetch_cap = 0; long long *d_rb_dec_off = nullptr, *h_rb_doff = nullptr; u32* d_rb_dec_len = nullptr;
     uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: no gzip / LZ4 batch)
+    // per batch the host's flag (ck_txn.h: bad / skipped), uploaded for a fetch that flags any (allocated on the first one);
+    // rb_hide: the read_committed mask ck_set_fetch_hidden gave for the next fetch
+    u32 *d_rb_flag = nullptr, *h_rb_flag = nullptr; std::vector<uint8_t> rb_hide; bool rb_hide_set = false;
     // frame pass (allocated on first use): per slot, then per record in group order; the frames and their table
     ck_fitem* d_fr_items = nullptr; u32 *d_fr_gkey = nullptr, *d_fr_idx = nullptr, *d_fr_head = nullptr, *d_fr_fstart = nullptr, *d_fr_gfirst = nullptr;
     u32 *d_fr_ffirst = nullptr, *d_fr_size = nullptr, *d_fr_nlive = nullptr, *d_fr_partial = nullptr;
@@ -207,9 +211,10 @@ extern "C" void ck_destroy(ck_handle* h) {
                      h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
                      h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
                      h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
-                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len};
+                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag};
     for (void* p : gptrs) if (p) cudaFree(p);
     if (h->h_rb_doff) cudaFreeHost(h->h_rb_doff);
+    if (h->h_rb_flag) cudaFreeHost(h->h_rb_flag);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
     if (h->d_recv) cudaFree(h->d_recv);
     if (h->d_x_overflow) cudaFree(h->d_x_overflow);
@@ -723,6 +728,14 @@ static int rb_lz_alloc(ck_handle* h) {
     CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_doff, sizeof(long long) * mr));
     return 0;
 }
+// the per-batch flags of fetches holding a control batch or under a read_committed mask, on the first such fetch
+static int rb_flag_alloc(ck_handle* h) {
+    if (h->d_rb_flag) return 0;
+    size_t mr = (size_t)h->max_records + 1;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_flag, sizeof(u32) * mr));
+    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_flag, sizeof(u32) * mr));
+    return 0;
+}
 // the fetch buffer: raw bytes, then the decoded slots.  Grown as fr_grow grows the frame buffer (waits for the stream once)
 static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
     if (h->d_rb_fetch) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_rb_fetch); }
@@ -739,9 +752,18 @@ static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
 // ISIZE (ck_gz_member), and through the frame header and block headers of a zstd batch to bound what it decodes to
 // (ck_zs_header, ck_zs_walk).  A fetch holding a gzip, LZ4 or zstd batch goes to the fetch buffer instead of d_in, with a
 // slot per such batch behind the raw bytes that the decode kernel of its codec fills (one launch per codec present); a
-// fetch without one takes the path it always took
+// fetch without one takes the path it always took.  The host also reads every control batch (ck_txn_control: its CRC32C,
+// its one record's key) and flags it skipped, or bad when malformed; a read_committed mask (ck_set_fetch_hidden) flags the
+// aborted transactions' batches skipped.  A flagged batch gets no slot: it is never sized or decoded
+extern "C" int ck_set_fetch_hidden(ck_handle* h, const uint8_t* mask, uint32_t nbatches) {
+    h->rb_hide.assign(mask, mask + nbatches);
+    h->rb_hide_set = true;
+    return 0;
+}
 extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint64_t nbytes, uint32_t* n_records) {
     cudaSetDevice(h->device);
+    bool hide = h->rb_hide_set;                        // the mask given for this fetch, consumed by it whatever happens
+    h->rb_hide_set = false;
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
     if (rb_alloc(h)) return 1;
     // the frame index is staged in page-locked memory the handle owns: its copies are asynchronous.  The staging is reused
@@ -750,15 +772,23 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
     bool lz = false, has_lz4 = false, has_gz = false, has_zs = false;   // lz: the fetch holds a decoded batch
+    bool flagged = false;                              // some batch is flagged bad or skipped by the host
     uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 and zstd bounds, the gzip ISIZEs)
-    while (pos + 12 <= nbytes) {
-        uint32_t blen = host_be32(host_buf + pos + 8);
-        uint64_t end = pos + 12 + (uint64_t)blen;
-        if ((int32_t)blen < (int32_t)(CK_RB_HEADER - 12) || end > nbytes) break;         // truncated trailing frame: legal in a fetch response
+    uint64_t end;
+    while ((end = ck_txn_frame_end(host_buf, nbytes, pos)) != 0) {   // stops at a truncated trailing frame: legal in a fetch response
         uint32_t cnt = host_be32(host_buf + pos + 57);
         if (total + cnt > h->max_records || nb >= h->max_records) return fail(h, "ck_submit_recordbatch: more records than max_records");
         u32 codec = host_buf[pos + 22] & 7u;
-        if (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD) {
+        int type = 0;
+        u32 flag = (host_buf[pos + 22] & CK_TXN_CONTROL) ? (u32)ck_txn_control(host_buf + pos, end - pos, &type)
+                 : hide && nb < h->rb_hide.size() && h->rb_hide[nb] ? (u32)CK_TXN_HIDE : (u32)CK_TXN_SHOW;
+        if (flag && !flagged) {                        // the batches before the first flagged one are delivered
+            if (rb_flag_alloc(h)) return 1;
+            for (u32 b = 0; b < nb; b++) h->h_rb_flag[b] = 0;
+            flagged = true;
+        }
+        if (flagged) h->h_rb_flag[nb] = flag;
+        if (!flag && (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD)) {
             if (!lz) {                                 // the batches before the first decoded one have empty slots
                 if (rb_lz_alloc(h)) return 1;
                 for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
@@ -793,6 +823,7 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
         total += cnt; pos = end;
     }
     boff[nb] = (long long)pos; rbase[nb] = (u32)total;
+    if (hide && h->rb_hide.size() != nb) return fail(h, "ck_submit_recordbatch: the mask of ck_set_fetch_hidden does not cover the fetch's batches");
     u32 n = (u32)total;
     if (n_records) *n_records = n;
     u8* buf = h->d_in;
@@ -809,11 +840,12 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     if (lz) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_dec_off, h->h_rb_doff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    if (flagged) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_flag, h->h_rb_flag, sizeof(u32) * nb, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaEventRecord(h->rb_ev, h->stream));
     h->rb_n = n; h->rb_dec_base = lz ? base : 0; h->rb_dec_bytes = lz ? dbytes : 0;
     if (nb) {
         KTimer t(h, CK_K_WALK);
-        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, nb, h->d_rb_batch_bad);
+        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, flagged ? h->d_rb_flag : nullptr, nb, h->d_rb_batch_bad);
         if (has_lz4) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
         if (has_gz) CKL(h) ck_rb_gzip_kernel<<<(nb + CK_GZ_WARPS - 1) / CK_GZ_WARPS, 32 * CK_GZ_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
                                                                                                           h->d_rb_batch_bad, h->d_rb_dec_len);
@@ -829,6 +861,17 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     h->cur_in = buf; h->cur_in_off = h->d_in_off; h->cur_len = h->d_rb_val_len; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
     if (launch_decode(h)) return 1;
     if (n) { CKL(h) ck_rb_mark_bad_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_rb_rec_bad, n, h->d_cols, n); CUDA_TRY(h, cudaGetLastError()); }
+    return 0;
+}
+
+// the read_committed mask of a whole fetch (ck_txn_mask): no handle, no device
+extern "C" int ck_fetch_txn_mask(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
+                                 const uint32_t* abort_run, const int64_t* abort_pid, const int64_t* abort_first, uint32_t naborts,
+                                 uint8_t* mask, uint32_t cap, uint32_t* nbatches) {
+    int64_t nb = ck_txn_mask(buf, nbytes, run_start, nruns, abort_run, abort_pid, abort_first, naborts, mask, cap);
+    if (nb < 0) { g_create_error = "ck_fetch_txn_mask: partition starts out of order, or an aborted transaction of no partition"; return 1; }
+    if (nbatches) *nbatches = (uint32_t)nb;
+    if ((uint64_t)nb > cap) { g_create_error = "ck_fetch_txn_mask: mask shorter than the fetch's batches"; return 1; }
     return 0;
 }
 

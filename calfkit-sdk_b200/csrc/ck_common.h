@@ -16,7 +16,9 @@ enum {
     CK_SCHEMA_INVALID = 3,   // pydantic: missing / string_type / union_tag_invalid / ... (detail in CK_COL_ERR)
     CK_UNSUPPORTED = 4,      // valid-looking but uses a construct the device path does not handle yet
     CK_EMPTY = 5,            // zero-length record
-    CK_BAD_FRAME = 6         // the Kafka record batch that carried it failed the CRC32C / framing check (ck_submit_recordbatch)
+    CK_BAD_FRAME = 6,        // the Kafka record batch that carried it failed the CRC32C / framing check (ck_submit_recordbatch)
+    CK_SKIPPED = 7           // a consumer does not deliver it: a control batch's marker, or under read_committed a record of
+                             // an aborted transaction (ck_submit_recordbatch, csrc/ck_txn.h)
 };
 
 // What the node does with the record (column CK_COL_ACTION), reference nodes/base.py:70-147.

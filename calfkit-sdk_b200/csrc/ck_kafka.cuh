@@ -15,6 +15,9 @@
 //   ck_rb_zstd_kernel    (a fetch holding zstd batches only) warp per zstd batch: its records section, one zstd frame,
 //                        decoded into the batch's slot (ck_zstd.cuh)
 //   ck_rb_split_kernel   thread per batch: hop from record to record (each starts with its own varint length)
+//                        (a batch the host flagged skipped — a control batch, or under read_committed a transactional
+//                        batch of an aborted producer, ck_txn.h — passes the CRC check, is neither decoded nor split, and
+//                        its records come out CK_SKIPPED)
 //   ck_rb_fields_kernel  thread per record: zig-zag varints -> key span, value span, the `correlation_id` header span
 // The walker then reads every value where it lies inside the buffer (ck_view.len): the raw bytes, or a compressed batch's
 // decoded slot.  No per-record slicing on the host.
@@ -116,8 +119,11 @@ __device__ __forceinline__ void ck_put_be64(u8* p, unsigned long long v) { ck_pu
 
 // ---- decode -------------------------------------------------------------------------------------------------------------
 // batch_off[b] .. batch_off[b+1]: frame b inside buf (indexed by the host: the frames chain through their own length field)
+// batch_bad[b] afterwards: 0 delivered, 1 bad (CK_TXN_BAD), 2 skipped (CK_TXN_HIDE): the host's flag (ck_txn.h; NULL: none
+// flagged) for a batch that passes the check, 1 for one that does not
 __global__ void __launch_bounds__(256)
-ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 nb, u32* __restrict__ batch_bad) {
+ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const u32* __restrict__ flag, u32 nb,
+                 u32* __restrict__ batch_bad) {
     __shared__ u32 t[1024];
     ck_crc_tables(t);
     u32 w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -131,7 +137,7 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
         u32 c = ck_crc_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
         if (c != ck_be32(f + 17)) bad = 1;
     }
-    if (lane == 0) batch_bad[w] = bad;
+    if (lane == 0) batch_bad[w] = bad ? 1u : flag ? flag[w] : 0u;
 }
 
 __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u32 end, long long& out) {
@@ -257,8 +263,8 @@ ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ bat
                    u32* __restrict__ batch_bad, long long* __restrict__ rec_pos, u32* __restrict__ rec_batch) {
     u32 b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
-    u32 r0 = rec_base[b], cnt = rec_base[b + 1] - r0;
-    bool ok = !batch_bad[b];
+    u32 r0 = rec_base[b], cnt = rec_base[b + 1] - r0, st = batch_bad[b];
+    bool ok = !st;                                              // a bad or skipped batch: its records get no span
     long long lo = batch_off[b] + CK_RB_HEADER, hi = batch_off[b + 1];
     if (ok && dec_off && ck_rb_is_decoded(buf, batch_off, b)) { lo = dec_off[b]; hi = lo + dec_len[b]; }
     const u8* f = buf + lo;
@@ -273,7 +279,7 @@ ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ bat
         pos += (u32)len;
     }
     if (ok && pos != flen) ok = false;
-    if (!ok) batch_bad[b] = 1;
+    if (!ok && !st) batch_bad[b] = 1;
 }
 
 // thread per record
@@ -286,7 +292,8 @@ ck_rb_fields_kernel(const u8* __restrict__ buf, long long buf_len, const long lo
     if (i >= n) return;
     val_off[i] = 0; val_len[i] = 0; key_off[i] = 0; key_len[i] = -1; corr_off[i] = 0; corr_len[i] = -1;
     long long rp = rec_pos[i];
-    if (rp < 0 || batch_bad[rec_batch[i]]) { rec_bad[i] = 1; return; }
+    u32 st = batch_bad[rec_batch[i]];
+    if (rp < 0 || st) { rec_bad[i] = st == 2u ? 2u : 1u; return; }
     const u8* p = buf + rp;
     u32 end = (u32)min((long long)0x7fffffff, buf_len - rp), pos = 0;
     long long len, t;
@@ -319,10 +326,12 @@ ck_rb_fields_kernel(const u8* __restrict__ buf, long long buf_len, const long lo
     if (!ok) { val_len[i] = 0; }
 }
 
+// rec_bad[i]: 1 the record's batch failed a check, 2 the consumer does not deliver it (a control batch, or an aborted
+// transaction's batch under read_committed).  Both have no span, so the walker passed over them as empty records
 __global__ void __launch_bounds__(256)
 ck_rb_mark_bad_kernel(const u32* __restrict__ rec_bad, u32 n, u32* __restrict__ cols, u32 stride) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && rec_bad[i]) cols[(size_t)CK_COL_STATUS * stride + i] = CK_BAD_FRAME;
+    if (i < n && rec_bad[i]) cols[(size_t)CK_COL_STATUS * stride + i] = rec_bad[i] == 2u ? CK_SKIPPED : CK_BAD_FRAME;
 }
 
 // ---- encode -------------------------------------------------------------------------------------------------------------

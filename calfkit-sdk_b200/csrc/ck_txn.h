@@ -1,0 +1,147 @@
+// Kafka transactions on the consume side (message format v2, KIP-98): which batches of a fetch response's record set a
+// consumer does not deliver.  Host code only, no device dependency: ck_submit_recordbatch uses it for the control batches
+// of every fetch, and ck_fetch_txn_mask for the read_committed mask of a whole fetch before it is split over engines.
+//
+// Two attributes bits of the batch header matter (attributes i16 at byte 21, so its low byte is byte 22):
+//   0x20 control batch: one record whose key is (version i16, type i16), type 0 = ABORT, 1 = COMMIT; its value
+//        (version i16, coordinatorEpoch i32) is not read.  Every consumer skips it, at both isolation levels.
+//   0x10 transactional batch: its records belong to the transaction of producerId (i64 at byte 43).
+// The rule, per partition of the record set, over its batches in order (the Java consumer's fetch loop):
+//   aborted = {}; pending = the partition's aborted transactions (producer id, first offset) sorted by first offset
+//   for each batch:
+//     a batch that fails its framing (magic 2, a known codec, the CRC32C) is bad: its records are bad frames, no state change
+//     while pending and pending[0].first_offset <= batch.lastOffset (baseOffset + lastOffsetDelta): aborted += pop(pending)
+//     control batch: skipped; an ABORT marker removes batch.producerId from aborted, any other type changes nothing
+//     transactional batch of a producer in aborted (read_committed only): skipped
+//     else delivered
+// A control batch that is compressed, holds recordsCount != 1, whose one record does not span its records section, or
+// whose key is shorter than 4 bytes or has a negative version, is bad and changes no state.  The Java consumer raises on
+// such a batch instead; here it is one more bad frame.  A producer whose abort marker lies past the end of the fetch stays
+// aborted to its end.  The broker never returns data past the partition's last stable offset to a read_committed fetch,
+// so a transaction still open there is not this code's concern.
+#ifndef CK_TXN_H
+#define CK_TXN_H
+
+#include <stdint.h>
+
+#include <algorithm>
+#include <set>
+#include <vector>
+
+#define CK_TXN_TRANSACTIONAL 0x10u
+#define CK_TXN_CONTROL 0x20u
+#define CK_TXN_ABORT 0                    // control record type of an abort marker
+enum { CK_TXN_SHOW = 0, CK_TXN_BAD = 1, CK_TXN_HIDE = 2 };   // per-batch flag: delivered / bad frame / skipped
+
+static inline uint32_t ck_txn_be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
+static inline int64_t ck_txn_be64(const uint8_t* p) { return (int64_t)(((uint64_t)ck_txn_be32(p) << 32) | ck_txn_be32(p + 4)); }
+
+// end of the complete frame at pos (12 + batchLength bytes, at least a header), 0 when none starts there: the end of the
+// record set or a truncated trailing frame, which a fetch response may carry
+static inline uint64_t ck_txn_frame_end(const uint8_t* buf, uint64_t n, uint64_t pos) {
+    if (pos + 12 > n) return 0;
+    uint32_t blen = ck_txn_be32(buf + pos + 8);
+    uint64_t end = pos + 12 + (uint64_t)blen;
+    return (int32_t)blen < 49 || end > n ? 0 : end;
+}
+
+static inline uint32_t ck_txn_crc32c(const uint8_t* p, uint64_t n) {
+    static const std::vector<uint32_t> t = [] {
+        std::vector<uint32_t> v(256);
+        for (uint32_t i = 0; i < 256; i++) {
+            uint32_t c = i;
+            for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((c & 1u) ? 0x82F63B78u : 0u);
+            v[i] = c;
+        }
+        return v;
+    }();
+    uint32_t c = 0xffffffffu;
+    for (uint64_t i = 0; i < n; i++) c = t[(c ^ p[i]) & 0xffu] ^ (c >> 8);
+    return ~c;
+}
+
+// the checks the device makes of every batch: magic 2, codec none / gzip / LZ4 / zstd, and (check_crc) the CRC32C
+static inline bool ck_txn_framed(const uint8_t* f, uint64_t flen, bool check_crc) {
+    uint32_t codec = f[22] & 7u;
+    if (f[16] != 2 || codec == 2 || codec > 4) return false;
+    return !check_crc || ck_txn_crc32c(f + 21, flen - 21) == ck_txn_be32(f + 17);
+}
+
+static inline bool ck_txn_varint(const uint8_t* p, uint64_t& pos, uint64_t end, int64_t& out) {
+    uint64_t u = 0;
+    for (uint32_t shift = 0;; shift += 7) {
+        if (pos >= end || shift > 63) return false;
+        uint8_t b = p[pos++];
+        u |= (uint64_t)(b & 0x7f) << shift;
+        if (!(b & 0x80)) break;
+    }
+    out = (int64_t)(u >> 1) ^ -(int64_t)(u & 1);
+    return true;
+}
+
+// a control batch f[0..flen): CK_TXN_HIDE and its marker's type in *type when it is well formed (see above), else CK_TXN_BAD
+static inline int ck_txn_control(const uint8_t* f, uint64_t flen, int* type) {
+    if (!ck_txn_framed(f, flen, true) || (f[22] & 7u) || ck_txn_be32(f + 57) != 1) return CK_TXN_BAD;
+    uint64_t pos = 61;
+    int64_t len, v, klen;
+    if (!ck_txn_varint(f, pos, flen, len) || len < 0 || (uint64_t)len != flen - pos) return CK_TXN_BAD;
+    pos += 1;                                                   // record attributes
+    if (!ck_txn_varint(f, pos, flen, v) || !ck_txn_varint(f, pos, flen, v) || !ck_txn_varint(f, pos, flen, klen)) return CK_TXN_BAD;
+    if (klen < 4 || (uint64_t)klen > flen - pos) return CK_TXN_BAD;
+    int16_t version = (int16_t)((f[pos] << 8) | f[pos + 1]);
+    if (version < 0) return CK_TXN_BAD;
+    *type = (int16_t)((f[pos + 2] << 8) | f[pos + 3]);
+    return CK_TXN_HIDE;
+}
+
+// The read_committed mask of a whole record set buf[0..n): mask[b] = 1 for each complete batch b the rule above skips
+// because it is a transactional batch of an aborted producer, else 0 (control batches included: ck_submit_recordbatch
+// flags those itself).  Partition r is the run of batches that start in [run_start[r], run_start[r + 1]) (the last run:
+// to the end); its aborted transactions are the entries k with abort_run[k] = r.  The CRC32C of a data batch is checked
+// only where it matters, when the batch would move aborted transactions into the set.  Returns the number of complete
+// batches (mask is written up to cap of them), or -1 when the runs are not in order or an entry names no run
+static inline int64_t ck_txn_mask(const uint8_t* buf, uint64_t n, const uint64_t* run_start, uint32_t nruns,
+                                  const uint32_t* abort_run, const int64_t* abort_pid, const int64_t* abort_first, uint32_t naborts,
+                                  uint8_t* mask, uint64_t cap) {
+    for (uint32_t r = 1; r < nruns; r++)
+        if (run_start[r] < run_start[r - 1]) return -1;
+    std::vector<uint32_t> order(naborts);
+    for (uint32_t k = 0; k < naborts; k++) {
+        if (abort_run[k] >= nruns) return -1;
+        order[k] = k;
+    }
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+        return abort_run[a] != abort_run[b] ? abort_run[a] < abort_run[b] : abort_first[a] < abort_first[b];
+    });
+    std::set<int64_t> aborted;
+    uint32_t next = 0;                                          // first entry of order not yet moved into `aborted`
+    int64_t run = -1;
+    uint64_t pos = 0, end;
+    int64_t b = 0;
+    for (; (end = ck_txn_frame_end(buf, n, pos)) != 0; pos = end, b++) {
+        while (run + 1 < (int64_t)nruns && run_start[run + 1] <= pos) {
+            run++;
+            aborted.clear();
+            while (next < naborts && abort_run[order[next]] < run) next++;   // a run no batch started in
+        }
+        uint8_t m = 0;
+        const uint8_t* f = buf + pos;
+        uint64_t flen = end - pos;
+        int64_t last = ck_txn_be64(f) + (int32_t)ck_txn_be32(f + 23), pid = ck_txn_be64(f + 43);
+        bool control = f[22] & CK_TXN_CONTROL;
+        auto due = [&] { return next < naborts && abort_run[order[next]] == run && abort_first[order[next]] <= last; };
+        int type = -1;
+        if (ck_txn_framed(f, flen, control || due()) && (!control || ck_txn_control(f, flen, &type) == CK_TXN_HIDE)) {
+            while (due()) aborted.insert(abort_pid[order[next++]]);
+            if (control) {
+                if (type == CK_TXN_ABORT) aborted.erase(pid);
+            } else if ((f[22] & CK_TXN_TRANSACTIONAL) && aborted.count(pid)) {
+                m = 1;
+            }
+        }
+        if ((uint64_t)b < cap) mask[b] = m;
+    }
+    return b;
+}
+
+#endif  // CK_TXN_H

@@ -134,6 +134,24 @@ int  ck_fetch_rb_index_async(ck_handle* h, int64_t* val_off, uint32_t* val_len, 
  * without a gzip, LZ4 or zstd batch), known as soon as ck_submit_recordbatch returns; with dst given (page-locked, cap >= *nbytes) their
  * D2H copy is queued: value offset v >= *base lies at dst[v - *base] after ck_sync. */
 int  ck_fetch_rb_decoded_async(ck_handle* h, uint8_t* dst, uint64_t cap, uint64_t* base, uint64_t* nbytes);
+/* Transactions (message format v2, KIP-98; the rule is in csrc/ck_txn.h).  Records a consumer does not deliver get status 7
+ * (skipped), val_len 0 and bad = 2 in ck_fetch_rb_index; bad = 1 still means a bad frame.  ck_submit_recordbatch skips
+ * every control batch (attributes bit 5) at both isolation levels after checking its CRC32C and its one record's key on
+ * the host; a malformed control batch (a bad CRC, a codec, recordsCount != 1, a key shorter than 4 bytes or of negative
+ * version) gets status 6, where the Java consumer raises.  Under read_committed the caller computes the mask of the whole
+ * fetch once with ck_fetch_txn_mask (no handle, no device): mask[b] = 1 for each complete batch b that is a transactional
+ * batch (attributes bit 4) of an aborted producer.  Partition r of the record set is the run of batches starting in
+ * [run_start[r], run_start[r + 1]); its aborted transactions (the fetch response's AbortedTransactions list) are the k
+ * with abort_run[k] = r, (abort_pid[k], abort_first[k]).  *nbatches = complete batches; fails when cap is smaller, the
+ * run starts decrease or an entry names no run.  ck_set_fetch_hidden hands a mask (a slice of it, when the fetch is split
+ * at batch boundaries over several handles) to the next ck_submit_recordbatch of the handle, which fails unless nbatches
+ * is the number of complete batches it finds; its flagged batches pass the CRC check and are neither decoded nor split.
+ * The broker never returns data past a partition's last stable offset to a read_committed fetch: a transaction still
+ * open there is the broker's concern, not this one's. */
+int  ck_set_fetch_hidden(ck_handle* h, const uint8_t* mask, uint32_t nbatches);
+int  ck_fetch_txn_mask(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
+                       const uint32_t* abort_run, const int64_t* abort_pid, const int64_t* abort_first, uint32_t naborts,
+                       uint8_t* mask, uint32_t cap, uint32_t* nbatches);
 int  ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uint32_t n, int64_t base_offset, int64_t timestamp_ms,
                            uint8_t* host_frame, uint64_t cap, uint64_t* frame_len);
 /* produce side for a whole step (reference: the producer aiokafka runs under broker.publish, nodes/base.py:82-87, and under the

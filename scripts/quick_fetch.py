@@ -12,6 +12,10 @@ two runs each, consume one of those fetch responses per step:
          copied back with the results (ck_fetch_rb_decoded_async)
   gzip   the same over the gzip frames (inflated on the device)
   zstd   the same over the zstd frames (decoded on the device)
+  txn    the uncompressed frames as transactions of four interleaved producers, each followed by its commit or abort
+         marker (about 10 % of the frames aborted), consumed read_committed: the mask of the whole fetch is computed once
+         (ck_fetch_txn_mask) and handed to every step (ck_set_fetch_hidden); the aborted and control batches' records
+         are skipped (CK_SKIPPED), so the leg's "skipped_records" are not walked
 Per leg: step time (CUDA events around the whole step, copies included), the fetch and walk kernels (profile timer
 "walk": CRC, decode, split, fields and the walker), each decode alone (walk of the leg minus walk of plain), events/s,
 and H2D / D2H bytes per step.  Prints one JSON line with the card name and power limit read in the same run.
@@ -96,9 +100,16 @@ def zstd_frames(buf: bytes) -> bytes:
 
 if zstd_ref.lib() is not None:
     fetch["zstd"] = zstd_frames(fetch["plain"])
-LEGS = [k for k in ("plain", "lz4", "gzip", "zstd") if k in fetch]
+import kafka_txn  # noqa: E402
+from calfkit.engine.batch import fetch_txn_mask  # noqa: E402
+_starts = [0]
+while _starts[-1] + 12 <= len(fetch["plain"]):
+    _starts.append(_starts[-1] + 12 + int.from_bytes(fetch["plain"][_starts[-1] + 8:_starts[-1] + 12], "big"))
+fetch["txn"], txn_aborted, _ab = kafka_txn.transactional_fetch([fetch["plain"][a:b] for a, b in zip(_starts, _starts[1:])], 0.1, seed=7)
+txn_mask = fetch_txn_mask(np.frombuffer(fetch["txn"], dtype=np.uint8), [(0, txn_aborted)])
+LEGS = [k for k in ("plain", "lz4", "gzip", "zstd", "txn") if k in fetch]
 
-e = BatchEngine(0, max_records=n, max_in_bytes=len(fetch["plain"]) + 4096)
+e = BatchEngine(0, max_records=n + len(_starts) + 64, max_in_bytes=len(fetch["txn"]) + 4096)
 e.register_topics(TOPICS, num_partitions=8)
 e.set_tool_node("tool.get_weather.output", ToolTemplate.from_format("It's sunny in {location}"))
 pinned = {}
@@ -106,9 +117,9 @@ for k, v in fetch.items():
     pinned[k] = PinnedBuffer(len(v))
     pinned[k].array[:len(v)] = np.frombuffer(v, dtype=np.uint8)
 b_out = PinnedBuffer(e.max_out + 64)
-b_off, b_len = PinnedBuffer(8 * (n + 1)), PinnedBuffer(4 * n)
-b_pubs = PinnedBuffer(PUB_DTYPE.itemsize * 2 * n)
-b_rb = PinnedBuffer(16 * n + 64)
+b_off, b_len = PinnedBuffer(8 * (e.max_payloads + 1)), PinnedBuffer(4 * e.max_payloads)
+b_pubs = PinnedBuffer(PUB_DTYPE.itemsize * 2 * e.max_records)
+b_rb = PinnedBuffer(16 * e.max_records + 64)
 b_dec = {}
 st = torch.cuda.ExternalStream(e.stream_ptr())
 
@@ -116,6 +127,8 @@ st = torch.cuda.ExternalStream(e.stream_ptr())
 def step(name: str) -> tuple[int, int]:
     buf = pinned[name]
     nrec = C.c_uint32(0)
+    if name == "txn":
+        e.set_fetch_hidden(txn_mask)
     e._check(e.lib.ck_submit_recordbatch(e.h, ptr(buf.array), buf.nbytes, C.byref(nrec)))
     e.n = m = nrec.value
     e.tool_plan()
@@ -137,7 +150,8 @@ def step(name: str) -> tuple[int, int]:
 def leg(name: str, steps: int = 5) -> dict:
     step(name)
     m = e.n
-    bad = int(b_rb.array[12 * m:16 * m].view(np.uint32).sum())
+    flags = b_rb.array[12 * m:16 * m].view(np.uint32)
+    bad, skipped = int((flags == 1).sum()), int((flags == 2).sum())
     e.profile(True)
     e.profile_read()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -150,7 +164,8 @@ def leg(name: str, steps: int = 5) -> dict:
     e.profile(False)
     ms = ev0.elapsed_time(ev1) / steps
     return {"step_ms": round(ms, 3), "walk_kernel_ms": round(prof["walk"][0] / steps, 3), "events_per_s": round(n / ms * 1e3),
-            "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "bad_records": bad}
+            "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "bad_records": bad,
+            "skipped_records": skipped}
 
 
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
@@ -165,5 +180,7 @@ walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k 
 res["lz4_decode_ms"] = round(walk["lz4"] - walk["plain"], 3)
 res["gzip_decode_ms"] = round(walk["gzip"] - walk["plain"], 3)
 res["zstd_decode_ms"] = round(walk["zstd"] - walk["plain"], 3) if "zstd" in walk else "not measured"
+res["txn_walk_minus_plain_ms"] = round(walk["txn"] - walk["plain"], 3)
+res["txn_aborted_frames"] = f"{sum(_ab)} of {len(_ab)}"
 res["decoded_bytes"] = {k: int(b.nbytes) for k, b in b_dec.items()}
 print(json.dumps(res))
