@@ -108,7 +108,7 @@ class _SpanOffsets:
 
 class FetchBytes:
     """the bytes value offsets of a fetch response index: offsets below len(raw) lie in the raw response, offsets from
-    `base` on in the gzip, LZ4 and zstd batches' decoded records sections, `decoded` (ck_fetch_rb_decoded_async).  Sliced like an array"""
+    `base` on in the gzip, snappy, LZ4 and zstd batches' decoded records sections, `decoded` (ck_fetch_rb_decoded_async).  Sliced like an array"""
     def __init__(self, raw: np.ndarray, base: int, decoded: np.ndarray):
         self.raw, self.base, self.decoded = raw, int(base), decoded
 
@@ -400,8 +400,8 @@ class BatchEngine:
         self._check(self.lib.ck_set_fetch_hidden(self.h, ptr(mask), len(mask)))
 
     def submit_recordbatch(self, buf: np.ndarray, aborted_transactions=None, partitions=None) -> int:
-        """H2D + CRC32C check + (gzip / LZ4 / zstd batches) decode + record split + field decode + walk of a fetch response's record set
-        (concatenated Kafka RecordBatch v2 frames, uncompressed, gzip, LZ4 or zstd); returns the number of records.  Column spans are
+        """H2D + CRC32C check + (gzip / snappy / LZ4 / zstd batches) decode + record split + field decode + walk of a fetch response's record set
+        (concatenated Kafka RecordBatch v2 frames, uncompressed, gzip, snappy, LZ4 or zstd); returns the number of records.  Column spans are
         relative to each VALUE.  Control batches are skipped; under read_committed so are the aborted transactions' batches, from
         `aborted_transactions` [(producer id, first offset), ...] of a one-partition record set or `partitions` (txn_partitions)"""
         assert buf.dtype == np.uint8
@@ -420,7 +420,7 @@ class BatchEngine:
 
     def rb_index(self) -> dict[str, np.ndarray]:
         """where value / key / the correlation_id header of every record lie (len -1 = absent), and under "data" the bytes
-        those offsets index: the submitted buffer, or a FetchBytes when the fetch held gzip, LZ4 or zstd batches"""
+        those offsets index: the submitted buffer, or a FetchBytes when the fetch held gzip, snappy, LZ4 or zstd batches"""
         n = self.n
         out = {"val_off": np.zeros(n, np.int64), "val_len": np.zeros(n, np.uint32), "key_off": np.zeros(n, np.int64),
                "key_len": np.zeros(n, np.int32), "corr_off": np.zeros(n, np.int64), "corr_len": np.zeros(n, np.int32),

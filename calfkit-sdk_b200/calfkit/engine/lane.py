@@ -7,7 +7,7 @@ table).  No Python object is created per record anywhere on this path.
 
   Arena          inbound batch: pinned uint8 bytes + int64 offsets[n+1]
   FetchArena     inbound batch as a Kafka fetch response carries it: the record set (RecordBatch v2 frames) in one pinned
-                 buffer; CRC check, gzip / LZ4 / zstd decode, record split and field decode run on the device (ck_submit_recordbatch)
+                 buffer; CRC check, gzip / snappy / LZ4 / zstd decode, record split and field decode run on the device (ck_submit_recordbatch)
   PublishBatch   outbound batch: pinned payload arena + the ck_publish table; resolves topic names / keys lazily,
                  per topic, vectorised
   PinnedPool     recycles page-locked buffers (cudaHostAlloc costs milliseconds; the steady state allocates nothing)
@@ -194,7 +194,7 @@ class FetchArena:
 
 class FetchRecords:
     """the records of a submitted FetchArena as the device split them: record i = its value, where it lies in the frame —
-    in the arena, or for a gzip, LZ4 or zstd batch in its decoded records section (`decoded` = (value offset of decoded[0], decoded))"""
+    in the arena, or for a gzip, snappy, LZ4 or zstd batch in its decoded records section (`decoded` = (value offset of decoded[0], decoded))"""
     def __init__(self, arena: FetchArena, val_off: np.ndarray, val_len: np.ndarray, bad: np.ndarray,
                  decoded: tuple[int, np.ndarray] | None = None):
         data = arena.data if decoded is None else FetchBytes(arena.data, decoded[0], decoded[1])
@@ -407,7 +407,7 @@ class Lane:
         eng._check(eng.lib.ck_fetch_groups(eng.h, ptr(order), ptr(key_counts), 0))
         self._views = (b_out.array[:nb], off, ln, pubs, rows, order, key_counts)
         # a fetch response: where every record's value lies in it, and whether its frame failed the check
-        # (and, when it held gzip, LZ4 or zstd batches, their decoded records sections, which those offsets point into)
+        # (and, when it held gzip, snappy, LZ4 or zstd batches, their decoded records sections, which those offsets point into)
         self._b_rb = self._rb = self._b_dec = self._dec = None
         if isinstance(self.arena, FetchArena):
             self._b_rb = b_rb = pool.take(16 * n + 64)

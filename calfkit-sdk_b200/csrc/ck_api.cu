@@ -58,6 +58,9 @@ struct ck_handle {
     // records section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
     u8* d_rb_fetch = nullptr; uint64_t rb_fetch_cap = 0; long long *d_rb_dec_off = nullptr, *h_rb_doff = nullptr; u32* d_rb_dec_len = nullptr;
     uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: no gzip / LZ4 batch)
+    // the chunk table of fetches holding snappy batches (ck_snappy.cuh; allocated on the first one, grown as needed): every
+    // raw snappy block of the fetch and its place in its batch's slot, staged in page-locked memory
+    ck_sn_chunk *d_rb_sn = nullptr, *h_rb_sn = nullptr; u32 rb_sn_cap = 0, rb_sn_dcap = 0;
     // per batch the host's flag (ck_txn.h: bad / skipped), uploaded for a fetch that flags any (allocated on the first one);
     // rb_hide: the read_committed mask ck_set_fetch_hidden gave for the next fetch
     u32 *d_rb_flag = nullptr, *h_rb_flag = nullptr; std::vector<uint8_t> rb_hide; bool rb_hide_set = false;
@@ -211,10 +214,11 @@ extern "C" void ck_destroy(ck_handle* h) {
                      h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
                      h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
                      h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
-                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag};
+                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag, h->d_rb_sn};
     for (void* p : gptrs) if (p) cudaFree(p);
     if (h->h_rb_doff) cudaFreeHost(h->h_rb_doff);
     if (h->h_rb_flag) cudaFreeHost(h->h_rb_flag);
+    if (h->h_rb_sn) cudaFreeHost(h->h_rb_sn);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
     if (h->d_recv) cudaFree(h->d_recv);
     if (h->d_x_overflow) cudaFree(h->d_x_overflow);
@@ -736,6 +740,17 @@ static int rb_flag_alloc(ck_handle* h) {
     CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_flag, sizeof(u32) * mr));
     return 0;
 }
+// room for n entries in the chunk table's staging, its first `used` entries kept (the caller has waited for rb_ev: no copy
+// reads the staging)
+static int rb_sn_reserve(ck_handle* h, u32 n, u32 used) {
+    if (n <= h->rb_sn_cap) return 0;
+    u32 cap = std::max(n, std::max(1024u, h->rb_sn_cap * 2u));
+    ck_sn_chunk* p = nullptr;
+    CUDA_TRY(h, cudaMallocHost((void**)&p, sizeof(ck_sn_chunk) * cap));
+    if (h->h_rb_sn) { memcpy(p, h->h_rb_sn, sizeof(ck_sn_chunk) * used); cudaFreeHost(h->h_rb_sn); }
+    h->h_rb_sn = p; h->rb_sn_cap = cap;
+    return 0;
+}
 // the fetch buffer: raw bytes, then the decoded slots.  Grown as fr_grow grows the frame buffer (waits for the stream once)
 static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
     if (h->d_rb_fetch) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_rb_fetch); }
@@ -749,12 +764,14 @@ static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
 // CRC32C check, record split and varint field decode run on the device and the walker reads every value where it lies.
 // The host only chains through the frame headers (12 + batchLength bytes each) to index the frames, through the LZ4 block
 // chain of an LZ4 batch (ck_lz_walk) to bound what it decodes to, through the member header of a gzip batch to read its
-// ISIZE (ck_gz_member), and through the frame header and block headers of a zstd batch to bound what it decodes to
-// (ck_zs_header, ck_zs_walk).  A fetch holding a gzip, LZ4 or zstd batch goes to the fetch buffer instead of d_in, with a
-// slot per such batch behind the raw bytes that the decode kernel of its codec fills (one launch per codec present); a
-// fetch without one takes the path it always took.  The host also reads every control batch (ck_txn_control: its CRC32C,
-// its one record's key) and flags it skipped, or bad when malformed; a read_committed mask (ck_set_fetch_hidden) flags the
-// aborted transactions' batches skipped.  A flagged batch gets no slot: it is never sized or decoded
+// ISIZE (ck_gz_member), through the frame header and block headers of a zstd batch to bound what it decodes to
+// (ck_zs_header, ck_zs_walk), and through the chunk chain of a snappy batch to read every block's declared length
+// (ck_sn_next), listing each block in the chunk table.  A fetch holding a gzip, snappy, LZ4 or zstd batch goes to the
+// fetch buffer instead of d_in, with a slot per such batch behind the raw bytes that the decode kernel of its codec fills
+// (one launch per codec present); a fetch without one takes the path it always took.  The host also reads every control
+// batch (ck_txn_control: its CRC32C, its one record's key) and flags it skipped, or bad when malformed; a read_committed
+// mask (ck_set_fetch_hidden) flags the aborted transactions' batches skipped.  A flagged batch gets no slot: it is never
+// sized or decoded
 extern "C" int ck_set_fetch_hidden(ck_handle* h, const uint8_t* mask, uint32_t nbatches) {
     h->rb_hide.assign(mask, mask + nbatches);
     h->rb_hide_set = true;
@@ -771,9 +788,10 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
     long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
-    bool lz = false, has_lz4 = false, has_gz = false, has_zs = false;   // lz: the fetch holds a decoded batch
+    bool lz = false, has_lz4 = false, has_gz = false, has_zs = false, has_sn = false;   // lz: the fetch holds a decoded batch
+    u32 nsn = 0;                                       // entries of the snappy chunk table
     bool flagged = false;                              // some batch is flagged bad or skipped by the host
-    uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 and zstd bounds, the gzip ISIZEs)
+    uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 and zstd bounds, the gzip ISIZEs, the snappy lengths)
     uint64_t end;
     while ((end = ck_txn_frame_end(host_buf, nbytes, pos)) != 0) {   // stops at a truncated trailing frame: legal in a fetch response
         uint32_t cnt = host_be32(host_buf + pos + 57);
@@ -788,7 +806,7 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
             flagged = true;
         }
         if (flagged) h->h_rb_flag[nb] = flag;
-        if (!flag && (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD)) {
+        if (!flag && (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD || codec == CK_RB_SNAPPY)) {
             if (!lz) {                                 // the batches before the first decoded one have empty slots
                 if (rb_lz_alloc(h)) return 1;
                 for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
@@ -796,9 +814,9 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
             }
             // the slot: LZ4, what the block chain decodes to at most; gzip, the member's ISIZE; zstd, what the blocks
             // decode to at most (compressed ones Block_Maximum_Size, even when Frame_Content_Size says less: their literals
-            // are decoded into the end of that room).  0 (the device marks the batch bad) when the chain or the blocks
-            // cannot be walked or the member header parsed, or the decoded batch would not fit the 32-bit lengths of the
-            // record split
+            // are decoded into the end of that room); snappy, exactly the sum of its blocks' declared lengths.  0 (the
+            // device marks the batch bad) when the chain or the blocks cannot be walked or the member header parsed, or the
+            // decoded batch would not fit the 32-bit lengths of the record split
             unsigned long long bound = 0;
             const u8* z = host_buf + pos + CK_RB_HEADER;
             if (codec == CK_RB_LZ4) {
@@ -811,6 +829,27 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
                 if (!ck_zs_header(z, end - pos - CK_RB_HEADER, f) || !ck_zs_walk(z, end - pos - CK_RB_HEADER, f, &bound) ||
                     CK_RB_HEADER + bound > 0x7fffffffull) bound = 0;
                 has_zs = true;
+            } else if (codec == CK_RB_SNAPPY) {
+                // one chunk table entry per block; a section the walk refuses has its entries dropped and gets one entry of
+                // no input, which the device refuses (so it marks the batch bad)
+                u32 first = nsn;
+                ck_sn_walker w;
+                ck_sn_begin(z, end - pos - CK_RB_HEADER, w);
+                unsigned long long off, o = 0; u32 len, dl;
+                int r;
+                while ((r = ck_sn_next(z, end - pos - CK_RB_HEADER, w, &off, &len, &dl)) > 0) {
+                    if (CK_RB_HEADER + o + dl > 0x7fffffffull) { r = -1; break; }
+                    if (rb_sn_reserve(h, nsn + 1, nsn)) return 1;
+                    h->h_rb_sn[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER + off), nb, len, (u32)o, dl};
+                    o += dl;
+                }
+                if (r < 0) {
+                    nsn = first;
+                    if (rb_sn_reserve(h, nsn + 1, nsn)) return 1;
+                    h->h_rb_sn[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER), nb, 0u, 0u, 0u};
+                }
+                bound = r < 0 ? 0 : o;
+                has_sn = true;
             } else {
                 u32 hdr = 0, isize = 0;
                 if (ck_gz_member(z, end - pos - CK_RB_HEADER, &hdr, &isize) && CK_RB_HEADER + (unsigned long long)isize <= 0x7fffffffull) bound = isize;
@@ -840,6 +879,16 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     if (lz) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_dec_off, h->h_rb_doff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    if (nsn) {
+        if (nsn > h->rb_sn_dcap) {                     // the last fetch's decode may still read the table: wait for it once
+            CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+            if (h->d_rb_sn) cudaFree(h->d_rb_sn);
+            h->d_rb_sn = nullptr; h->rb_sn_dcap = 0;
+            CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_sn, sizeof(ck_sn_chunk) * h->rb_sn_cap));
+            h->rb_sn_dcap = h->rb_sn_cap;
+        }
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_sn, h->h_rb_sn, sizeof(ck_sn_chunk) * nsn, cudaMemcpyHostToDevice, h->stream));
+    }
     if (flagged) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_flag, h->h_rb_flag, sizeof(u32) * nb, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaEventRecord(h->rb_ev, h->stream));
     h->rb_n = n; h->rb_dec_base = lz ? base : 0; h->rb_dec_bytes = lz ? dbytes : 0;
@@ -851,6 +900,8 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
                                                                                                           h->d_rb_batch_bad, h->d_rb_dec_len);
         if (has_zs) CKL(h) ck_rb_zstd_kernel<<<(nb + CK_ZS_WARPS - 1) / CK_ZS_WARPS, 32 * CK_ZS_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
                                                                                                           h->d_rb_batch_bad, h->d_rb_dec_len);
+        if (has_sn) CKL(h) ck_rb_snappy_kernel<<<(nsn + CK_SN_WARPS - 1) / CK_SN_WARPS, 32 * CK_SN_WARPS, 0, h->stream>>>(buf, h->d_rb_sn, nsn, h->d_rb_dec_off,
+                                                                                                              h->d_rb_batch_bad, h->d_rb_dec_len);
         CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off, lz ? h->d_rb_dec_off : nullptr,
                                                                         lz ? h->d_rb_dec_len : nullptr, h->d_rb_rec_base, nb,
                                                                         h->d_rb_batch_bad, h->d_rb_rec_pos, h->d_rb_rec_batch);

@@ -14,6 +14,8 @@
 //                        inflated into the batch's slot (ck_inflate.cuh) and checked against the trailer's CRC32
 //   ck_rb_zstd_kernel    (a fetch holding zstd batches only) warp per zstd batch: its records section, one zstd frame,
 //                        decoded into the batch's slot (ck_zstd.cuh)
+//   ck_rb_snappy_kernel  (a fetch holding snappy batches only) warp per snappy chunk, over the chunks of all the fetch's
+//                        snappy batches: each raw snappy block decoded into its place in its batch's slot (ck_snappy.cuh)
 //   ck_rb_split_kernel   thread per batch: hop from record to record (each starts with its own varint length)
 //                        (a batch the host flagged skipped — a control batch, or under read_committed a transactional
 //                        batch of an aborted producer, ck_txn.h — passes the CRC check, is neither decoded nor split, and
@@ -30,12 +32,14 @@
 #include "ck_lz4.cuh"
 #include "ck_inflate.cuh"
 #include "ck_zstd.cuh"
+#include "ck_snappy.cuh"
 
 #define CK_CRC_POLY 0x82F63B78u      // CRC32C (Castagnoli), reflected
 #define CK_CRC32_POLY 0xEDB88320u    // CRC32 (IEEE), reflected: gzip's
 #define CK_RB_HEADER 61u
 #define CK_RB_CRC_FROM 21u
 #define CK_RB_GZIP 1u                // attributes & 7: Kafka's codec ids of gzip
+#define CK_RB_SNAPPY 2u              // snappy
 #define CK_RB_LZ4 3u                 // LZ4
 #define CK_RB_ZSTD 4u                // and zstd
 
@@ -132,7 +136,7 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
     u32 flen = (u32)(batch_off[w + 1] - batch_off[w]);
     u32 bad = 0;
     u32 codec = flen >= CK_RB_HEADER ? f[22] & 7u : 0u;
-    if (flen < CK_RB_HEADER || f[16] != 2 || (codec != 0 && codec != CK_RB_GZIP && codec != CK_RB_LZ4 && codec != CK_RB_ZSTD)) bad = 1;   // not magic 2 / snappy
+    if (flen < CK_RB_HEADER || f[16] != 2 || codec > CK_RB_ZSTD) bad = 1;   // not magic 2 / a codec id Kafka does not define
     else {
         u32 c = ck_crc_warp(t, f + CK_RB_CRC_FROM, flen - CK_RB_CRC_FROM, lane);
         if (c != ck_be32(f + 17)) bad = 1;
@@ -156,10 +160,10 @@ __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u3
 __device__ __forceinline__ bool ck_rb_is_lz4(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
     return (buf[batch_off[b] + 22] & 7u) == CK_RB_LZ4;
 }
-// a batch whose records section is decoded into a slot: gzip, LZ4 or zstd
+// a batch whose records section is decoded into a slot: gzip, snappy, LZ4 or zstd
 __device__ __forceinline__ bool ck_rb_is_decoded(const u8* __restrict__ buf, const long long* __restrict__ batch_off, u32 b) {
     u32 codec = buf[batch_off[b] + 22] & 7u;
-    return codec == CK_RB_GZIP || codec == CK_RB_LZ4 || codec == CK_RB_ZSTD;
+    return codec == CK_RB_GZIP || codec == CK_RB_SNAPPY || codec == CK_RB_LZ4 || codec == CK_RB_ZSTD;
 }
 
 // warp per batch of a fetch that holds LZ4 batches; the uncompressed ones and those the CRC check refused are skipped.
@@ -253,9 +257,29 @@ ck_rb_zstd_kernel(u8* buf, const long long* __restrict__ batch_off, const long l
     if (lane == 0) { dec_len[w] = r >= 0 ? (u32)r : 0u; if (r < 0) batch_bad[w] = 1; }
 }
 
+// warp per chunk of a fetch that holds snappy batches: ch[0, nc) lists every raw snappy block of every snappy batch the
+// host delivers (ck_sn_next: one for a raw-block section, one per chunk of a framed one), each with its place in its
+// batch's slot.  dec_off[b] .. dec_off[b+1]: the slot of batch b, exactly the sum of its blocks' declared lengths.  A batch
+// the host could not walk (or whose slot would pass the 32-bit lengths of the record split) has an empty slot and one
+// entry of no input, which every decode refuses.  A batch the CRC check refused is skipped; a block that snappy refuses
+// or that does not decode to exactly its declared length marks its batch bad; the batch's first block writes dec_len[b]
+#define CK_SN_WARPS 8u
+__global__ void __launch_bounds__(32 * CK_SN_WARPS)
+ck_rb_snappy_kernel(u8* buf, const ck_sn_chunk* __restrict__ ch, u32 nc, const long long* __restrict__ dec_off,
+                    u32* __restrict__ batch_bad, u32* __restrict__ dec_len) {
+    u32 w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (w >= nc) return;
+    const ck_sn_chunk c = ch[w];
+    if (*(volatile u32*)(batch_bad + c.batch)) return;         // only ever set to 1 by the other chunks: any read is safe
+    long long slot = dec_off[c.batch];
+    if (c.out_off == 0 && lane == 0) dec_len[c.batch] = (u32)(dec_off[c.batch + 1] - slot);
+    long long r = ck_sn_decode_block(buf + c.in_off, c.in_len, buf + slot + c.out_off, c.out_len, lane);
+    if (r < 0 && lane == 0) batch_bad[c.batch] = 1;
+}
+
 // thread per batch: where does each record start.  rec_base[b] = records in the batches before b (host prefix sum of
 // the recordsCount header fields); a batch whose records do not add up to its records section is marked bad.  The records
-// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for a gzip, LZ4 or zstd batch (dec_off given) its decoded
+// section is [batch_off[b] + 61, batch_off[b+1]) of the raw bytes, or for a gzip, snappy, LZ4 or zstd batch (dec_off given) its decoded
 // slot [dec_off[b], dec_off[b] + dec_len[b])
 __global__ void __launch_bounds__(128)
 ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch_off, const long long* __restrict__ dec_off,

@@ -60,10 +60,10 @@ static inline uint32_t ck_txn_crc32c(const uint8_t* p, uint64_t n) {
     return ~c;
 }
 
-// the checks the device makes of every batch: magic 2, codec none / gzip / LZ4 / zstd, and (check_crc) the CRC32C
+// the checks the device makes of every batch: magic 2, codec none / gzip / snappy / LZ4 / zstd, and (check_crc) the CRC32C
 static inline bool ck_txn_framed(const uint8_t* f, uint64_t flen, bool check_crc) {
     uint32_t codec = f[22] & 7u;
-    if (f[16] != 2 || codec == 2 || codec > 4) return false;
+    if (f[16] != 2 || codec > 4) return false;
     return !check_crc || ck_txn_crc32c(f + 21, flen - 21) == ck_txn_be32(f + 17);
 }
 

@@ -102,7 +102,7 @@ int  ck_fetch_groups(ck_handle* h, uint32_t* host_order, uint32_t* host_key_coun
 
 /* Kafka RecordBatch v2 framing on the device (reference: aiokafka under broker.subscriber / broker.publish,
  * calfkit/worker/worker.py:45-53, calfkit/nodes/base.py:82-87).  ck_submit_recordbatch takes a fetch response's record set
- * (concatenated v2 frames, uncompressed, gzip, LZ4 or zstd, below) as it came off the socket: one H2D copy (the frame index goes through page-locked
+ * (concatenated v2 frames, uncompressed, gzip, snappy, LZ4 or zstd, below) as it came off the socket: one H2D copy (the frame index goes through page-locked
  * staging the handle owns: nothing waits for the stream), then CRC32C verification, record split and
  * zig-zag varint field decode on the device; the walker reads each value where it lies.  Records of a frame that fails the
  * CRC / framing check get status 6 (bad frame); a truncated trailing frame is ignored.  *n_records = records decoded.
@@ -129,9 +129,13 @@ int  ck_fetch_rb_index_async(ck_handle* h, int64_t* val_off, uint32_t* val_len, 
  * present) decoded into a slot of the bound the host's walk of its block headers gives (raw and RLE blocks their size,
  * compressed blocks the block maximum, even when the frame states a smaller content size: the literals are decoded into
  * the end of that room); a malformed frame, a skippable or second frame, or anything after the frame gets status 6.
- * Snappy batches always do.
+ * Snappy batches (attributes & 7 = 2) are decoded the same way, a warp per chunk: the records section is snappy-java's
+ * framing (longer than 16 bytes, magic 82 'SNAPPY' 00, two version words, then big-endian u32 lengths each followed by
+ * one raw snappy block, tiling the section) or else one raw snappy block; each block (what Google snappy's RawUncompress
+ * accepts) decodes into its place in a slot of exactly the blocks' summed declared lengths.  A section whose chunks do not
+ * tile it, a block that snappy refuses or that declares more than 22 times its size, gets status 6.
  * ck_fetch_rb_decoded_async: where those slots start in value-offset space (*base) and their bytes (*nbytes; 0 for a fetch
- * without a gzip, LZ4 or zstd batch), known as soon as ck_submit_recordbatch returns; with dst given (page-locked, cap >= *nbytes) their
+ * without a gzip, snappy, LZ4 or zstd batch), known as soon as ck_submit_recordbatch returns; with dst given (page-locked, cap >= *nbytes) their
  * D2H copy is queued: value offset v >= *base lies at dst[v - *base] after ck_sync. */
 int  ck_fetch_rb_decoded_async(ck_handle* h, uint8_t* dst, uint64_t cap, uint64_t* base, uint64_t* nbytes);
 /* Transactions (message format v2, KIP-98; the rule is in csrc/ck_txn.h).  Records a consumer does not deliver get status 7

@@ -1,17 +1,22 @@
-"""Cost of consuming LZ4, gzip and zstd fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
+"""Cost of consuming LZ4, gzip, zstd and snappy fetch responses on a config-2 step (device-template tool node, 1M events), engine level.
 
 The step's tool events are framed once by the record form of the frame pass (ck_encode_frames_records), uncompressed and
 with LZ4 (ck_set_option 3 = 3), as a producer would write them to the tool's input topic; the gzip fetch is the same
 step's uncompressed frames with every records section recompressed on the host by zlib at level 6 (the level Java's
 GZIPOutputStream uses), one member per batch; the zstd fetch is the same with every records section recompressed by
 libzstd at level 3 (Kafka's default zstd level) and fed to it in 64 KB pieces, so that its frames carry no content size
-(the zstd leg is left out, and reported as not measured, when libzstd.so.1 cannot be loaded).  Four legs, alternating,
-two runs each, consume one of those fetch responses per step:
+(the zstd leg is left out, and reported as not measured, when libzstd.so.1 cannot be loaded).  The snappy fetches are the
+same with every records section recompressed by Google snappy (pyarrow's): framed by snappy-java in 32 KB chunks, as Java's
+producer, kafka-python and aiokafka write them, and as one raw block per batch, as librdkafka and sarama write them (both
+legs are left out, and reported as not measured, without pyarrow).  The legs, alternating, two runs each, consume one of
+those fetch responses per step:
   plain  ck_submit_recordbatch over the uncompressed frames + plan + the copies a Lane makes (results, record index)
   lz4    the same over the LZ4 frames: their records sections are decoded on the device, and the decoded region is
          copied back with the results (ck_fetch_rb_decoded_async)
   gzip   the same over the gzip frames (inflated on the device)
   zstd   the same over the zstd frames (decoded on the device)
+  snappy the same over the snappy-java framed frames (decoded on the device, a warp per 32 KB chunk)
+  snappy_raw  the same over the raw-block snappy frames (a warp per batch: each batch is one block)
   txn    the uncompressed frames as transactions of four interleaved producers, each followed by its commit or abort
          marker (about 10 % of the frames aborted), consumed read_committed: the mask of the whole fetch is computed once
          (ck_fetch_txn_mask) and handed to every step (ck_set_fetch_hidden); the aborted and control batches' records
@@ -100,6 +105,27 @@ def zstd_frames(buf: bytes) -> bytes:
 
 if zstd_ref.lib() is not None:
     fetch["zstd"] = zstd_frames(fetch["plain"])
+import snappy_ref  # noqa: E402
+
+
+def snappy_frames(buf: bytes, chunk) -> bytes:
+    """every frame's records section in snappy, attributes codec 2: framed in `chunk`-byte chunks, or one raw block (None)"""
+    import kafka_snappy
+    from oracle import kafka_batch as kb
+    out, pos = [], 0
+    while pos + 12 <= len(buf):
+        end = pos + 12 + int.from_bytes(buf[pos + 8:pos + 12], "big")
+        f = buf[pos:end]
+        sec = snappy_ref.compress(f[61:]) if chunk is None else kafka_snappy.xerial(f[61:], chunk)
+        covered = struct.pack(">h", (struct.unpack_from(">h", f, 21)[0] & ~7) | 2) + f[23:61] + sec
+        out.append(f[:8] + struct.pack(">i", len(covered) + 9) + f[12:17] + struct.pack(">I", kb.crc32c(covered)) + covered)
+        pos = end
+    return b"".join(out)
+
+
+if snappy_ref.available():
+    fetch["snappy"] = snappy_frames(fetch["plain"], 32 << 10)
+    fetch["snappy_raw"] = snappy_frames(fetch["plain"], None)
 import kafka_txn  # noqa: E402
 from calfkit.engine.batch import fetch_txn_mask  # noqa: E402
 _starts = [0]
@@ -107,7 +133,7 @@ while _starts[-1] + 12 <= len(fetch["plain"]):
     _starts.append(_starts[-1] + 12 + int.from_bytes(fetch["plain"][_starts[-1] + 8:_starts[-1] + 12], "big"))
 fetch["txn"], txn_aborted, _ab = kafka_txn.transactional_fetch([fetch["plain"][a:b] for a, b in zip(_starts, _starts[1:])], 0.1, seed=7)
 txn_mask = fetch_txn_mask(np.frombuffer(fetch["txn"], dtype=np.uint8), [(0, txn_aborted)])
-LEGS = [k for k in ("plain", "lz4", "gzip", "zstd", "txn") if k in fetch]
+LEGS = [k for k in ("plain", "lz4", "gzip", "zstd", "snappy", "snappy_raw", "txn") if k in fetch]
 
 e = BatchEngine(0, max_records=n + len(_starts) + 64, max_in_bytes=len(fetch["txn"]) + 4096)
 e.register_topics(TOPICS, num_partitions=8)
@@ -170,6 +196,7 @@ def leg(name: str, steps: int = 5) -> dict:
 
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
 res = {"events": n, "gpu": q.stdout.strip(), "libzstd": zstd_ref.version() if "zstd" in fetch else None,
+       "pyarrow_snappy": snappy_ref.version() if "snappy" in fetch else None,
        "fetch_bytes": {k: len(v) for k, v in fetch.items()}, "runs": []}
 t0 = time.time()
 for _ in range(2):
@@ -180,6 +207,8 @@ walk = {k: min(r["walk_kernel_ms"] for r in res["runs"] if r["leg"] == k) for k 
 res["lz4_decode_ms"] = round(walk["lz4"] - walk["plain"], 3)
 res["gzip_decode_ms"] = round(walk["gzip"] - walk["plain"], 3)
 res["zstd_decode_ms"] = round(walk["zstd"] - walk["plain"], 3) if "zstd" in walk else "not measured"
+for k in ("snappy", "snappy_raw"):
+    res[f"{k}_decode_ms"] = round(walk[k] - walk["plain"], 3) if k in walk else "not measured"
 res["txn_walk_minus_plain_ms"] = round(walk["txn"] - walk["plain"], 3)
 res["txn_aborted_frames"] = f"{sum(_ab)} of {len(_ab)}"
 res["decoded_bytes"] = {k: int(b.nbytes) for k, b in b_dec.items()}
