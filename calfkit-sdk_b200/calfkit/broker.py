@@ -16,8 +16,9 @@ Two granularities share the topics:
     next batch for its topics, bounded by records AND bytes (a batch never exceeds what an engine was sized for), zero-copy
     when the entry is contiguous.
 Kafka's own granularity — record batches — at both ends:
-  * `produce_fetch(topic, buf)` enqueues a fetch response's record set (engine.lane.FetchArena); `poll_arena` splits such
-    entries only at frame boundaries and the device checks, splits and decodes them.  Transactions (KIP-98): a record set
+  * `produce_fetch(topic, buf)` enqueues a fetch response's record set (engine.lane.FetchArena); `poll_arena` (device-template
+    nodes) and `poll_fetch` (Agent nodes, Python-tool nodes, the client's replies) split such entries only at frame boundaries,
+    and the device checks, splits and decodes them.  Transactions (KIP-98): a record set
     holds the batches of one or more partitions back to back, `partitions=[(byte start, aborted), ...]` in byte order,
     where `aborted` is that partition's AbortedTransactions from the fetch response, [(producer id, first offset), ...];
     `aborted_transactions=aborted` alone is the one-partition case.  Control batches are skipped at every isolation level;
@@ -244,7 +245,7 @@ class MemoryBroker:
                 out.append(q.popleft())
             if self.arenas.get(t) and type(self.arenas[t][0]).__name__ == "FetchArena":
                 from calfkit.exceptions import EngineError
-                raise EngineError(f"topic {t!r} holds fetch responses: they are decoded on the device by a device-template node")
+                raise EngineError(f"topic {t!r} holds fetch responses: they are decoded on the device, take them with poll_fetch")
             if len(out) < max_records and (self.arenas.get(t) or self.frags.get(t)):
                 arena = self.poll_arena((t,), max_records - len(out), None if max_bytes is None else max(max_bytes - nbytes, 1),
                                         records_too=False)
@@ -255,29 +256,24 @@ class MemoryBroker:
                     arena.release()
         return out
 
+    def poll_fetch(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None):
+        """the next fetch response (engine.lane.FetchArena) of the first of these topics whose next entry is one, split
+        at frame boundaries under the same bounds as poll_arena (None when none is): what a consumer that decodes fetches
+        on the device (a node's engine, the client's replies) takes before it asks poll_batch for Records"""
+        for t in topics:
+            head = _take_fetch(self.arenas.get(t), max_records, max_bytes)
+            if head is not None:
+                return head
+        return None
+
     def poll_arena(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None, records_too: bool = True):
         """the next batch for these topics as one contiguous Arena (None when idle).  Never returns more than max_records
         records or max_bytes bytes (one oversized record is still returned alone: the engine reports it per record)."""
         from calfkit.engine.lane import Arena
         for t in topics:
             q = self.arenas.get(t)
-            from calfkit.engine.lane import FetchArena
-            while q and isinstance(q[0], FetchArena) and len(q[0].frames()[1]) == 0:
-                q.popleft().release()                       # nothing but a truncated frame: no record in it
-            if q and isinstance(q[0], FetchArena):
-                # split only at frame boundaries, at least one frame (an oversized frame alone: the engine reports it)
-                a = q[0]
-                starts, counts = a.frames()
-                cum_rec, cum_bytes = np.cumsum(counts), starts[1:] - starts[0]
-                fits = cum_rec <= max_records
-                if max_bytes is not None:
-                    fits &= cum_bytes <= max_bytes
-                k = max(int(np.argmin(fits)) if not fits.all() else len(counts), 1)
-                if k >= len(counts):
-                    return q.popleft()                      # the truncated tail (if any) goes along and is ignored
-                head, rest = a.slice_frames(0, k), a.slice_frames(k, None)
-                rest._on_release, a._on_release = a._on_release, None
-                q[0] = rest
+            head = _take_fetch(q, max_records, max_bytes)
+            if head is not None:
                 return head
             if q:
                 a = q[0]
@@ -309,6 +305,31 @@ class MemoryBroker:
     def pending(self) -> int:
         return (sum(len(q) for q in self.queues.values()) + sum(len(r) for r in self._frame_pending.values()) + sum(a.n for q in self.arenas.values() for a in q)
                 + sum(len(i) for q in self.frags.values() for _b, i in q))
+
+
+def _take_fetch(q: deque | None, max_records: int, max_bytes: int | None):
+    """the head of q when it is a fetch response, split only at frame boundaries: its leading frames that fit max_records
+    records and max_bytes bytes, at least one (an oversized frame alone: the engine reports it); the rest stays at the
+    head, and the truncated tail (if any) travels with the last piece.  The read_committed mask is sliced along
+    (FetchArena.slice_frames).  None when q's head is not a fetch"""
+    from calfkit.engine.lane import FetchArena
+    while q and isinstance(q[0], FetchArena) and len(q[0].frames()[1]) == 0:
+        q.popleft().release()                       # nothing but a truncated frame: no record in it
+    if not (q and isinstance(q[0], FetchArena)):
+        return None
+    a = q[0]
+    starts, counts = a.frames()
+    cum_rec, cum_bytes = np.cumsum(counts), starts[1:] - starts[0]
+    fits = cum_rec <= max_records
+    if max_bytes is not None:
+        fits &= cum_bytes <= max_bytes
+    k = max(int(np.argmin(fits)) if not fits.all() else len(counts), 1)
+    if k >= len(counts):
+        return q.popleft()                          # the truncated tail (if any) goes along and is ignored
+    head, rest = a.slice_frames(0, k), a.slice_frames(k, None)
+    rest._on_release, a._on_release = a._on_release, None
+    q[0] = rest
+    return head
 
 
 def _fit(offsets, max_records: int, max_bytes: int | None) -> int:

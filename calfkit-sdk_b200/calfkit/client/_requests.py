@@ -25,6 +25,7 @@ from calfkit.client.middleware import ContextInjectionMiddleware
 from calfkit.exceptions import DeserializationError
 from calfkit.models import ContentPart, DataPart, State, TextPart
 from calfkit.models.messages import ModelMessage
+from calfkit.nodes.base import submit_inbound
 from calfkit.models.wire import CallFrame, CallFrameStack, Deps, Envelope, OverridesState, SessionRunContext, WorkflowState
 
 logger = logging.getLogger(__name__)
@@ -103,6 +104,10 @@ class _ReplyDispatcher:
     def __init__(self) -> None:
         self._pending: dict[str, asyncio.Future[Envelope]] = {}
         self._topic: str | None = None
+        self._engine = None             # decodes fetch responses on the reply topic; created on the first one
+
+    # a reply fetch is taken in pieces an engine of this size holds (replies carry the whole message history)
+    FETCH_RECORDS, FETCH_BYTES = 1 << 12, 32 << 20
 
     def register(self, broker, reply_topic: str, group_id: str) -> None:
         self._topic = reply_topic
@@ -119,13 +124,37 @@ class _ReplyDispatcher:
         future.set_result(envelope)
 
     async def drain(self, broker) -> int:
-        """deliver every queued reply record (the batch worker's stand-in for FastStream's consume task)"""
-        recs = broker.poll_batch((self._topic,), 1 << 16) if self._topic else []
+        """deliver every queued reply record (the batch worker's stand-in for FastStream's consume task); fetch responses
+        on the reply topic are checked, decompressed and split on the device (control and bad-frame records are not
+        delivered; the latter are logged)"""
+        if not self._topic:
+            return 0
+        n = 0
+        while (fetch := broker.poll_fetch((self._topic,), self.FETCH_RECORDS, self.FETCH_BYTES)) is not None:
+            try:
+                n += fetch.n
+                inb = submit_inbound(self._fetch_engine(), fetch)
+                for i in range(inb.n):
+                    if inb.values.bad[i] == 1:
+                        logger.error("reply record %d rejected: its record batch failed the check", i)
+                    elif inb.values.bad[i] == 0:
+                        await self._deliver(inb.value(i).tobytes(), inb.correlation_ids[i])
+            finally:
+                fetch.release()
+        recs = broker.poll_batch((self._topic,), 1 << 16)
         for r in recs:
-            envelope = Envelope.model_validate_json(r.value)     # reply -> Python objects at the user-API edge
-            corr = r.correlation_id or envelope.context.deps.correlation_id
-            await self._handle_reply(envelope, corr)
-        return len(recs)
+            await self._deliver(r.value, r.correlation_id)
+        return n + len(recs)
+
+    async def _deliver(self, value, correlation_id: str | None) -> None:
+        envelope = Envelope.model_validate_json(value)     # reply -> Python objects at the user-API edge
+        await self._handle_reply(envelope, correlation_id or envelope.context.deps.correlation_id)
+
+    def _fetch_engine(self):
+        if self._engine is None:
+            from calfkit.engine import BatchEngine
+            self._engine = BatchEngine(int(os.environ.get("LOCAL_RANK", 0)), max_records=self.FETCH_RECORDS, max_in_bytes=self.FETCH_BYTES)
+        return self._engine
 
     def expect(self, correlation_id: str) -> asyncio.Future[Envelope]:
         if correlation_id in self._pending:
@@ -140,6 +169,9 @@ class _ReplyDispatcher:
             if not future.done():
                 future.cancel()
         self._pending.clear()
+        if self._engine is not None:
+            self._engine.close()
+            self._engine = None
 
 
 # ----------------------------------------------------------------------------------------------------

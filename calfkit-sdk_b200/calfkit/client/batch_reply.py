@@ -19,7 +19,8 @@ from calfkit.broker import Record
 from calfkit.client.deserialize import _UNSET
 from calfkit.engine._lib import CK_ACT_REPLY, CK_OK, CK_SKIPPED, COL, STATUS_NAMES
 from calfkit.exceptions import DeserializationError, RecordRejected
-from calfkit.nodes.base import pack_records
+from calfkit.engine.lane import FetchArena
+from calfkit.nodes.base import submit_inbound
 
 
 @dataclass
@@ -33,25 +34,26 @@ class BatchReplyDecoder:
     def __init__(self, engine):
         self.engine = engine
 
-    def decode(self, records: list[Record] | list[bytes], output_type: type[Any] = _UNSET) -> list[ReplyOutput]:
-        recs = [r if isinstance(r, Record) else Record("", r, None, None) for r in records]
-        if not recs:
-            return []
-        data, offsets = pack_records(recs)
+    def decode(self, records: list[Record] | list[bytes] | FetchArena, output_type: type[Any] = _UNSET) -> list[ReplyOutput]:
+        """one ReplyOutput per delivered record, Records or the records of a fetch response alike"""
+        if not isinstance(records, FetchArena):
+            records = [r if isinstance(r, Record) else Record("", r, None, None) for r in records]
+            if not records:
+                return []
         eng = self.engine
-        eng.submit(data, offsets)
+        inb = submit_inbound(eng, records)
         mode = 0 if output_type is _UNSET else (1 if output_type is str else 2)
         eng.reply_plan(mode)
         out = eng.fetch()
         cols = out.cols
         adapter = TypeAdapter(output_type) if mode == 2 else None
         res: list[ReplyOutput] = []
-        for i, r in enumerate(recs):
+        for i in range(inb.n):
             if cols[COL["STATUS"], i] == CK_SKIPPED:          # not delivered to a consumer (a control / aborted batch)
                 continue
             if cols[COL["STATUS"], i] != CK_OK:
                 st = int(cols[COL["STATUS"], i])
-                res.append(ReplyOutput(r.correlation_id, error=RecordRejected(st, STATUS_NAMES[st], i)))
+                res.append(ReplyOutput(inb.correlation_ids[i], error=RecordRejected(st, STATUS_NAMES[st], i)))
                 continue
             rec = out.record_bytes(i)
             c0 = int(cols[COL["CORR_OFF"], i])

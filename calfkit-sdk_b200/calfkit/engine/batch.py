@@ -262,6 +262,7 @@ class BatchEngine:
         self._in_data = self._in_off = self._rb_raw = None
         self.frame_topics: list[str] = []
         self.read_committed = False
+        self.skipped = 0                # records of the fetches submitted so far that were not delivered (CK_SKIPPED)
 
     # ------------------------------------------------------------------------------------------
     def close(self) -> None:
@@ -416,7 +417,13 @@ class BatchEngine:
         # the host-side view of the batch for result decoding: record i = data[val_off[i] : val_off[i] + val_len[i]]
         self._in_data, self._in_off = idx["data"], _SpanOffsets(idx["val_off"], idx["val_len"])
         self._rb = idx
+        self.skipped += int(np.count_nonzero(idx["bad"] == 2))
         return self.n
+
+    @property
+    def fetch_index(self) -> dict[str, np.ndarray]:
+        """rb_index() of the fetch submit_recordbatch submitted last, as that call read it"""
+        return self._rb
 
     def rb_index(self) -> dict[str, np.ndarray]:
         """where value / key / the correlation_id header of every record lie (len -1 = absent), and under "data" the bytes

@@ -33,7 +33,8 @@ from calfkit.models.messages import (ModelMessage, ModelRequest, ModelResponse, 
 from calfkit.models.node_schema import BaseToolNodeSchema
 from calfkit.models.payload import DataPart, TextPart
 from calfkit.models.state import OverridesState, PendingToolBatch
-from calfkit.nodes.base import BaseNodeDef, pack_records
+from calfkit.engine.lane import FetchArena
+from calfkit.nodes.base import BaseNodeDef, pack_records, submit_inbound
 from calfkit.nodes.tool import ToolNodeDef
 
 logger = logging.getLogger(__name__)
@@ -180,9 +181,8 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
         engine.register_topics(topics, num_partitions=engine.num_partitions)
         self.configure_engine(engine)
 
-    def process_batch(self, engine, records: list[Record]) -> list[Record]:
-        data, offsets = pack_records(records)
-        engine.submit(data, offsets)
+    def process_batch(self, engine, records: list[Record] | FetchArena) -> list[Record]:
+        inb = submit_inbound(engine, records)
         gated = not self.sequential_only_mode and getattr(engine, "_gate_ready", False)
         merged_env = None
         if gated:
@@ -190,18 +190,17 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
             # becoming Python objects; the completing one comes back as the envelope carrying base_state + collected results
             engine.gate_compact()           # gives back what finished fan-outs used once the gate is half full
             engine.gate_arrive(self._gate_stamp)
-            self._gate_stamp += len(records)
+            self._gate_stamp += inb.n
             merged_env = engine.fetch()
             failed = engine.gate_stats()["failures"]
             if failed:
                 logger.error("aggregation gate: %d tool results found no room in the arena; their fan-outs are declined", failed)
         cols = merged_env.cols if merged_env is not None else engine.columns()
-        mv = memoryview(data)
         ovl = engine.overlay()          # records that arrived in another spelling: their canonical re-emission (the columns refer to it)
         post: dict[Any, list[tuple[int, bytes]]] = {"fanout": [], "return": []}
         canonical_in: dict[int, Any] = {}
         silent_returns: list[Record] = []
-        for i in range(len(records)):
+        for i in range(inb.n):
             if cols[COL["STATUS"], i] != CK_OK:
                 if cols[COL["STATUS"], i] != CK_SKIPPED:      # skipped: not delivered to a consumer (a control / aborted batch)
                     logger.error("record %d rejected: %s", i, STATUS_NAMES[int(cols[COL["STATUS"], i])])
@@ -210,12 +209,12 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
                 if self.publish_topic:          # handler return of a Silent: the inbound envelope (nodes/base.py:137-145, worker.py:52-53)
                     corr_raw = merged_env.record_bytes(i)[int(cols[COL["CORR_OFF"], i]):][:int(cols[COL["CORR_LEN"], i])].tobytes()
                     silent_returns.append(Record(self.publish_topic, merged_env.payload(i), None,
-                                                 records[i].correlation_id or pydantic_core.from_json(b'"' + corr_raw + b'"')))
+                                                 inb.correlation_ids[i] or pydantic_core.from_json(b'"' + corr_raw + b'"')))
                 continue
             if ovl is not None and ovl[1][i] >= 0:
                 rec = memoryview(ovl[0])[int(ovl[1][i]):int(ovl[1][i]) + int(ovl[2][i])]
             else:
-                rec = mv[offsets[i]:offsets[i + 1]]
+                rec = inb.value(i)
             canonical_in[i] = rec
             s0, s1 = 20, int(cols[COL["SOV_OFF"], i] + cols[COL["SOV_LEN"], i]) + 1       # the `state` object span
             state_json = bytes(rec[s0:s1])
@@ -237,7 +236,7 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
                 # Silent (aggregation still incomplete): nothing is routed, but the handler returns the inbound envelope and
                 # the worker publishes that return value to publish_topic (reference nodes/base.py:137-145, worker/worker.py:52-53)
                 if self.publish_topic:
-                    silent_returns.append(Record(self.publish_topic, bytes(rec), None, records[i].correlation_id or corr))
+                    silent_returns.append(Record(self.publish_topic, bytes(rec), None, inb.correlation_ids[i] or corr))
                 continue
             new_bytes = bytes(rec[:s0]) + new_state.model_dump_json().encode() + bytes(rec[s1:])
             group: Any = action                                   # "tailcall": all requested tools invalid (agent.py:171-175)
@@ -253,7 +252,7 @@ class BaseAgentNodeDef(Generic[AgentOutputT], BaseNodeDef):
             if not items:
                 continue
             kind, override_registry = (group[0], dict(group[1])) if isinstance(group, tuple) else (group, None)
-            recs2 = [Record(records[i].topic, b, records[i].key, records[i].correlation_id) for i, b in items]
+            recs2 = [Record(self.subscribe_topics[0], b, inb.keys[i], inb.correlation_ids[i]) for i, b in items]
             d2, o2 = pack_records(recs2)
             saved_topics = self._use_registry(engine, override_registry) if override_registry is not None else None
             try:

@@ -17,6 +17,8 @@ from typing import Any
 import numpy as np
 
 from calfkit.broker import Record
+from calfkit.engine.batch import FetchBytes, _SpanOffsets
+from calfkit.engine.lane import Arena, FetchArena, FetchRecords
 from calfkit.models import NodeResult, State
 from calfkit.models.envelope import Envelope
 from calfkit.models.node_schema import BaseNodeSchema
@@ -43,7 +45,7 @@ class BaseNodeDef(BaseNodeSchema):
         raise NotImplementedError(f"{type(self).__name__} has no batch plan: the GPU worker accelerates the node kinds "
                                   "the reference ships (@agent_tool nodes, Agent); custom run() bodies are out of scope")
 
-    def process_batch(self, engine, records: list[Record]) -> list[Record]:
+    def process_batch(self, engine, records: list[Record] | FetchArena) -> list[Record]:
         raise NotImplementedError
 
     # ---- object-level compatibility ----------------------------------------------------------------
@@ -79,3 +81,41 @@ def pack_records(records: list[Record]):
     np.cumsum(lens, out=offsets[1:])
     data = np.frombuffer(b"".join(r.value for r in records) or b"\0", dtype=np.uint8)
     return data, offsets
+
+
+class Inbound:
+    """what a node reads of each record of the batch it submitted (submit_inbound): value(i), the record's value bytes —
+    for a fetch, where the device found them: in the response or in a compressed batch's decoded records section —, and
+    keys[i] and correlation_ids[i] (Record fields, or a fetch record's key and `correlation_id` header; None: absent)"""
+    def __init__(self, values: Arena | FetchRecords, keys: list[bytes | None], correlation_ids: list[str | None]):
+        self.values, self.keys, self.correlation_ids = values, keys, correlation_ids
+
+    @property
+    def n(self) -> int:
+        return len(self.keys)
+
+    def value(self, i: int) -> memoryview:
+        o = self.values.offsets
+        return memoryview(self.values.data[int(o[i]):(o.end(i) if isinstance(o, _SpanOffsets) else int(o[i + 1]))])
+
+
+def submit_inbound(engine, batch: list[Record] | FetchArena) -> Inbound:
+    """submit an inbound batch to the engine, either form: Records through engine.submit, a fetch response through
+    engine.submit_recordbatch with the subscription's read_committed mask (set when the engine is at read_committed).
+    The column spans of record i then lie in inbound.value(i)"""
+    if not isinstance(batch, FetchArena):
+        data, offsets = pack_records(batch)
+        engine.submit(data, offsets)
+        return Inbound(Arena(data, offsets), [r.key for r in batch], [r.correlation_id for r in batch])
+    if engine.read_committed and batch.hidden() is not None:
+        engine.set_fetch_hidden(batch.hidden())
+    engine.submit_recordbatch(batch.data)
+    ix = engine.fetch_index
+    data = ix["data"]
+    values = FetchRecords(batch, ix["val_off"], ix["val_len"], ix["bad"],
+                          decoded=(data.base, data.decoded) if isinstance(data, FetchBytes) else None)
+
+    def spans(off, ln):
+        return [None if n < 0 else data[int(o):int(o) + int(n)].tobytes() for o, n in zip(off, ln)]
+    return Inbound(values, spans(ix["key_off"], ix["key_len"]),
+                   [None if c is None else c.decode() for c in spans(ix["corr_off"], ix["corr_len"])])

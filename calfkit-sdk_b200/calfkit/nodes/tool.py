@@ -29,7 +29,8 @@ from calfkit.models import SessionRunContext, State, ToolContext
 from calfkit.models.actions import NodeResult
 from calfkit.models.messages import ModelMessagesTypeAdapter, ToolDefinition
 from calfkit.models.node_schema import BaseToolNodeSchema
-from calfkit.nodes.base import BaseNodeDef, pack_records
+from calfkit.engine.lane import FetchArena
+from calfkit.nodes.base import BaseNodeDef, submit_inbound
 
 logger = logging.getLogger(__name__)
 
@@ -274,24 +275,22 @@ class ToolNodeDef(BaseToolNodeDef):
                 results.append(b"null")
         return results, failed
 
-    def process_batch(self, engine, records: list[Record], force_host: bool = False) -> list[Record]:
+    def process_batch(self, engine, records: list[Record] | FetchArena, force_host: bool = False) -> list[Record]:
         """force_host: evaluate the Python callable even though the node has a device template — used for the records the
         template declined (`args` given as a JSON string, a non-string argument ...: the reference's args_as_dict / the
         callable itself handle those, nodes/tool.py:53-64), so nothing is dropped on the template path"""
         failed: set[int] = set()
-        data, offsets = pack_records(records)
-        engine.submit(data, offsets)
+        inb = submit_inbound(engine, records)
         if self._template is not None and not force_host:
             engine.tool_plan()
         else:
             blob, off, ln = engine.tool_args()
             cols = engine.columns()
-            mv = memoryview(data)
             ovl = engine.overlay() if self._tool.takes_ctx else None     # the column spans refer to the canonical spelling of a record
-            results, failed = self._host_results(len(records), lambda i: blob[off[i]:off[i] + ln[i]].tobytes(),
+            results, failed = self._host_results(inb.n, lambda i: blob[off[i]:off[i] + ln[i]].tobytes(),
                                                  lambda i: (memoryview(ovl[0])[int(ovl[1][i]):int(ovl[1][i]) + int(ovl[2][i])]
-                                                            if ovl is not None and ovl[1][i] >= 0 else mv[offsets[i]:offsets[i + 1]]), cols)
-            aux_off = np.zeros(len(records) + 1, dtype=np.int64)
+                                                            if ovl is not None and ovl[1][i] >= 0 else inb.value(i)), cols)
+            aux_off = np.zeros(inb.n + 1, dtype=np.int64)
             np.cumsum([len(r) for r in results], out=aux_off[1:])
             engine.tool_plan(np.frombuffer(b"".join(results) or b"\0", dtype=np.uint8), aux_off)
         out = engine.fetch()
@@ -311,12 +310,13 @@ class ToolNodeDef(BaseToolNodeDef):
         for p in out.publishes():
             if p.record in failed:
                 continue
-            corr = records[p.record].correlation_id
+            corr = inb.correlation_ids[p.record]
             if corr is None and p.key is not None:
                 corr = p.key.decode()
             produced.append(Record(p.topic, p.payload, p.key, corr))
         if declined:
-            produced += self.process_batch(engine, [records[i] for i in declined], force_host=True)
+            produced += self.process_batch(engine, [Record(self.subscribe_topics[0], inb.value(i).tobytes(), inb.keys[i], inb.correlation_ids[i])
+                                                    for i in declined], force_host=True)
         return produced
 
 

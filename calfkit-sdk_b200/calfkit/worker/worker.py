@@ -7,8 +7,9 @@ node.handler.  Here run() is the batch loop itself.  Two paths per node:
   * device-template tool nodes (the data-parallel hot path): `broker.poll_arena` -> one pinned batch arena ->
     `LanePipeline.push` (H2D + decode + plan + encode + route on one of K lanes while an older step's results come
     back) -> `broker.produce_publishes(PublishBatch)`.  No Python object per record.
-  * nodes with a host half (Python tools, the Agent's LLM boundary): `broker.poll_batch` -> `node.process_batch`
-    (engine for decode / plan / encode, Python only for the user callable) -> `broker.produce_batch`.
+  * nodes with a host half (Python tools, the Agent's LLM boundary): `broker.poll_fetch`, else `broker.poll_batch` ->
+    `node.process_batch` (engine for decode / plan / encode, Python only for the user callable; a fetch response is
+    decoded there on the device, as on the lanes) -> `broker.produce_batch`.
 
 A poll is bounded by records AND bytes, an engine-level failure splits the batch and retries (dequeued records are never
 lost), and records the device declines as CK_UNSUPPORTED are re-run through the host-tool path.  Records of a fetch
@@ -31,7 +32,7 @@ from calfkit.engine import BatchEngine
 from calfkit.engine.batch import FRAME_CODECS, ISOLATION_LEVELS
 from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_SKIPPED, CK_UNSUPPORTED, STATUS_NAMES
 from calfkit.exceptions import EngineError
-from calfkit.engine.lane import LanePipeline, PublishBatch
+from calfkit.engine.lane import FetchArena, LanePipeline, PublishBatch
 from calfkit.nodes import BaseNodeDef
 
 logger = logging.getLogger(__name__)
@@ -43,8 +44,9 @@ def _EMPTY_ARENA():
 
 
 def engine_for(node: BaseNodeDef, *, device: int = 0, max_records: int = 1 << 14, max_in_bytes: int = 64 << 20,
-               extra_topics: list[str] | None = None) -> BatchEngine:
-    """lazily created, per-node engine (also used by the object-level BaseNodeDef.handler)"""
+               extra_topics: list[str] | None = None, isolation_level: str | None = None) -> BatchEngine:
+    """lazily created, per-node engine (also used by the object-level BaseNodeDef.handler); isolation_level: what the
+    fetches the node submits from now on deliver (BatchEngine.set_isolation_level), None: as it is"""
     eng = getattr(node, "_ck_engine", None)     # the engine lives (and dies) with its node: no id()-keyed registry
     if eng is None:
         eng = BatchEngine(device, max_records=max_records, max_in_bytes=max_in_bytes,
@@ -55,6 +57,8 @@ def engine_for(node: BaseNodeDef, *, device: int = 0, max_records: int = 1 << 14
         eng.register_topics(topics + (extra_topics or []), num_partitions=0)
         node.configure_engine(eng)
         node._ck_engine = eng
+    if isolation_level is not None:
+        eng.set_isolation_level(isolation_level)
     return eng
 
 
@@ -172,22 +176,36 @@ class Worker:
         broker.produce_publishes(batch)
 
     # ---- host-side nodes (Python tools, the Agent's LLM boundary): per-record objects are inherent there -----------
-    def _run_host(self, node: BaseNodeDef, records: list[Record], **kw: Any) -> None:
+    def _run_host(self, node: BaseNodeDef, records: list[Record] | FetchArena, **kw: Any) -> None:
         """never loses a dequeued record: an engine-level failure (a batch the buffers cannot hold) splits the batch and
-        retries; a single record that still fails is logged and dropped alone"""
+        retries, a fetch response at frame boundaries; a single record, or a single frame, that still fails is logged and
+        dropped alone"""
         broker = self._client._connection
-        engine = engine_for(node, device=self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes)
+        engine = engine_for(node, device=self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes,
+                            isolation_level=self._levels.get(id(node), "read_uncommitted"))
+        fetch = isinstance(records, FetchArena)
+        skipped = engine.skipped if fetch else 0
         try:
             broker.produce_batch(node.process_batch(engine, records, **kw) if kw else node.process_batch(engine, records))
-            self.stats["records"] += 0 if kw else len(records)
+            self.stats["records"] += 0 if kw else (records.n if fetch else len(records))
+            if fetch:
+                self.stats["skipped"] += engine.skipped - skipped
         except Exception:  # noqa: BLE001  (EngineError: capacity; user code outside the per-record guards)
-            if len(records) == 1:
-                logger.exception("node %s: record dropped after failing alone", node.name)
+            pieces = len(records.frames()[1]) if fetch else len(records)
+            if pieces <= 1:
+                if fetch:
+                    logger.exception("node %s: frame of %d records dropped after failing alone", node.name, records.n)
+                else:
+                    logger.exception("node %s: record dropped after failing alone", node.name)
                 return
-            mid = len(records) // 2
-            logger.warning("node %s: batch of %d failed, retrying in halves", node.name, len(records))
-            self._run_host(node, records[:mid], **kw)
-            self._run_host(node, records[mid:], **kw)
+            mid = pieces // 2
+            logger.warning("node %s: batch of %d %s failed, retrying in halves", node.name, pieces, "frames" if fetch else "records")
+            if fetch:
+                self._run_host(node, records.slice_frames(0, mid), **kw)
+                self._run_host(node, records.slice_frames(mid, None), **kw)
+            else:
+                self._run_host(node, records[:mid], **kw)
+                self._run_host(node, records[mid:], **kw)
 
     def _frame_codec(self) -> str | None:
         """the broker's compression_type for the frames built on the device: None or "lz4"; any other codec is refused"""
@@ -251,6 +269,14 @@ class Worker:
                 for rb in pipe.take_received():                # forwarded here by the owners of other partitions' inputs
                     self.stats["received"] = self.stats.get("received", 0) + rb.n_publishes
                     broker.produce_publishes(rb)
+                continue
+            fetch = broker.poll_fetch(sub.topics, self._batch_records, self._batch_bytes)
+            if fetch is not None:
+                consumed += fetch.n
+                try:
+                    self._run_host(node, fetch)
+                finally:
+                    fetch.release()
                 continue
             records: list[Record] = broker.poll_batch(sub.topics, self._batch_records, self._batch_bytes)
             if not records:
