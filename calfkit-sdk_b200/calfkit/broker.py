@@ -30,6 +30,14 @@ Kafka's own granularity — record batches — at both ends:
     CPU encoder: without a framer, flushing them fails loudly.  `MemoryBroker(compression_type="lz4")` (the keyword a
     FastStream KafkaBroker takes) makes every frame an LZ4-compressed batch, compressed on the device; other codecs are
     refused by the Worker when frame sinks are registered.
+Idempotent and transactional produce (KIP-98), as aiokafka and the Java producer apply `enable_idempotence=True` and
+`transactional_id="..."` (which implies idempotence): `init_producer_id` hands out producer ids and epochs; every frame
+carries its producer's id and epoch, and the broker writes its baseSequence when it hands the frame to its sink, from one
+counter per (producer id, topic, partition): contiguous per partition in the order frames reach the sinks, whichever
+engine built them.  A topic's unkeyed publishes go to one sticky partition per frame pass (`next_sticky`), advanced round
+robin, so every frame has a partition.  With a transactional id, each Worker.run tick is one transaction: data frames
+carry attributes bit 4, and when the tick ends every (topic, partition) that received frames in it gets a COMMIT marker
+(a control batch) through the same sink, or an ABORT marker when the tick raised.
 Publishes to topics nobody subscribes to are counted and dropped when they arrive batch-wise (a long-running worker must
 not grow without bound); per-record publishes are kept (tests read such topics afterwards).
 Limitation (documented, not hidden): one shared queue per topic — consumer GROUPS are not modelled (two subscriptions to
@@ -84,6 +92,14 @@ class MemoryBroker:
         # (compressed on the device); the Worker refuses any other codec when frame sinks are registered
         self.compression_type: str | None = kwargs.get("compression_type")
         self.num_partitions = num_partitions       # partitions per topic (Kafka's default partitioner: murmur2(key) % partitions)
+        # idempotent / transactional produce (frame sinks): KafkaBroker(enable_idempotence=True) / (transactional_id="...")
+        self.transactional_id: str | None = kwargs.get("transactional_id")
+        self.enable_idempotence: bool = bool(kwargs.get("enable_idempotence")) or self.transactional_id is not None
+        self._next_pid = 0
+        self._txn_producers: dict[str, tuple[int, int]] = {}          # transactional id -> (producer id, epoch)
+        self._seq: dict[tuple[int, str, int], int] = {}               # (producer id, topic, partition) -> next baseSequence
+        self._sticky: dict[str, int] = {}                             # topic -> sticky partition of the next pass
+        self._txn: dict[tuple[str, int], tuple[int, int]] | None = None   # open transaction: (topic, partition) -> (pid, epoch)
         self._connection: Any = None
         self.queues: dict[str, deque[Record]] = defaultdict(deque)
         self.arenas: dict[str, deque] = defaultdict(deque)            # topic -> deque[Arena]
@@ -114,7 +130,10 @@ class MemoryBroker:
         RecordBatch v2 frame built on the device (partition None: unkeyed records, the producer client picks one).  The
         frame (uint8 array) is valid during the call, like `sink`'s batch.  With compression_type="lz4" every frame is an
         LZ4-compressed batch (attributes 3) as Kafka clients decode it; the table's records count stays the uncompressed
-        one."""
+        one.  With enable_idempotence or a transactional_id the partition is always an int (unkeyed records went to their
+        topic's sticky partition), the frame carries producerId, producerEpoch and its baseSequence, and under a
+        transactional_id fn also receives each partition's COMMIT / ABORT marker: a control batch (attributes 0x30) of one
+        record, n_records 1."""
         self.frame_sinks[topic] = fn
 
     def publisher(self, topic: str, **kwargs: Any):
@@ -162,8 +181,79 @@ class MemoryBroker:
                     frames.release()
 
     def _hand_frames(self, frames) -> None:
+        if not self.enable_idempotence:
+            for topic, part, frame, n in frames:
+                self.frame_sinks[topic](topic, part, frame, n)
+            return
+        from calfkit.engine.batch import patch_base_sequence
+        from calfkit.exceptions import EngineError
         for topic, part, frame, n in frames:
+            pid, epoch = int.from_bytes(frame[43:51].tobytes(), "big", signed=True), int.from_bytes(frame[51:53].tobytes(), "big", signed=True)
+            if pid < 0 or part is None:
+                raise EngineError(f"frame for {topic!r} without a producer id or a partition: the engine that built it was not set up for idempotence")
+            key = (pid, topic, part)
+            seq = self._seq.get(key, 0)
+            patch_base_sequence(frame, seq)
+            self._seq[key] = (seq + n) & 0x7FFFFFFF               # DefaultRecordBatch.incrementSequence: wraps to 0
+            if frame[22] & 0x10:
+                if self._txn is None:
+                    raise EngineError(f"transactional frame for {topic!r} outside a transaction (begin_transaction first)")
+                self._txn.setdefault((topic, part), (pid, epoch))
             self.frame_sinks[topic](topic, part, frame, n)
+
+    # --- idempotent / transactional produce -------------------------------------------------------------
+    def init_producer_id(self, transactional_id: str | None = None) -> tuple[int, int]:
+        """(producer id, epoch) of a new producer (Kafka's InitProducerId): a fresh id for an idempotent producer; a
+        transactional id keeps its producer id and each call bumps its epoch, fencing the previous holder.  The sequences
+        of a re-initialised producer start again at 0"""
+        if transactional_id is not None and transactional_id in self._txn_producers:
+            pid, epoch = self._txn_producers[transactional_id]
+            epoch += 1
+            if epoch > 0x7FFF:                                # the epoch is an i16: exhausted, a fresh id as Kafka gives one
+                pid, epoch = self._next_pid, 0
+                self._next_pid += 1
+            self._seq = {k: v for k, v in self._seq.items() if k[0] != pid}
+        else:
+            pid, epoch = self._next_pid, 0
+            self._next_pid += 1
+        if transactional_id is not None:
+            self._txn_producers[transactional_id] = (pid, epoch)
+        return pid, epoch
+
+    def next_sticky(self, topics) -> dict[str, int]:
+        """the sticky partition of each topic's unkeyed publishes for one frame pass; each call moves every one of these
+        topics to its next partition, round robin (Kafka's uniform sticky partitioner, switching per pass)"""
+        out = {}
+        for t in topics:
+            p = self._sticky.get(t, 0)
+            out[t] = p
+            self._sticky[t] = (p + 1) % max(self.num_partitions, 1)
+        return out
+
+    def begin_transaction(self) -> None:
+        from calfkit.exceptions import EngineError
+        if self._txn is not None:
+            raise EngineError("a transaction is already open")
+        self._txn = {}
+
+    def commit_transaction(self) -> None:
+        """end the open transaction: a COMMIT marker to every (topic, partition) that received its frames"""
+        self._end_transaction(True)
+
+    def abort_transaction(self) -> None:
+        """end the open transaction: an ABORT marker to every (topic, partition) that received its frames"""
+        self._end_transaction(False)
+
+    def _end_transaction(self, commit: bool) -> None:
+        import time
+        from calfkit.engine.batch import control_batch
+        from calfkit.exceptions import EngineError
+        if self._txn is None:
+            raise EngineError("no transaction is open")
+        touched, self._txn = self._txn, None
+        ts = int(time.time() * 1000)
+        for (topic, part), (pid, epoch) in touched.items():
+            self.frame_sinks[topic](topic, part, control_batch(pid, epoch, commit, ts), 1)
 
     def produce_batch(self, records: list[Record]) -> None:
         for r in records:

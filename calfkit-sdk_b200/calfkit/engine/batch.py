@@ -170,10 +170,35 @@ class BatchOutput:
                           int(p["partition"]))
 
 
+def patch_base_sequence(frame: np.ndarray, seq: int) -> None:
+    """write baseSequence `seq` into a RecordBatch v2 frame (uint8 array, in place) and patch its CRC32C by linearity
+    (ck_crc32c_patch: O(log length), however long the frame)"""
+    new = np.frombuffer((seq & 0xFFFFFFFF).to_bytes(4, "big"), dtype=np.uint8)
+    old = frame[SEQ_AT:SEQ_AT + 4].copy()
+    crc = C.c_uint32(int.from_bytes(frame[17:21].tobytes(), "big"))
+    lib = _lib.load()
+    if lib.ck_crc32c_patch(C.byref(crc), len(frame) - 21, SEQ_AT - 21, ptr(old), ptr(new)):
+        raise EngineError(lib.ck_last_error(None).decode())
+    frame[SEQ_AT:SEQ_AT + 4] = new
+    frame[17:21] = np.frombuffer(crc.value.to_bytes(4, "big"), dtype=np.uint8)
+
+
+def control_batch(producer_id: int, producer_epoch: int, commit: bool, timestamp_ms: int, base_offset: int = 0) -> np.ndarray:
+    """the COMMIT or ABORT marker the broker appends to a partition when a transaction ends (ck_encode_control_batch)"""
+    lib = _lib.load()
+    out, n = np.empty(78, dtype=np.uint8), C.c_uint64(0)
+    if lib.ck_encode_control_batch(base_offset, timestamp_ms, producer_id, producer_epoch, 1 if commit else 0, ptr(out), out.nbytes, C.byref(n)):
+        raise EngineError(lib.ck_last_error(None).decode())
+    return out[:n.value]
+
+
+SEQ_AT = 53                    # baseSequence i32 in a RecordBatch v2 header (producerId i64 at 43, producerEpoch i16 at 51)
+
+
 class Frames:
     """Kafka RecordBatch v2 frames of one frame pass, produce-ready: `table` (FRAME_DTYPE: topic id, partition, records,
     first record, offset, length) and the frame bytes back to back in `data`.  Partition -1 holds unkeyed records: the
-    producer client picks their partition."""
+    producer client picks their partition (with sticky partitions set, BatchEngine.set_sticky_partitions, they have one)."""
 
     def __init__(self, table: np.ndarray, data: np.ndarray, topic_names: dict[int, str], on_release=None):
         self.table, self.data, self.topic_names, self._on_release = table, data, topic_names, on_release
@@ -474,6 +499,25 @@ class BatchEngine:
         if codec not in FRAME_CODECS:
             raise EngineError(f"frame compression {codec!r} is not supported (None or 'lz4')")
         self._check(self.lib.ck_set_option(self.h, 3, FRAME_CODECS[codec]))
+
+    def set_producer(self, pid: int, epoch: int, transactional: bool = False) -> None:
+        """the producer fields of the frames the following passes build (ck_set_producer): pid -1 none (producerId and
+        producerEpoch -1, the default); else the idempotent producer (pid, epoch), with attributes bit 4 when transactional.
+        baseSequence stays -1: the broker writes it at hand-off (patch_base_sequence)"""
+        flags = 0 if pid < 0 else 1 | (2 if transactional else 0)
+        self._check(self.lib.ck_set_producer(self.h, pid, epoch if pid >= 0 else -1, flags))
+
+    def set_sticky_partitions(self, sticky: dict[str, int] | None) -> None:
+        """topic -> the partition its unkeyed publishes join in the following passes (ck_set_sticky_partitions); None or {}:
+        they stay the partition -1 group"""
+        sticky = sticky or {}
+        missing = [t for t in sticky if t not in self.topic_ids]
+        if missing:
+            raise EngineError(f"sticky partitions of topics not registered: {missing}")
+        parts = np.full(max([self.topic_ids[t] + 1 for t in sticky] or [0]), -1, dtype=np.int32)
+        for t, p in sticky.items():
+            parts[self.topic_ids[t]] = p
+        self._check(self.lib.ck_set_sticky_partitions(self.h, ptr(parts) if len(parts) else None, len(parts)))
 
     def encode_frames(self, timestamp_ms: int) -> None:
         """queue the frame pass over the current plan: every live publish to a frame topic, grouped by (topic, partition)

@@ -361,11 +361,12 @@ class Lane:
             rank, world = exchange
             self.px = PeerExchange(self.eng, rank, world, max_fwd=max_records, data_cap=max_in_bytes + 64 * max_records)
 
-    def submit(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None) -> None:
+    def submit(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None, sticky: dict[str, int] | None = None) -> None:
         """device-template tool node: decode + plan + encode + route (+ frame pass, + forward to the owning ranks), all
         asynchronous.  A FetchArena goes to the device as it is (ck_submit_recordbatch), with its read_committed mask when
         the engine's isolation level is read_committed.  With frame topics set on the engine,
-        their publishes are framed with baseTimestamp timestamp_ms (default: now)"""
+        their publishes are framed with baseTimestamp timestamp_ms (default: now), and, given `sticky` (topic -> partition),
+        the unkeyed ones join that partition of their topic (BatchEngine.set_sticky_partitions)"""
         self.arena, self.busy = arena, True
         eng = self.eng
         if isinstance(arena, FetchArena):
@@ -378,6 +379,8 @@ class Lane:
             eng.submit(arena.data, arena.offsets)
         eng.tool_plan()
         if eng.frame_topics:
+            if sticky is not None:
+                eng.set_sticky_partitions(sticky)
             eng.encode_frames(int(time.time() * 1000) if timestamp_ms is None else timestamp_ms)
         if self.px is not None:
             self.step_no += 1
@@ -510,13 +513,13 @@ class LanePipeline:
         self._k = 0
         self._inflight: list[Lane] = []
 
-    def push(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None) -> PublishBatch | None:
+    def push(self, arena: "Arena | FetchArena", timestamp_ms: int | None = None, sticky: dict[str, int] | None = None) -> PublishBatch | None:
         """queue one step; returns the results of an older step once the pipe is full.  Order of work per call:
         (1) H2D + kernels of the new step are queued, (2) the copy-back that was started by the previous call is
         awaited and handed out, (3) the copy-back of the next-oldest step is started — it runs while the caller
         produces the batch just returned and while the new step computes."""
         lane = next(l for l in self.lanes if not l.busy)    # invariant: at most K-1 lanes busy between calls
-        lane.submit(arena, timestamp_ms)
+        lane.submit(arena, timestamp_ms, sticky)
         self._inflight.append(lane)
         ready = None
         if self._inflight[0].collecting:

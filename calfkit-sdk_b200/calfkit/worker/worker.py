@@ -15,10 +15,16 @@ A poll is bounded by records AND bytes, an engine-level failure splits the batch
 lost), and records the device declines as CK_UNSUPPORTED are re-run through the host-tool path.  Records of a fetch
 response that a consumer does not deliver (control batches; under the subscriber's isolation_level="read_committed" the
 aborted transactions' batches) come out CK_SKIPPED: counted in stats["skipped"], neither logged nor re-run.
+
+A broker with enable_idempotence or a transactional_id (frame sinks only) gives the Worker one producer id and epoch
+(MemoryBroker.init_producer_id) when it builds its first engine that frames; every lane engine and the framer engine write
+them into their frames, and each frame pass takes the broker's next sticky partitions for the unkeyed publishes.  With a
+transactional_id, each tick of run() is one transaction: committed when the tick ends, aborted when it raises.
 """
 from __future__ import annotations
 
 import asyncio
+import contextlib
 import logging
 import os
 import time
@@ -103,6 +109,7 @@ class Worker:
         self._framer_eng: BatchEngine | None = None
         self._frame_pool = None
         self._levels: dict[int, str] = {}          # node -> its subscription's isolation_level
+        self._producer: tuple[int, int] | None = None   # (producer id, epoch) of an idempotent broker, taken once
         self.stats = {"records": 0, "publishes": 0, "rejected": 0, "skipped": 0, "raises": 0, "host_fallback": 0, "steps": 0}
 
     def add_nodes(self, *nodes: BaseNodeDef) -> None:
@@ -136,6 +143,7 @@ class Worker:
             topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics + frame_topics
             codec = self._frame_codec() if frame_topics else None
             level = self._levels.get(id(node), "read_uncommitted")
+            producer = self._producer_of(self._client._connection) if frame_topics else None
 
             def configure(eng: BatchEngine) -> None:
                 eng.register_topics(topics, num_partitions=getattr(self._client._connection, "num_partitions", 0))
@@ -144,6 +152,8 @@ class Worker:
                 if frame_topics:
                     eng.set_frame_topics(frame_topics)
                     eng.set_frame_compression(codec)
+                    if producer is not None:
+                        eng.set_producer(*producer)
             pipe = LanePipeline(self._device, configure, lanes=self._lanes, max_records=self._batch_records,
                                 max_in_bytes=self._batch_bytes, exchange=(self._rank, self._world) if self._world > 1 else None)
             self._pipes[id(node)] = pipe
@@ -207,6 +217,28 @@ class Worker:
                 self._run_host(node, records[:mid], **kw)
                 self._run_host(node, records[mid:], **kw)
 
+    def _producer_of(self, broker) -> tuple[int, int, bool] | None:
+        """(producer id, epoch, transactional) the engines that frame write into their frames; None: not idempotent"""
+        if not getattr(broker, "enable_idempotence", False):
+            return None
+        if self._producer is None:
+            self._producer = broker.init_producer_id(broker.transactional_id)
+        return self._producer + (broker.transactional_id is not None,)
+
+    @contextlib.contextmanager
+    def _transaction(self, broker):
+        """one tick of run() under a transactional broker: committed when it ends, aborted (then re-raised) when it raises"""
+        if getattr(broker, "transactional_id", None) is None:
+            yield
+            return
+        broker.begin_transaction()
+        try:
+            yield
+        except BaseException:
+            broker.abort_transaction()
+            raise
+        broker.commit_transaction()
+
     def _frame_codec(self) -> str | None:
         """the broker's compression_type for the frames built on the device: None or "lz4"; any other codec is refused"""
         codec = getattr(self._client._connection, "compression_type", None)
@@ -222,6 +254,9 @@ class Worker:
             self._framer_eng = BatchEngine(self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes)
             self._framer_eng.register_topics(list(broker.frame_sinks), num_partitions=getattr(broker, "num_partitions", 0))
             self._framer_eng.set_frame_compression(self._frame_codec())
+            producer = self._producer_of(broker)
+            if producer is not None:
+                self._framer_eng.set_producer(*producer)
             self._frame_pool = PinnedPool()
         eng, ts = self._framer_eng, int(time.time() * 1000)
         if topic not in eng.topic_ids:
@@ -237,6 +272,8 @@ class Worker:
                     break
                 nbytes += size
                 b += 1
+            if getattr(broker, "enable_idempotence", False):
+                eng.set_sticky_partitions(broker.next_sticky([topic]))
             eng.encode_frames_records(topic, [(r.value, r.key, r.correlation_id) for r in records[a:b]], ts)
             yield eng.fetch_frames(self._frame_pool)
             a = b
@@ -259,7 +296,12 @@ class Worker:
                 if arena is not None:
                     consumed += arena.n
                     # the step's timestamp is the frames' baseTimestamp (only framing lanes use it)
-                    done = pipe.push(arena, int(time.time() * 1000)) if broker.frame_sinks else pipe.push(arena)
+                    if not broker.frame_sinks:
+                        done = pipe.push(arena)
+                    elif getattr(broker, "enable_idempotence", False):
+                        done = pipe.push(arena, int(time.time() * 1000), broker.next_sticky(broker.frame_sinks))
+                    else:
+                        done = pipe.push(arena, int(time.time() * 1000))
                     if done is not None:
                         self._produce_fast(node, done)
                 elif pipe.pending:                             # input idle (single rank): flush what is in flight
@@ -315,10 +357,12 @@ class Worker:
         if not broker._connection:
             await broker.start()
         while True:
-            n = self.step()
-            n += await self._client._dispatcher.drain(broker) if hasattr(self._client, "_dispatcher") else 0
-            if self._all_idle(n + sum(p.pending_records for p in self._pipes.values())):
-                if until_idle:
+            finished = False
+            with self._transaction(broker):                # a transactional broker: one transaction per tick
+                n = self.step()
+                n += await self._client._dispatcher.drain(broker) if hasattr(self._client, "_dispatcher") else 0
+                idle = self._all_idle(n + sum(p.pending_records for p in self._pipes.values()))
+                if idle and until_idle:
                     flushed = 0
                     for node, _sub in self._subs:          # nothing in flight on any rank: flush (no exchange involved)
                         pipe = self._pipes.get(id(node))
@@ -330,9 +374,10 @@ class Worker:
                                 flushed += rb.n_publishes
                                 broker.produce_publishes(rb)
                     broker.flush_frames()
-                    if self._all_idle(flushed):            # nothing came out that a subscribed node still has to consume
-                        return
-                    continue
+                    finished = self._all_idle(flushed)     # nothing came out that a subscribed node still has to consume
+            if finished:
+                return
+            if idle and not until_idle:
                 await asyncio.sleep(idle_sleep)
-            else:
+            elif not idle:
                 await asyncio.sleep(0)

@@ -73,6 +73,11 @@ struct ck_handle {
     const u32* fr_order = nullptr; long long fr_base = 0, fr_ts = 0;   // what the write half of the last pass needs to run again
     u8* d_fr_blob = nullptr; long long* d_fr_desc = nullptr; long long* h_fr_info = nullptr;   // h_fr_info: pinned {frames, bytes}
     int32_t* d_fr_slot = nullptr; u32 fr_nslots = 0, fr_ntopics = 0;
+    // idempotent / transactional produce: the producer fields the passes write (ck_set_producer; fr_prod: those of the last
+    // pass, which a rewrite into a grown buffer uses again) and, by topic id, the sticky partition of the topic's unkeyed
+    // publishes (ck_set_sticky_partitions; host copy for the record form, device copy for the plan's publishes)
+    ck_producer prod{-1, -1, 0}, fr_prod{-1, -1, 0};
+    std::vector<int32_t> fr_sticky; int32_t* d_fr_sticky = nullptr; u32 fr_sticky_cap = 0;
     uint64_t fr_window = 1ull << 20;                 // frame_bytes (ck_set_option 2)
     // LZ4 frames (ck_set_option 3; allocated on the first compressed pass): the uncompressed frames, then the block slots,
     // each fr_raw_cap bytes; per block slot its size and their scan; the offsets of the compressed frames
@@ -214,7 +219,8 @@ extern "C" void ck_destroy(ck_handle* h) {
                      h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
                      h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
                      h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
-                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag, h->d_rb_sn};
+                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag, h->d_rb_sn,
+                     h->d_fr_sticky};
     for (void* p : gptrs) if (p) cudaFree(p);
     if (h->h_rb_doff) cudaFreeHost(h->h_rb_doff);
     if (h->h_rb_flag) cudaFreeHost(h->h_rb_flag);
@@ -915,6 +921,22 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     return 0;
 }
 
+// idempotent produce's sequence hand-off: the CRC32C of a span after 4 of its bytes changed (ck_txn_crc32c_patch)
+extern "C" int ck_crc32c_patch(uint32_t* crc, uint64_t len, uint64_t pos, const uint8_t* old4, const uint8_t* new4) {
+    if (len < 4 || pos > len - 4) { g_create_error = "ck_crc32c_patch: the 4 bytes lie outside the span"; return 1; }
+    *crc = ck_txn_crc32c_patch(*crc, len, pos, old4, new4);
+    return 0;
+}
+
+// a transaction marker as the broker appends it (ck_txn_control_batch): no handle, no device
+extern "C" int ck_encode_control_batch(int64_t base_offset, int64_t timestamp_ms, int64_t producer_id, int16_t producer_epoch,
+                                       int16_t type, uint8_t* out, uint64_t cap, uint64_t* len) {
+    if (cap < CK_TXN_CONTROL_LEN) { g_create_error = "ck_encode_control_batch: buffer shorter than a control batch"; return 1; }
+    ck_txn_control_batch(out, base_offset, timestamp_ms, producer_id, producer_epoch, type);
+    if (len) *len = CK_TXN_CONTROL_LEN;
+    return 0;
+}
+
 // the read_committed mask of a whole fetch (ck_txn_mask): no handle, no device
 extern "C" int ck_fetch_txn_mask(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
                                  const uint32_t* abort_run, const int64_t* abort_pid, const int64_t* abort_first, uint32_t naborts,
@@ -1024,7 +1046,7 @@ static int fr_alloc(ck_handle* h) {
 static int frame_write(ck_handle* h);
 static int lz_compress(ck_handle* h);
 static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long long window, long long base_offset, long long ts) {
-    h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec;
+    h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec; h->fr_prod = h->prod;
     if (!n) return 0;
     if (h->fr_pass_codec && !h->d_fr_raw && lz_grow(h, h->fr_cap)) return 1;
     const u32* order = nullptr;
@@ -1083,7 +1105,7 @@ static int frame_write(ck_handle* h) {
     {
         KTimer t(h, CK_K_FRAME);   // chunk counts per frame go to d_fr_head (free again), their scan to d_fr_S
         CKL(h) ck_fr_table_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_ffirst, h->d_fr_F, h->d_fr_R, n, h->d_fr_nlive,
-                                                          h->fr_base, h->fr_ts, cap, h->d_fr_table, dst, h->d_fr_head);
+                                                          h->fr_base, h->fr_ts, h->fr_prod, cap, h->d_fr_table, dst, h->d_fr_head);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (!lz && run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
@@ -1174,10 +1196,39 @@ extern "C" int ck_encode_frames(ck_handle* h, int64_t timestamp_ms) {
     {
         KTimer t(h, CK_K_FRAME);
         if (n) CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, nullptr, n, h->d_pay_len, h->d_out_off, h->d_out,
-            h->d_cols, h->n, h->d_fr_slot, h->fr_nslots, h->num_partitions, excl, h->d_fr_items, h->d_fr_gkey);
+            h->d_cols, h->n, h->d_fr_slot, h->fr_nslots, h->num_partitions, excl, h->fr_sticky.empty() ? nullptr : h->d_fr_sticky,
+            (u32)h->fr_sticky.size(), h->d_fr_items, h->d_fr_gkey);
         CUDA_TRY(h, cudaGetLastError());
     }
     return frame_pass(h, n, passes, excl, h->fr_window, 0, timestamp_ms);
+}
+
+// the producer fields of the following passes' frames: flags 0 none (producerId / producerEpoch -1), CK_PRODUCER_IDEMPOTENT
+// pid and epoch, | CK_PRODUCER_TRANSACTIONAL and attributes bit 4
+extern "C" int ck_set_producer(ck_handle* h, int64_t pid, int16_t epoch, uint32_t flags) {
+    if (flags & ~(u32)(CK_PRODUCER_IDEMPOTENT | CK_PRODUCER_TRANSACTIONAL)) return fail(h, "ck_set_producer: unknown flags");
+    if (flags && !(flags & CK_PRODUCER_IDEMPOTENT)) return fail(h, "ck_set_producer: a transactional producer is idempotent");
+    if (flags && (pid < 0 || epoch < 0)) return fail(h, "ck_set_producer: producer id and epoch must be >= 0");
+    h->prod = flags ? ck_producer{(long long)pid, (int)epoch, (flags & CK_PRODUCER_TRANSACTIONAL) ? 0x10u : 0u} : ck_producer{-1, -1, 0};
+    return 0;
+}
+
+// parts[topic id] for ids < n: the partition of the topic's unkeyed publishes in the following passes (-1: they stay the
+// partition -1 group); n = 0 clears the table.  The copy is queued on the stream, ahead of the passes that read it
+extern "C" int ck_set_sticky_partitions(ck_handle* h, const int32_t* parts, uint32_t n) {
+    cudaSetDevice(h->device);
+    for (u32 i = 0; i < n; i++)
+        if (parts[i] < -1 || (parts[i] >= 0 && (u32)parts[i] >= h->num_partitions))
+            return fail(h, "ck_set_sticky_partitions: a partition outside [0, num_partitions)");
+    if (n > h->fr_sticky_cap) {
+        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+        if (h->d_fr_sticky) { cudaFree(h->d_fr_sticky); h->d_fr_sticky = nullptr; }
+        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_sticky, sizeof(int32_t) * n));
+        h->fr_sticky_cap = n;
+    }
+    h->fr_sticky.assign(parts, parts + n);
+    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_sticky, h->fr_sticky.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    return 0;
 }
 
 // records a host path produced for one topic (host tools, the LLM boundary, declined records re-run on the host)
@@ -1205,8 +1256,9 @@ extern "C" int ck_encode_frames_records(ck_handle* h, int32_t topic_id, const ui
     if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_desc, host_desc, sizeof(long long) * 6 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
     {
         KTimer t(h, CK_K_FRAME);
+        int32_t sticky = topic_id >= 0 && (size_t)topic_id < h->fr_sticky.size() ? h->fr_sticky[topic_id] : -1;
         if (n) CKL(h) ck_fr_src_recs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_fr_blob, h->d_fr_desc, n, topic_id, h->num_partitions,
-                                                                                   h->d_fr_items, h->d_fr_gkey);
+                                                                                   sticky, h->d_fr_items, h->d_fr_gkey);
         CUDA_TRY(h, cudaGetLastError());
     }
     return frame_pass(h, n, passes, (u32)((1ull << (6 * passes)) - 1), h->fr_window, 0, timestamp_ms);
@@ -1261,7 +1313,7 @@ extern "C" int ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uin
     {
         KTimer t(h, CK_K_FRAME);
         CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, h->d_fr_idx, n, h->d_pay_len, h->d_out_off, h->d_out,
-            h->d_cols, h->n, nullptr, 0, 0, CK_RB_NONE, h->d_fr_items, h->d_fr_gkey);
+            h->d_cols, h->n, nullptr, 0, 0, CK_RB_NONE, nullptr, 0, h->d_fr_items, h->d_fr_gkey);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (frame_pass(h, n, 0, CK_RB_NONE, ~0ull, base_offset, timestamp_ms)) return 1;

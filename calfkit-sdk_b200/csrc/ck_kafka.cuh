@@ -362,7 +362,9 @@ ck_rb_mark_bad_kernel(const u32* __restrict__ rec_bad, u32 n, u32* __restrict__ 
 // Every live publish to a frame topic of the current plan (or every record of a small host-produced batch) becomes one
 // record of a frame, in one pass queued on the stream (nothing in it waits for the host):
 //   source   thread per publish / record: its value, key and correlation id (ck_fitem) and its group key (frame topic,
-//            partition + 1); partition -1 (unkeyed) is a group of its own per topic, the producer client picks its partition
+//            partition + 1); partition -1 (unkeyed) is a group of its own per topic, the producer client picks its partition,
+//            unless the host gave the topic a sticky partition for the pass (idempotent produce: a sequence exists only per
+//            partition), which the unkeyed publishes then join before the key is built
 //   group    stable LSD radix sort by the group key (group_sort, ck_group.cuh): one run per group, send order kept
 //   split    s_k = encoded size of record k with offsetDelta = its rank in the group, P_k = exclusive prefix of s inside the
 //            group; record k starts a frame when it heads its group or floor(P_k / W) != floor(P_{k-1} / W), W = frame_bytes.
@@ -400,6 +402,10 @@ struct ck_fitem {                    // one record to frame
     u32 corr_raw, corr_len;          // same for the correlation_id header (CK_RB_NONE: no header)
     int32_t topic_id, partition;
 };
+// the producer fields of a pass's frame headers (ck_set_producer): none = producerId -1, producerEpoch -1, attributes 0;
+// idempotent = the producer's id and epoch; transactional = those and attributes bit 4.  baseSequence is always -1 here: the
+// host writes each frame's sequence when it hands the frame out, and patches the CRC32C (ck_crc32c_patch)
+struct ck_producer { long long pid; int epoch; u32 attr; };
 struct ck_frame_ent {                // one frame of the frame table (mirrors ck_frame in include/calfkit_b200.h)
     int32_t topic_id, partition;     // partition -1: unkeyed records, the producer client picks the partition
     uint32_t n_records, first;       // records, first record in group order
@@ -425,12 +431,13 @@ __device__ __forceinline__ u32 ck_rb_measure(const ck_fitem& it, u32 rank) {
 __device__ __forceinline__ u32 ck_rb_encoded_size(const ck_fitem& it, u32 rank) { u32 b = ck_rb_measure(it, rank); return ck_varint_size(b) + b; }
 
 // source: publishes idx[i] (NULL: publish i) of the plan.  frame_slot[topic id] = index of the frame topic or -1; NULL: one
-// group for all of them (ck_encode_recordbatch).  Unframed slots get the key `excl`, which sorts last
+// group for all of them (ck_encode_recordbatch).  Unframed slots get the key `excl`, which sorts last.  sticky[topic id]
+// (n_sticky of them; NULL: none): the partition the topic's unkeyed publishes go to in this pass, -1 none
 __global__ void __launch_bounds__(256)
 ck_fr_src_pubs_kernel(ck_view vw, const ck_pub* __restrict__ pubs, const u32* __restrict__ idx, u32 n, const u32* __restrict__ pay_len,
                       const long long* __restrict__ out_off, const u8* __restrict__ out, const u32* __restrict__ cols, u32 stride,
                       const int32_t* __restrict__ frame_slot, u32 n_slots, u32 nparts, u32 excl,
-                      ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
+                      const int32_t* __restrict__ sticky, u32 n_sticky, ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     ck_pub p = pubs[idx ? idx[i] : i];
@@ -444,15 +451,17 @@ ck_fr_src_pubs_kernel(ck_view vw, const ck_pub* __restrict__ pubs, const u32* __
     it.corr = rec + co; it.corr_raw = cl; it.corr_len = ck_unescaped_len(it.corr, cl);
     it.key = it.corr; it.key_raw = p.has_key ? cl : CK_RB_NONE; it.key_len = p.has_key ? it.corr_len : CK_RB_NONE;
     it.topic_id = p.topic_id; it.partition = p.has_key ? p.partition : -1;
+    if (!p.has_key && sticky && (u32)p.topic_id < n_sticky) it.partition = sticky[p.topic_id];
     items[i] = it;
     gkey[i] = frame_slot ? (u32)slot * (nparts + 1) + (u32)(it.partition + 1) : 0u;
 }
 
 // source: records a host path produced for one topic.  desc[i] = {value off, len, key off, len, correlation id off, len}
-// into blob (len -1: absent); key and id are JSON string content, the partition is the plan's: murmur2(key) % nparts
+// into blob (len -1: absent); key and id are JSON string content, the partition is the plan's: murmur2(key) % nparts, or
+// for an unkeyed record `sticky` (the topic's sticky partition of the pass; -1: none)
 __global__ void __launch_bounds__(256)
 ck_fr_src_recs_kernel(const u8* __restrict__ blob, const long long* __restrict__ desc, u32 n, int32_t topic_id, u32 nparts,
-                      ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
+                      int32_t sticky, ck_fitem* __restrict__ items, u32* __restrict__ gkey) {
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long* d = desc + 6 * (size_t)i;
@@ -460,7 +469,7 @@ ck_fr_src_recs_kernel(const u8* __restrict__ blob, const long long* __restrict__
     it.val = blob + d[0]; it.val_len = (u32)d[1];
     it.key = blob + (d[3] >= 0 ? d[2] : 0); it.key_raw = d[3] >= 0 ? (u32)d[3] : CK_RB_NONE; it.key_len = ck_unescaped_len(it.key, it.key_raw);
     it.corr = blob + (d[5] >= 0 ? d[4] : 0); it.corr_raw = d[5] >= 0 ? (u32)d[5] : CK_RB_NONE; it.corr_len = ck_unescaped_len(it.corr, it.corr_raw);
-    int part = -1;
+    int part = sticky;
     if (it.key_raw != CK_RB_NONE && nparts) { GRd r; r.init(it.key, it.key_raw); part = (int)((ck_murmur2_key(r, 0, it.key_raw) & 0x7fffffffu) % nparts); }
     it.topic_id = topic_id; it.partition = part;
     items[i] = it;
@@ -507,18 +516,19 @@ ck_fr_split_kernel(const u32* __restrict__ head, const long long* __restrict__ g
     fstart[k] = (unsigned long long)(S[k] - base) / window != (unsigned long long)(S[k - 1] - base) / window;
 }
 
-__device__ __forceinline__ void ck_rb_put_header(u8* __restrict__ f, unsigned long long total, u32 n, long long base_offset, long long ts) {
+__device__ __forceinline__ void ck_rb_put_header(u8* __restrict__ f, unsigned long long total, u32 n, long long base_offset, long long ts,
+                                                 const ck_producer& prod) {
     ck_put_be64(f, (unsigned long long)base_offset);
     ck_put_be32(f + 8, (u32)(total - 12));
     ck_put_be32(f + 12, 0);                                  // partitionLeaderEpoch
     f[16] = 2;
     ck_put_be32(f + 17, 0);                                  // crc: folded in last
-    f[21] = 0; f[22] = 0;                                    // attributes: no compression, CreateTime
+    f[21] = 0; f[22] = (u8)prod.attr;                        // attributes: no compression, CreateTime, transactional or not
     ck_put_be32(f + 23, n - 1);                              // lastOffsetDelta
     ck_put_be64(f + 27, (unsigned long long)ts);
     ck_put_be64(f + 35, (unsigned long long)ts);
-    ck_put_be64(f + 43, ~0ull);                              // producerId -1
-    f[51] = 0xff; f[52] = 0xff;                              // producerEpoch -1
+    ck_put_be64(f + 43, (unsigned long long)prod.pid);       // producerId (-1: none)
+    f[51] = (u8)(prod.epoch >> 8); f[52] = (u8)prod.epoch;   // producerEpoch (-1: none)
     ck_put_be32(f + 53, 0xffffffffu);                        // baseSequence -1
     ck_put_be32(f + 57, n);
 }
@@ -527,7 +537,7 @@ __device__ __forceinline__ void ck_rb_put_header(u8* __restrict__ f, unsigned lo
 __global__ void __launch_bounds__(256)
 ck_fr_table_kernel(const u32* __restrict__ order, const ck_fitem* __restrict__ items, const u32* __restrict__ ffirst,
                    const long long* __restrict__ F, const long long* __restrict__ R, u32 n, const u32* __restrict__ n_live,
-                   long long base_offset, long long ts, unsigned long long cap, ck_frame_ent* __restrict__ table, u8* __restrict__ frames,
+                   long long base_offset, long long ts, ck_producer prod, unsigned long long cap, ck_frame_ent* __restrict__ table, u8* __restrict__ frames,
                    u32* __restrict__ chunks) {
     u32 f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n) return;
@@ -541,7 +551,7 @@ ck_fr_table_kernel(const u32* __restrict__ order, const ck_fitem* __restrict__ i
     table[f] = e;
     bool fits = (unsigned long long)(e.offset + e.length) <= cap;
     chunks[f] = fits ? (u32)((e.length - CK_RB_CRC_FROM + CK_RB_CRC_CHUNK - 1) / CK_RB_CRC_CHUNK) : 0u;
-    if (fits) ck_rb_put_header(frames + e.offset, (unsigned long long)e.length, b - a, base_offset, ts);
+    if (fits) ck_rb_put_header(frames + e.offset, (unsigned long long)e.length, b - a, base_offset, ts, prod);
 }
 
 // key / header value: JSON string content written unescaped (warp copy when it holds no escape)
@@ -708,7 +718,8 @@ ck_lz_gather_kernel(const ck_frame_ent* __restrict__ table, const long long* __r
         ck_warp_copy(d + 4, (stored ? raw : slots) + at, z, lane);
     }
 }
-// thread per frame: batch header (attributes 3, batchLength of the compressed frame), LZ4 frame header and end mark; the
+// thread per frame: batch header (codec 3, batchLength of the compressed frame; producer fields as the uncompressed frame
+// has them), LZ4 frame header and end mark; the
 // table entry moves to the compressed frame; CRC chunk count as ck_fr_table_kernel gives it (0: not written)
 __global__ void __launch_bounds__(256)
 ck_lz_head_kernel(ck_frame_ent* __restrict__ table, const long long* __restrict__ F, u32 n, const long long* __restrict__ Z,
@@ -727,7 +738,7 @@ ck_lz_head_kernel(ck_frame_ent* __restrict__ table, const long long* __restrict_
 #pragma unroll 1
         for (u32 i = 0; i < CK_RB_HEADER; i++) d[i] = s[i];
         ck_put_be32(d + 8, len - 12u);
-        d[22] = 3;                                           // attributes: LZ4, CreateTime
+        d[22] = s[22] | CK_RB_LZ4;                           // attributes: LZ4, CreateTime, the transactional bit kept
         ck_put_be32(d + CK_RB_HEADER, 0x04224D18u);          // magic 0x184D2204, little-endian
         d[CK_RB_HEADER + 4] = 0x60; d[CK_RB_HEADER + 5] = 0x40; d[CK_RB_HEADER + 6] = 0x82;   // FLG, BD, HC
         ck_put_be32(d + len - 4, 0u);

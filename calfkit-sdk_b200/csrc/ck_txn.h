@@ -60,6 +60,34 @@ static inline uint32_t ck_txn_crc32c(const uint8_t* p, uint64_t n) {
     return ~c;
 }
 
+// a(x) * b(x) mod P(x) over GF(2), CRC32C's reflected representation (bit 31 = x^0)
+static inline uint32_t ck_txn_gf_mul(uint32_t a, uint32_t b) {
+    uint32_t p = 0;
+    for (uint32_t m = 0x80000000u; m; m >>= 1) {
+        if (a & m) p ^= b;
+        b = (b & 1u) ? (b >> 1) ^ 0x82F63B78u : b >> 1;
+    }
+    return p;
+}
+
+// The CRC32C of a span of len bytes whose CRC was crc, after its 4 bytes at pos changed from old4 to new4.  The CRC is
+// affine in the message, so the change adds the CRC (zero init, no final xor) of the message that is zero but for
+// old4 ^ new4 at pos.  Leading zeros do not move that CRC and each trailing zero byte multiplies it by x^8, so it is the
+// CRC of the 4 delta bytes times x^(8 (len - pos - 4)) mod P: O(log len), whatever the span's length
+static inline uint32_t ck_txn_crc32c_patch(uint32_t crc, uint64_t len, uint64_t pos, const uint8_t* old4, const uint8_t* new4) {
+    uint32_t d = 0;                                             // raw CRC of the 4 delta bytes
+    for (int i = 0; i < 4; i++) {
+        d ^= (uint8_t)(old4[i] ^ new4[i]);
+        for (int k = 0; k < 8; k++) d = (d >> 1) ^ ((d & 1u) ? 0x82F63B78u : 0u);
+    }
+    uint32_t p = 0x80000000u, sq = 0x00800000u;                 // x^0, x^8
+    for (uint64_t n = len - pos - 4; n; n >>= 1) {
+        if (n & 1u) p = ck_txn_gf_mul(sq, p);
+        sq = ck_txn_gf_mul(sq, sq);
+    }
+    return crc ^ ck_txn_gf_mul(p, d);
+}
+
 // the checks the device makes of every batch: magic 2, codec none / gzip / snappy / LZ4 / zstd, and (check_crc) the CRC32C
 static inline bool ck_txn_framed(const uint8_t* f, uint64_t flen, bool check_crc) {
     uint32_t codec = f[22] & 7u;
@@ -92,6 +120,32 @@ static inline int ck_txn_control(const uint8_t* f, uint64_t flen, int* type) {
     if (version < 0) return CK_TXN_BAD;
     *type = (int16_t)((f[pos + 2] << 8) | f[pos + 3]);
     return CK_TXN_HIDE;
+}
+
+// The control batch the broker appends when producer (pid, epoch) ends its transaction on a partition: type CK_TXN_ABORT
+// or 1 (COMMIT), attributes transactional | control, baseSequence -1, one record of offsetDelta 0 whose key is (version 0,
+// type) and whose value is (version 0, coordinatorEpoch 0), no headers.  CK_TXN_CONTROL_LEN bytes into out; ck_txn_control
+// accepts it
+#define CK_TXN_CONTROL_LEN 78u
+static inline void ck_txn_put_be(uint8_t* p, uint64_t v, int n) { for (int i = n - 1; i >= 0; i--, v >>= 8) p[i] = (uint8_t)v; }
+static inline void ck_txn_control_batch(uint8_t* out, int64_t base_offset, int64_t timestamp_ms, int64_t pid, int16_t epoch, int16_t type) {
+    static const uint8_t rec[17] = {32, 0, 0, 0, 8, 0, 0, 0, 0, 12, 0, 0, 0, 0, 0, 0, 0};   // 16-byte body (varint 32)
+    uint8_t* f = out;
+    ck_txn_put_be(f, (uint64_t)base_offset, 8);
+    ck_txn_put_be(f + 8, CK_TXN_CONTROL_LEN - 12, 4);          // batchLength
+    ck_txn_put_be(f + 12, 0, 4);                                // partitionLeaderEpoch
+    f[16] = 2;
+    ck_txn_put_be(f + 21, CK_TXN_TRANSACTIONAL | CK_TXN_CONTROL, 2);
+    ck_txn_put_be(f + 23, 0, 4);                                // lastOffsetDelta
+    ck_txn_put_be(f + 27, (uint64_t)timestamp_ms, 8);
+    ck_txn_put_be(f + 35, (uint64_t)timestamp_ms, 8);
+    ck_txn_put_be(f + 43, (uint64_t)pid, 8);
+    ck_txn_put_be(f + 51, (uint16_t)epoch, 2);
+    ck_txn_put_be(f + 53, 0xffffffffu, 4);                      // baseSequence -1
+    ck_txn_put_be(f + 57, 1, 4);
+    for (int i = 0; i < 17; i++) f[61 + i] = rec[i];
+    ck_txn_put_be(f + 61 + 7, (uint16_t)type, 2);               // key: version 0 (bytes 5, 6), type
+    ck_txn_put_be(f + 17, ck_txn_crc32c(f + 21, CK_TXN_CONTROL_LEN - 21), 4);
 }
 
 // The read_committed mask of a whole record set buf[0..n): mask[b] = 1 for each complete batch b the rule above skips

@@ -39,7 +39,8 @@ typedef struct {           /* one publish; mirrors struct ck_pub in csrc/ck_kern
 
 typedef struct {           /* one frame of a frame pass; mirrors struct ck_frame_ent in csrc/ck_kafka.cuh */
     int32_t  topic_id;     /* registered topic id */
-    int32_t  partition;    /* -1: unkeyed records (the handler-return publish, worker/worker.py:52-53): the producer picks */
+    int32_t  partition;    /* -1: unkeyed records (the handler-return publish, worker/worker.py:52-53): the producer picks;
+                              with a sticky partition set for the topic (ck_set_sticky_partitions) they are in that one */
     uint32_t n_records;
     uint32_t first;        /* first record, counted in group order */
     int64_t  offset;       /* into the frame bytes */
@@ -179,6 +180,34 @@ int  ck_encode_frames_records(ck_handle* h, int32_t topic_id, const uint8_t* hos
                               uint32_t n, int64_t timestamp_ms);
 int  ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes);
 int  ck_fetch_frames_async(ck_handle* h, ck_frame* host_table, uint32_t table_cap, uint8_t* host_frames, uint64_t cap);
+
+/* Idempotent and transactional produce (KIP-98; the Java producer's enable.idempotence and transactional.id).
+ *   ck_set_producer           the producer fields of the frames the following passes build (ck_encode_frames,
+ *                             ck_encode_frames_records, ck_encode_recordbatch; LZ4 frames too).  flags 0 (the default):
+ *                             producerId -1, producerEpoch -1, attributes bit 4 clear.  CK_PRODUCER_IDEMPOTENT: pid and epoch
+ *                             (both >= 0); | CK_PRODUCER_TRANSACTIONAL: and attributes bit 4 on every frame.  baseSequence
+ *                             stays -1: frames of different passes and handles reach a partition in an order only the host
+ *                             knows, so the host writes each frame's baseSequence when it hands the frame out and patches the
+ *                             CRC32C with ck_crc32c_patch.  A pass takes the fields when it is queued; the rewrite
+ *                             ck_frames_size makes into a grown buffer writes the same headers.
+ *   ck_set_sticky_partitions  parts[topic id] (ids < n) the partition the topic's unkeyed publishes join in the following
+ *                             passes, -1 none (n = 0: none at all, the default).  The unkeyed publishes are then grouped,
+ *                             split and written with that partition's keyed ones, as if they had that partition (Kafka's
+ *                             uniform sticky partitioner; an idempotent sequence exists only per partition).  Each entry is
+ *                             -1 or in [0, num_partitions).
+ *   ck_crc32c_patch           *crc = the CRC32C of a span of len bytes whose CRC32C was *crc, after its 4 bytes at pos changed
+ *                             from old4 to new4: O(log len), no handle, no device.  For a frame: span = [21, length), the
+ *                             baseSequence at 53 - 21 = 32 of it.
+ *   ck_encode_control_batch   the transaction marker the broker appends to a partition when producer (producer_id,
+ *                             producer_epoch) commits (type 1) or aborts (type 0): a 78-byte control batch (attributes 0x30,
+ *                             baseSequence -1, one record: key version 0 and type, value version 0 and coordinatorEpoch 0),
+ *                             CRC32C included, into out (cap >= 78); no handle, no device */
+enum { CK_PRODUCER_IDEMPOTENT = 1, CK_PRODUCER_TRANSACTIONAL = 2 };
+int  ck_set_producer(ck_handle* h, int64_t pid, int16_t epoch, uint32_t flags);
+int  ck_set_sticky_partitions(ck_handle* h, const int32_t* parts, uint32_t n);
+int  ck_crc32c_patch(uint32_t* crc, uint64_t len, uint64_t pos, const uint8_t* old4, const uint8_t* new4);
+int  ck_encode_control_batch(int64_t base_offset, int64_t timestamp_ms, int64_t producer_id, int16_t producer_epoch, int16_t type,
+                             uint8_t* out, uint64_t cap, uint64_t* len);
 
 /* tool node, host tools only: gather every record's tool-call `args` JSON into the output buffer
  * (payload i = args of record i, empty when the record does not reach the tool). */
