@@ -19,9 +19,10 @@ Kafka's own granularity — record batches — at both ends:
   * `produce_fetch(topic, buf)` enqueues a fetch response's record set (engine.lane.FetchArena); `poll_arena` (device-template
     nodes) and `poll_fetch` (Agent nodes, Python-tool nodes, the client's replies) split such entries only at frame boundaries,
     and the device checks, splits and decodes them.  Transactions (KIP-98): a record set
-    holds the batches of one or more partitions back to back, `partitions=[(byte start, aborted), ...]` in byte order,
-    where `aborted` is that partition's AbortedTransactions from the fetch response, [(producer id, first offset), ...];
-    `aborted_transactions=aborted` alone is the one-partition case.  Control batches are skipped at every isolation level;
+    holds the batches of one or more partitions back to back, `partitions=[(byte start, aborted, partition id), ...]` in
+    byte order, where `aborted` is that partition's AbortedTransactions from the fetch response, [(producer id, first
+    offset), ...] (without an id, an entry is the partition of its place in the list); `aborted_transactions=aborted`
+    alone is the one-partition case, partition 0.  Control batches are skipped at every isolation level;
     a consumer at isolation_level="read_committed" also skips the aborted transactions' batches.  The mask of those is
     computed once over the whole entry (an aborted producer stays aborted across a split) and sliced with it;
   * `frame_sink(topic, fn)`: `fn(topic, partition_or_None, frame, n_records)` once per produce-ready RecordBatch v2 frame.
@@ -38,6 +39,14 @@ engine built them.  A topic's unkeyed publishes go to one sticky partition per f
 robin, so every frame has a partition.  With a transactional id, each Worker.run tick is one transaction: data frames
 carry attributes bit 4, and when the tick ends every (topic, partition) that received frames in it gets a COMMIT marker
 (a control batch) through the same sink, or an ABORT marker when the tick raised.
+Exactly-once consume-transform-produce (KIP-447, Kafka Streams' processing.guarantee="exactly_once_v2"): committed
+offsets are kept per (consumer group, topic, partition).  `send_offsets_to_transaction(offsets, group_id)` adds a group's
+consumed positions to the open transaction; they become `committed(...)` at commit_transaction and are dropped at
+abort_transaction.  A fetch slice that `poll_fetch` / `poll_arena` hand out with a `group_id` (only inside an open
+transaction) is kept, its buffer not released, until a commit covers every partition it holds (FetchArena.positions);
+an abort puts the slices no commit covers back at the head of their topic's queue, in poll order, without the batches
+already covered, and with their read_committed mask, so that the next poll delivers them again.  Fetches are the only
+input with offsets: a poll with a group_id refuses Records and arenas, before it takes any.
 Publishes to topics nobody subscribes to are counted and dropped when they arrive batch-wise (a long-running worker must
 not grow without bound); per-record publishes are kept (tests read such topics afterwards).
 Limitation (documented, not hidden): one shared queue per topic — consumer GROUPS are not modelled (two subscriptions to
@@ -100,6 +109,9 @@ class MemoryBroker:
         self._seq: dict[tuple[int, str, int], int] = {}               # (producer id, topic, partition) -> next baseSequence
         self._sticky: dict[str, int] = {}                             # topic -> sticky partition of the next pass
         self._txn: dict[tuple[str, int], tuple[int, int]] | None = None   # open transaction: (topic, partition) -> (pid, epoch)
+        self._committed: dict[tuple[str, str, int], int] = {}          # (group, topic, partition) -> committed offset
+        self._txn_offsets: dict[tuple[str, str, int], int] = {}        # the offsets sent to the open transaction
+        self._kept: dict[str, list] = defaultdict(list)               # topic -> [(group, FetchArena, release)] in poll order
         self._connection: Any = None
         self.queues: dict[str, deque[Record]] = defaultdict(deque)
         self.arenas: dict[str, deque] = defaultdict(deque)            # topic -> deque[Arena]
@@ -164,6 +176,10 @@ class MemoryBroker:
         else:
             self.queues[rec.topic].append(rec)
         self.produced += 1
+
+    def discard_frames(self) -> None:
+        """drop the Records collected for frame-sink topics and not framed yet (the outputs of a step being undone)"""
+        self._frame_pending.clear()
 
     def flush_frames(self) -> None:
         """frame the per-record Records collected for frame-sink topics (engine record form) and hand the frames out"""
@@ -251,9 +267,72 @@ class MemoryBroker:
         if self._txn is None:
             raise EngineError("no transaction is open")
         touched, self._txn = self._txn, None
+        offsets, self._txn_offsets = self._txn_offsets, {}
         ts = int(time.time() * 1000)
         for (topic, part), (pid, epoch) in touched.items():
             self.frame_sinks[topic](topic, part, control_batch(pid, epoch, commit, ts), 1)
+        if commit:
+            self._committed.update(offsets)
+            self._release_covered()
+        else:
+            self._rewind()
+
+    # --- exactly-once: consumed offsets in the transaction ----------------------------------------------
+    def send_offsets_to_transaction(self, offsets: dict[tuple[str, int], int], group_id: str) -> None:
+        """consumer group `group_id`'s next offsets {(topic, partition): offset} (Kafka's sendOffsetsToTransaction): they
+        are committed with the open transaction, or dropped when it aborts"""
+        from calfkit.exceptions import EngineError
+        if self._txn is None:
+            raise EngineError("send_offsets_to_transaction outside a transaction (begin_transaction first)")
+        for (topic, part), off in offsets.items():
+            self._txn_offsets[(group_id, topic, int(part))] = int(off)
+
+    def committed(self, group_id: str, topic: str, partition: int) -> int | None:
+        """the offset consumer group `group_id` resumes (topic, partition) from, None when it never committed one"""
+        return self._committed.get((group_id, topic, int(partition)))
+
+    def _check_keep(self, group_id: str | None, topics) -> None:
+        """a poll for a group's offsets is refused, before anything is taken, outside a transaction"""
+        if group_id is not None and self._txn is None:
+            from calfkit.exceptions import EngineError
+            raise EngineError(f"a poll of {tuple(topics)} for group {group_id!r}'s offsets outside a transaction (begin_transaction first)")
+
+    def _keep(self, topic: str, group_id: str, fetch):
+        """hold `fetch`, polled for `group_id`, until a commit covers it; its consumer's release no longer frees the buffer"""
+        self._kept[topic].append((group_id, fetch, fetch._on_release))
+        fetch._on_release = None
+        return fetch
+
+    def _covered(self, group_id: str, topic: str, fetch) -> bool:
+        return all(self._committed.get((group_id, topic, p), -1) >= nxt for p, nxt in fetch.positions().items())
+
+    def _release_covered(self) -> None:
+        """release the kept slices the committed offsets cover, from the oldest on: a fetch's buffer is released by its last
+        slice, so none is released before a slice polled earlier"""
+        for topic, kept in self._kept.items():
+            while kept and self._covered(kept[0][0], topic, kept[0][1]):
+                _g, _f, release = kept.pop(0)
+                if release is not None:
+                    release()
+
+    def _rewind(self) -> None:
+        """after an abort: the kept slices back at the head of their topics' queues, in poll order, less what is committed"""
+        for topic, kept in self._kept.items():
+            back, releases = [], []
+            for group, fetch, release in kept:
+                rest = fetch.without_consumed({p: o for (g, t, p), o in self._committed.items() if g == group and t == topic})
+                if rest is None:
+                    releases.append(release)
+                else:
+                    rest._on_release = release
+                    back.append(rest)
+            if back:                                        # a dropped slice's buffer may hold a later slice: freed with the last one
+                releases.append(back[-1]._on_release)
+                back[-1]._on_release = _chain(releases)
+            else:
+                _chain(releases)()
+            self.arenas[topic].extendleft(reversed(back))
+        self._kept.clear()
 
     def produce_batch(self, records: list[Record]) -> None:
         for r in records:
@@ -267,6 +346,7 @@ class MemoryBroker:
             from calfkit.exceptions import EngineError
             raise EngineError("a FetchArena carries its own partitions: give them to FetchArena.of")
         fa = buf if isinstance(buf, FetchArena) else FetchArena.of(buf, aborted_transactions=aborted_transactions, partitions=partitions)
+        fa.topic = topic
         self.arenas[topic].append(fa)
         self.produced += fa.n
 
@@ -322,8 +402,14 @@ class MemoryBroker:
             self.dropped_unsubscribed += len(idx)
 
     # --- consume side -------------------------------------------------------------------------------
-    def poll_batch(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None) -> list[Record]:
-        """per-record consume, bounded by records and (optionally) bytes; batch-wise entries are materialised as Records"""
+    def poll_batch(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None,
+                   group_id: str | None = None) -> list[Record]:
+        """per-record consume, bounded by records and (optionally) bytes; batch-wise entries are materialised as Records.
+        With a group_id (a consumer that commits offsets) any such input is refused: records have no offsets"""
+        if group_id is not None:
+            for t in topics:
+                if self.queues.get(t) or self.arenas.get(t) or self.frags.get(t):
+                    _no_offsets(t)
         out: list[Record] = []
         nbytes = 0
         for t in topics:
@@ -346,25 +432,32 @@ class MemoryBroker:
                     arena.release()
         return out
 
-    def poll_fetch(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None):
+    def poll_fetch(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None, group_id: str | None = None):
         """the next fetch response (engine.lane.FetchArena) of the first of these topics whose next entry is one, split
         at frame boundaries under the same bounds as poll_arena (None when none is): what a consumer that decodes fetches
-        on the device (a node's engine, the client's replies) takes before it asks poll_batch for Records"""
+        on the device (a node's engine, the client's replies) takes before it asks poll_batch for Records.  With a
+        group_id (inside a transaction only) the slice is kept until a commit of that group's offsets covers it"""
+        self._check_keep(group_id, topics)
         for t in topics:
             head = _take_fetch(self.arenas.get(t), max_records, max_bytes)
             if head is not None:
-                return head
+                return head if group_id is None else self._keep(t, group_id, head)
         return None
 
-    def poll_arena(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None, records_too: bool = True):
+    def poll_arena(self, topics: tuple[str, ...], max_records: int, max_bytes: int | None = None, records_too: bool = True,
+                   group_id: str | None = None):
         """the next batch for these topics as one contiguous Arena (None when idle).  Never returns more than max_records
-        records or max_bytes bytes (one oversized record is still returned alone: the engine reports it per record)."""
+        records or max_bytes bytes (one oversized record is still returned alone: the engine reports it per record).  A
+        fetch slice polled with a group_id is kept as poll_fetch keeps it"""
         from calfkit.engine.lane import Arena
+        self._check_keep(group_id, topics)
         for t in topics:
             q = self.arenas.get(t)
             head = _take_fetch(q, max_records, max_bytes)
             if head is not None:
-                return head
+                return head if group_id is None else self._keep(t, group_id, head)
+            if group_id is not None and (q or self.frags.get(t) or (records_too and self.queues.get(t))):
+                _no_offsets(t)
             if q:
                 a = q[0]
                 k = _fit(a.offsets, max_records, max_bytes)
@@ -420,6 +513,22 @@ def _take_fetch(q: deque | None, max_records: int, max_bytes: int | None):
     rest._on_release, a._on_release = a._on_release, None
     q[0] = rest
     return head
+
+
+def _no_offsets(topic: str) -> None:
+    from calfkit.exceptions import EngineError
+    raise EngineError(f"topic {topic!r} holds records without offsets (Records or arenas): a consumer that commits its "
+                      "offsets (exactly-once) consumes fetch responses only")
+
+
+def _chain(fns):
+    """one callable that calls the non-None callables of fns in order"""
+    fns = [f for f in fns if f is not None]
+
+    def call() -> None:
+        for f in fns:
+            f()
+    return call
 
 
 def _fit(offsets, max_records: int, max_bytes: int | None) -> int:

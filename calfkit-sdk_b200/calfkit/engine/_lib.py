@@ -47,7 +47,7 @@ EXPORTS = ["ck_create", "ck_destroy", "ck_last_error", "ck_version", "ck_registe
            "ck_fetch_rb_index", "ck_encode_recordbatch", "ck_group_publishes", "ck_fetch_groups", "ck_comm_create", "ck_comm_connect", "ck_exchange_send", "ck_recv_info", "ck_fetch_received", "ck_peek_received", "ck_fetch_received_async", "ck_set_option",
            "ck_set_frame_topics", "ck_encode_frames", "ck_encode_frames_records", "ck_frames_size", "ck_fetch_frames_async",
            "ck_fetch_rb_index_async", "ck_fetch_rb_decoded_async", "ck_set_fetch_hidden", "ck_fetch_txn_mask",
-           "ck_set_producer", "ck_set_sticky_partitions", "ck_crc32c_patch", "ck_encode_control_batch"]
+           "ck_set_producer", "ck_set_sticky_partitions", "ck_crc32c_patch", "ck_encode_control_batch", "ck_fetch_positions"]
 
 _lib = None
 
@@ -111,6 +111,7 @@ def load() -> C.CDLL:
         "ck_fetch_rb_decoded_async": (C.c_int, [vp, u8p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
         "ck_set_fetch_hidden": (C.c_int, [vp, u8p, C.c_uint32]),
         "ck_fetch_txn_mask": (C.c_int, [u8p, C.c_uint64, vp, C.c_uint32, u32p, i64p, i64p, C.c_uint32, u8p, C.c_uint32, C.POINTER(C.c_uint32)]),
+        "ck_fetch_positions": (C.c_int, [u8p, C.c_uint64, vp, C.c_uint32, i64p, i64p, C.c_uint32, C.POINTER(C.c_uint32)]),
         "ck_set_producer": (C.c_int, [vp, C.c_int64, C.c_int16, C.c_uint32]),
         "ck_set_sticky_partitions": (C.c_int, [vp, i32p, C.c_uint32]),
         "ck_crc32c_patch": (C.c_int, [C.POINTER(C.c_uint32), C.c_uint64, C.c_uint64, u8p, u8p]),

@@ -28,30 +28,51 @@ FRAME_CODECS = {None: 0, "lz4": 3}
 ISOLATION_LEVELS = ("read_uncommitted", "read_committed")
 
 
-def txn_partitions(aborted_transactions=None, partitions=None) -> list[tuple[int, list[tuple[int, int]]]]:
+def txn_partitions(aborted_transactions=None, partitions=None) -> list[tuple[int, list[tuple[int, int]], int]]:
     """the partition model of a fetch response's record set: [(byte start of the partition's batches, its AbortedTransactions
-    [(producer id, first offset), ...]), ...] in byte order; `aborted_transactions` alone: one partition, the whole record set"""
+    [(producer id, first offset), ...], its partition id), ...] in byte order; `aborted_transactions` alone: one partition,
+    the whole record set, partition 0.  An entry given as (start, aborted) without an id is partition r, its place in
+    the list"""
     if aborted_transactions is not None and partitions is not None:
         raise EngineError("give aborted_transactions (one partition) or partitions, not both")
     if partitions is None:
         partitions = [(0, aborted_transactions or [])]
-    return [(int(start), [(int(pid), int(first)) for pid, first in ab]) for start, ab in partitions]
+    return [(int(e[0]), [(int(pid), int(first)) for pid, first in e[1]], int(e[2]) if len(e) > 2 else r)
+            for r, e in enumerate(partitions)]
 
 
 def fetch_txn_mask(buf: np.ndarray, partitions) -> np.ndarray:
     """per complete batch of the record set `buf`: 1 where a read_committed consumer skips it, a transactional batch of an
     aborted producer (ck_fetch_txn_mask; control batches are skipped by the engine itself)"""
     lib = _lib.load()
-    starts = np.asarray([s for s, _ab in partitions], dtype=np.uint64)
-    runs = np.asarray([r for r, (_s, ab) in enumerate(partitions) for _e in ab], dtype=np.uint32)
-    pids = np.asarray([pid for _s, ab in partitions for pid, _f in ab], dtype=np.int64)
-    firsts = np.asarray([first for _s, ab in partitions for _p, first in ab], dtype=np.int64)
+    starts = np.asarray([e[0] for e in partitions], dtype=np.uint64)
+    runs = np.asarray([r for r, e in enumerate(partitions) for _e in e[1]], dtype=np.uint32)
+    pids = np.asarray([pid for e in partitions for pid, _f in e[1]], dtype=np.int64)
+    firsts = np.asarray([first for e in partitions for _p, first in e[1]], dtype=np.int64)
     cap = buf.nbytes // 61 + 1
     mask, nb = np.zeros(cap, dtype=np.uint8), C.c_uint32(0)
     if lib.ck_fetch_txn_mask(ptr(buf), buf.nbytes, ptr(starts), len(starts), ptr(runs), ptr(pids), ptr(firsts), len(runs),
                              ptr(mask), cap, C.byref(nb)):
         raise EngineError(lib.ck_last_error(None).decode())
     return mask[:nb.value]
+
+
+def fetch_positions(buf: np.ndarray, partitions) -> tuple[dict[int, int], np.ndarray]:
+    """where a consumer of the record set `buf` (a fetch, or a slice of one with its partition model) resumes: ({partition
+    id: lastOffset + 1 of its last complete batch} for every partition a complete batch of buf belongs to, lastOffset + 1
+    of each complete batch).  Every batch counts, delivered, skipped or bad (ck_fetch_positions reads only the headers)"""
+    lib = _lib.load()
+    starts = np.asarray([e[0] for e in partitions], dtype=np.uint64)
+    nxt = np.empty(len(starts), dtype=np.int64)
+    cap = buf.nbytes // 61 + 1
+    per_batch, nb = np.empty(cap, dtype=np.int64), C.c_uint32(0)
+    if lib.ck_fetch_positions(ptr(buf), buf.nbytes, ptr(starts), len(starts), ptr(nxt), ptr(per_batch), cap, C.byref(nb)):
+        raise EngineError(lib.ck_last_error(None).decode())
+    out = {}
+    for e, x in zip(partitions, nxt.tolist()):
+        if x >= 0:
+            out[e[2]] = x
+    return out, per_batch[:nb.value]
 
 
 @dataclass
@@ -432,7 +453,7 @@ class BatchEngine:
         `aborted_transactions` [(producer id, first offset), ...] of a one-partition record set or `partitions` (txn_partitions)"""
         assert buf.dtype == np.uint8
         parts = txn_partitions(aborted_transactions, partitions)
-        if self.read_committed and any(ab for _s, ab in parts):
+        if self.read_committed and any(e[1] for e in parts):
             self.set_fetch_hidden(fetch_txn_mask(buf, parts))
         n = C.c_uint32(0)
         self._check(self.lib.ck_submit_recordbatch(self.h, ptr(buf), buf.nbytes, C.byref(n)))

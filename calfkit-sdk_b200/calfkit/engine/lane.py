@@ -26,7 +26,7 @@ import numpy as np
 
 from calfkit.engine import _lib
 from calfkit.engine._lib import COL, FRAME_DTYPE, PUB_DTYPE, ptr
-from calfkit.engine.batch import BatchEngine, FetchBytes, Frames, ToolTemplate, _SpanOffsets, fetch_txn_mask, txn_partitions
+from calfkit.engine.batch import BatchEngine, FetchBytes, Frames, ToolTemplate, _SpanOffsets, fetch_positions, fetch_txn_mask, txn_partitions
 from calfkit.exceptions import EngineError
 
 NO_PAYLOAD = 0xFFFFFFFF
@@ -130,18 +130,22 @@ class FetchArena:
     """the record set of one fetch response — concatenated RecordBatch v2 frames as they came off the socket — in one
     buffer.  The host only chains through the 12-byte frame prefixes (baseOffset, batchLength) to count frames and records;
     a truncated trailing frame (legal in a fetch response) is carried along and ignored by the device.
-    `partitions` (engine.batch.txn_partitions): where each partition's batches start and its AbortedTransactions, from
-    which hidden() gives the read_committed mask; a slice carries its part of the mask instead"""
+    `partitions` (engine.batch.txn_partitions): where each partition's batches start, its AbortedTransactions, from
+    which hidden() gives the read_committed mask, and its partition id, from which positions() gives the offsets a
+    consumer resumes from; a slice carries its part of the mask and its partitions rebased to its own bytes.  `topic`:
+    the topic the broker queued it on (None: not queued)"""
     def __init__(self, data: np.ndarray, on_release: Callable[[], None] | None = None, partitions=None,
-                 hidden: np.ndarray | None = None):
+                 hidden: np.ndarray | None = None, topic: str | None = None):
         assert data.dtype == np.uint8
         self.data, self._on_release, self._index = data, on_release, None
-        self.partitions, self._hidden = partitions, hidden
+        self.partitions, self._hidden, self.topic = partitions, hidden, topic
+        self._positions = None
 
     @classmethod
     def of(cls, buf, pool: PinnedPool | None = None, aborted_transactions=None, partitions=None) -> "FetchArena":
         """land a fetch response (bytes / uint8 array) in a page-locked buffer; aborted_transactions [(producer id, first
-        offset), ...] of its one partition, or partitions [(byte start, [(producer id, first offset), ...]), ...]"""
+        offset), ...] of its one partition (partition 0), or partitions [(byte start, [(producer id, first offset), ...],
+        partition id), ...] (without the id: the entry's place in the list)"""
         parts = txn_partitions(aborted_transactions, partitions)
         src = np.frombuffer(bytes(buf), dtype=np.uint8) if not isinstance(buf, np.ndarray) else buf
         if pool is None:
@@ -153,9 +157,48 @@ class FetchArena:
     def hidden(self) -> np.ndarray | None:
         """per complete frame, 1 where a read_committed consumer skips it; computed once over the whole fetch, since the
         aborted producers carry from batch to batch across any split.  None: the fetch names no aborted transaction"""
-        if self._hidden is None and self.partitions and any(ab for _s, ab in self.partitions):
+        if self._hidden is None and self.partitions and any(e[1] for e in self.partitions):
             self._hidden = fetch_txn_mask(self.data, self.partitions)
         return self._hidden
+
+    def positions(self) -> dict[int, int]:
+        """{partition id: the offset after its last complete batch here} (engine.batch.fetch_positions): what a consumer
+        that has handed out this arena's results commits.  {} without a partition model"""
+        return self._batch_positions()[0]
+
+    def _batch_positions(self) -> tuple[dict[int, int], np.ndarray, np.ndarray]:
+        """(positions(), per complete frame its partition id and the offset after it)"""
+        if self._positions is None:
+            starts = self.frames()[0][:-1]
+            if not self.partitions:
+                self._positions = ({}, np.full(len(starts), -1, np.int64), np.full(len(starts), -1, np.int64))
+            else:
+                pos, nxt = fetch_positions(self.data, self.partitions)
+                run = np.searchsorted(np.asarray([e[0] for e in self.partitions], dtype=np.int64), starts, side="right") - 1
+                ids = np.asarray([e[2] for e in self.partitions] + [-1], dtype=np.int64)[run]   # run -1: before the first start
+                self._positions = (pos, ids, nxt)
+        return self._positions
+
+    def without_consumed(self, committed: dict[int, int]) -> "FetchArena | None":
+        """this arena without its frames that offsets `committed` ({partition id: committed offset}) already cover, the
+        read_committed mask and the topic kept: a zero-copy slice when what stays is one run of frames, else a copy.  None
+        when nothing stays.  The release stays with this arena"""
+        _pos, ids, nxt = self._batch_positions()
+        keep = np.asarray([nx < 0 or nx > committed.get(int(p), -1) for p, nx in zip(ids.tolist(), nxt.tolist())], dtype=bool)
+        if not keep.any():
+            return None
+        k = np.nonzero(keep)[0]
+        a, b = int(k[0]), int(k[-1]) + 1
+        if b - a == len(k):
+            return self.slice_frames(a, b if b < len(keep) else None)
+        starts, hidden = self.frames()[0], self.hidden()
+        pieces = [self.data[int(starts[i]):int(starts[i + 1])] for i in k]
+        parts, at = [], 0
+        for i, piece in zip(k.tolist(), pieces):
+            if not parts or parts[-1][2] != int(ids[i]):
+                parts.append((at, [], int(ids[i])))
+            at += piece.nbytes
+        return FetchArena(np.concatenate(pieces), partitions=parts, hidden=None if hidden is None else hidden[k], topic=self.topic)
 
     def frames(self) -> tuple[np.ndarray, np.ndarray]:
         """(starts[k + 1], records[k]) of the k complete frames; starts[k] is where the truncated tail (if any) begins"""
@@ -183,8 +226,12 @@ class FetchArena:
     def slice_frames(self, a: int, b: int | None) -> "FetchArena":
         """frames [a, b) as a zero-copy view; b None: to the end of the buffer (the truncated tail included)"""
         starts, hidden = self.frames()[0], self.hidden()
-        return FetchArena(self.data[int(starts[a]):(int(starts[b]) if b is not None else self.data.nbytes)],
-                          hidden=None if hidden is None else hidden[a:b])
+        lo, hi = int(starts[a]), (int(starts[b]) if b is not None else self.data.nbytes)
+        parts = None
+        if self.partitions:                 # rebased to the slice: the partition it starts in at 0, those after it shifted
+            first = max((r for r, e in enumerate(self.partitions) if e[0] <= lo), default=0)
+            parts = [(max(e[0] - lo, 0), [], e[2]) for e in self.partitions[first:] if e[0] < hi]
+        return FetchArena(self.data[lo:hi], hidden=None if hidden is None else hidden[a:b], partitions=parts, topic=self.topic)
 
     def release(self) -> None:
         if self._on_release is not None:

@@ -20,6 +20,16 @@ A broker with enable_idempotence or a transactional_id (frame sinks only) gives 
 (MemoryBroker.init_producer_id) when it builds its first engine that frames; every lane engine and the framer engine write
 them into their frames, and each frame pass takes the broker's next sticky partitions for the unkeyed publishes.  With a
 transactional_id, each tick of run() is one transaction: committed when the tick ends, aborted when it raises.
+
+Worker(..., processing_guarantee="exactly_once_v2") makes a transactional Worker exactly-once for the fetches it consumes
+(Kafka Streams' guarantee of that name): every fetch slice is polled for its subscription's consumer group and kept by
+the broker; when a step's results are handed out (a lane's results come back, a host node returns) the slice's
+positions (FetchArena.positions) become the group's handed-out offsets, and at the end of the tick they are sent to the
+tick's transaction (send_offsets_to_transaction) before it commits.  Input still in flight on a lane stays uncommitted:
+its outputs and its offsets go into the later transaction that hands them out.  When a tick raises, the results in
+flight are dropped, the transaction aborts, the broker puts the uncommitted slices back, and run() re-raises; a later
+run() consumes them again.  Only fetches carry offsets: under this guarantee a subscribed topic that holds Records or
+arenas makes the poll raise EngineError before anything is taken.
 """
 from __future__ import annotations
 
@@ -38,7 +48,7 @@ from calfkit.engine import BatchEngine
 from calfkit.engine.batch import FRAME_CODECS, ISOLATION_LEVELS
 from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_SKIPPED, CK_UNSUPPORTED, STATUS_NAMES
 from calfkit.exceptions import EngineError
-from calfkit.engine.lane import FetchArena, LanePipeline, PublishBatch
+from calfkit.engine.lane import FetchArena, FetchRecords, LanePipeline, PublishBatch
 from calfkit.nodes import BaseNodeDef
 
 logger = logging.getLogger(__name__)
@@ -68,12 +78,16 @@ def engine_for(node: BaseNodeDef, *, device: int = 0, max_records: int = 1 << 14
     return eng
 
 
+PROCESSING_GUARANTEES = ("at_least_once", "exactly_once_v2")
+
+
 class Worker:
     def __init__(self, client: Client, nodes: list[BaseNodeDef] | None = None, max_workers: int = 1,
                  group_id: str | None = None, extra_publish_kwargs: dict[str, Any] | None = None,
                  extra_subscribe_kwargs: dict[str, Any] | None = None, *, device: int | None = None,
                  batch_records: int = 1 << 14, batch_bytes: int = 64 << 20, lanes: int = 3,
-                 route_topics: list[str] | None = None, rank: int | None = None, world: int | None = None):
+                 route_topics: list[str] | None = None, rank: int | None = None, world: int | None = None,
+                 processing_guarantee: str = "at_least_once"):
         """Reference signature (worker/worker.py:13-31) plus keyword-only engine knobs: `device` (default: LOCAL_RANK of a
         one-process-per-GPU launch, else 0), the batch bounds a poll honours (records AND bytes: a batch never exceeds what
         the engines were sized for), the number of pipelined lanes per device-template node, and `route_topics`: names of
@@ -83,7 +97,15 @@ class Worker:
         partition (reference: consumer-group sharding, worker/worker.py:38,47, with every hop keyed by correlation_id,
         nodes/base.py:86,103,117,134).  A keyed publish whose partition (murmur2(key) % partitions) is owned by another rank
         (partition % world) is stored straight into that rank's receive buffer over NVLink and produced THERE; all ranks
-        tick in lockstep (an idle rank submits an empty batch) so that the per-step barriers of the exchange match."""
+        tick in lockstep (an idle rank submits an empty batch) so that the per-step barriers of the exchange match.
+        `processing_guarantee`: "at_least_once" (the default) or "exactly_once_v2", which needs a broker with a
+        transactional_id: each tick commits the consumed offsets of the results it hands out with the frames they made."""
+        if processing_guarantee not in PROCESSING_GUARANTEES:
+            raise EngineError(f"processing_guarantee {processing_guarantee!r}: expected one of {PROCESSING_GUARANTEES}")
+        if processing_guarantee == "exactly_once_v2" and getattr(client._connection, "transactional_id", None) is None:
+            raise EngineError("processing_guarantee='exactly_once_v2' needs a broker with a transactional_id")
+        self._exactly_once = processing_guarantee == "exactly_once_v2"
+        self._handed: dict[str, dict[tuple[str, int], int]] = {}   # group -> {(topic, partition): next offset} handed out this tick
         self._client = client
         self._nodes = nodes or list()
         self._max_workers = max_workers
@@ -109,6 +131,7 @@ class Worker:
         self._framer_eng: BatchEngine | None = None
         self._frame_pool = None
         self._levels: dict[int, str] = {}          # node -> its subscription's isolation_level
+        self._groups: dict[int, str] = {}          # node -> its subscription's consumer group
         self._producer: tuple[int, int] | None = None   # (producer id, epoch) of an idempotent broker, taken once
         self.stats = {"records": 0, "publishes": 0, "rejected": 0, "skipped": 0, "raises": 0, "host_fallback": 0, "steps": 0}
 
@@ -128,6 +151,7 @@ class Worker:
             if level not in ISOLATION_LEVELS:
                 raise EngineError(f"node {node.name}: isolation_level {level!r}, expected one of {ISOLATION_LEVELS}")
             self._levels[id(node)] = level
+            self._groups[id(node)] = group_id
             handler = subscriber(node.handler)
             if node.publish_topic:
                 self._client._connection.publisher(node.publish_topic, **self._extra_publish_kwargs)(handler)
@@ -161,6 +185,7 @@ class Worker:
 
     def _produce_fast(self, node: BaseNodeDef, batch: PublishBatch) -> None:
         broker = self._client._connection
+        self._hand_out(node, batch.source)
         n = batch.source.n
         if n == 0:
             batch.release()
@@ -217,6 +242,31 @@ class Worker:
                 self._run_host(node, records[:mid], **kw)
                 self._run_host(node, records[mid:], **kw)
 
+    def _hand_out(self, node: BaseNodeDef, source) -> None:
+        """exactly-once: the positions of a fetch slice whose results are being handed out become its group's offsets of
+        this tick"""
+        if not self._exactly_once:
+            return
+        arena = source.arena if isinstance(source, FetchRecords) else source
+        if isinstance(arena, FetchArena) and arena.topic is not None:
+            handed = self._handed.setdefault(self._groups[id(node)], {})
+            for part, nxt in arena.positions().items():
+                handed[(arena.topic, part)] = nxt
+
+    def _drop_in_flight(self, broker) -> None:
+        """exactly-once, a tick that raised: the results still on the lanes and the Records not yet framed belong to input
+        the abort gives back, so they are dropped, not produced"""
+        for pipe in self._pipes.values():
+            try:
+                for done in pipe.drain():
+                    done.release()
+                for rb in pipe.take_received():
+                    rb.release()
+            except Exception:  # noqa: BLE001  (the tick's own failure is what run() re-raises)
+                logger.exception("dropping the results in flight after a failed tick")
+        broker.discard_frames()
+        self._handed.clear()
+
     def _producer_of(self, broker) -> tuple[int, int, bool] | None:
         """(producer id, epoch, transactional) the engines that frame write into their frames; None: not idempotent"""
         if not getattr(broker, "enable_idempotence", False):
@@ -234,7 +284,12 @@ class Worker:
         broker.begin_transaction()
         try:
             yield
+            for group, offsets in self._handed.items():
+                broker.send_offsets_to_transaction(offsets, group)
+            self._handed.clear()
         except BaseException:
+            if self._exactly_once:
+                self._drop_in_flight(broker)
             broker.abort_transaction()
             raise
         broker.commit_transaction()
@@ -288,9 +343,10 @@ class Worker:
                 raise EngineError("frame sinks need world == 1: publishes forwarded by other ranks are not framed yet")
             broker.framer = self._frame_records
         for node, sub in self._subs:
+            group = {"group_id": sub.group_id} if self._exactly_once else {}   # exactly-once: the broker keeps the slice
             if getattr(node, "_template", None) is not None:
                 pipe = self._pipeline(node)
-                arena = broker.poll_arena(sub.topics, self._batch_records, self._batch_bytes)
+                arena = broker.poll_arena(sub.topics, self._batch_records, self._batch_bytes, **group)
                 if arena is None and self._world > 1:
                     arena = _EMPTY_ARENA()                     # lockstep: every rank runs the exchange on every tick
                 if arena is not None:
@@ -312,15 +368,16 @@ class Worker:
                     self.stats["received"] = self.stats.get("received", 0) + rb.n_publishes
                     broker.produce_publishes(rb)
                 continue
-            fetch = broker.poll_fetch(sub.topics, self._batch_records, self._batch_bytes)
+            fetch = broker.poll_fetch(sub.topics, self._batch_records, self._batch_bytes, **group)
             if fetch is not None:
                 consumed += fetch.n
                 try:
                     self._run_host(node, fetch)
+                    self._hand_out(node, fetch)
                 finally:
                     fetch.release()
                 continue
-            records: list[Record] = broker.poll_batch(sub.topics, self._batch_records, self._batch_bytes)
+            records: list[Record] = broker.poll_batch(sub.topics, self._batch_records, self._batch_bytes, **group)
             if not records:
                 continue
             consumed += len(records)

@@ -948,6 +948,16 @@ extern "C" int ck_fetch_txn_mask(const uint8_t* buf, uint64_t nbytes, const uint
     return 0;
 }
 
+// the consumed positions of a fetch or a slice of one (ck_txn_positions): no handle, no device
+extern "C" int ck_fetch_positions(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
+                                  int64_t* next, int64_t* batch_next, uint32_t cap, uint32_t* nbatches) {
+    int64_t nb = ck_txn_positions(buf, nbytes, run_start, nruns, next, batch_next, cap);
+    if (nb < 0) { g_create_error = "ck_fetch_positions: partition starts out of order"; return 1; }
+    if (nbatches) *nbatches = (uint32_t)nb;
+    if (batch_next && (uint64_t)nb > cap) { g_create_error = "ck_fetch_positions: batch_next shorter than the fetch's batches"; return 1; }
+    return 0;
+}
+
 // per record of the last ck_submit_recordbatch: where value / key / correlation_id header lie in the submitted buffer
 // (key_len / corr_len = -1: absent), and whether its frame failed the CRC / framing check
 static int fetch_rb_index_impl(ck_handle* h, int64_t* val_off, uint32_t* val_len, int64_t* key_off, int32_t* key_len,

@@ -198,4 +198,28 @@ static inline int64_t ck_txn_mask(const uint8_t* buf, uint64_t n, const uint64_t
     return b;
 }
 
+// The consumed positions of a record set buf[0..n) with the partition runs above: next[r] = lastOffset + 1 (baseOffset +
+// lastOffsetDelta + 1) of the last complete batch that starts in run r, or -1 when none does; batch_next[b] (up to cap of
+// them, null: not wanted) the same of batch b.  Every complete batch moves its partition's position, delivered or not:
+// control batches, aborted transactions' batches and batches that fail their framing or CRC32C alike, as the Java
+// consumer advances past them.  Only the 61-byte headers are read.  Returns the number of complete batches, or -1 when
+// the runs are not in order
+static inline int64_t ck_txn_positions(const uint8_t* buf, uint64_t n, const uint64_t* run_start, uint32_t nruns,
+                                       int64_t* next, int64_t* batch_next, uint64_t cap) {
+    for (uint32_t r = 0; r < nruns; r++) {
+        if (r && run_start[r] < run_start[r - 1]) return -1;
+        next[r] = -1;
+    }
+    int64_t run = -1;
+    uint64_t pos = 0, end;
+    int64_t b = 0;
+    for (; (end = ck_txn_frame_end(buf, n, pos)) != 0; pos = end, b++) {
+        while (run + 1 < (int64_t)nruns && run_start[run + 1] <= pos) run++;
+        int64_t nx = ck_txn_be64(buf + pos) + (int32_t)ck_txn_be32(buf + pos + 23) + 1;
+        if (run >= 0) next[run] = nx;
+        if (batch_next && (uint64_t)b < cap) batch_next[b] = nx;
+    }
+    return b;
+}
+
 #endif  // CK_TXN_H

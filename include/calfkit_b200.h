@@ -157,6 +157,14 @@ int  ck_set_fetch_hidden(ck_handle* h, const uint8_t* mask, uint32_t nbatches);
 int  ck_fetch_txn_mask(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
                        const uint32_t* abort_run, const int64_t* abort_pid, const int64_t* abort_first, uint32_t naborts,
                        uint8_t* mask, uint32_t cap, uint32_t* nbatches);
+/* ck_fetch_positions (no handle, no device): the offsets a consumer of a fetch, or of a slice of one cut at batch
+ * boundaries, resumes from.  With the partition runs of ck_fetch_txn_mask, next[r] (nruns entries) = lastOffset + 1
+ * (baseOffset + lastOffsetDelta + 1) of the last complete batch starting in run r, -1 when none does; batch_next[b] (cap
+ * entries; may be null) the same of each complete batch.  Every batch advances its partition's position, whether it is
+ * delivered, skipped (control, aborted) or bad (framing, CRC32C): only the 61-byte headers are read.  *nbatches = complete
+ * batches; fails when the run starts decrease or batch_next is shorter. */
+int  ck_fetch_positions(const uint8_t* buf, uint64_t nbytes, const uint64_t* run_start, uint32_t nruns,
+                        int64_t* next, int64_t* batch_next, uint32_t cap, uint32_t* nbatches);
 int  ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uint32_t n, int64_t base_offset, int64_t timestamp_ms,
                            uint8_t* host_frame, uint64_t cap, uint64_t* frame_len);
 /* produce side for a whole step (reference: the producer aiokafka runs under broker.publish, nodes/base.py:82-87, and under the
