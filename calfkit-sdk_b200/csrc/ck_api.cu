@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/calfkit_b200.h"
+#include "ck_buf.h"
 #include "ck_kernels.cuh"
 #include "ck_txn.h"
 
@@ -18,6 +19,15 @@ static_assert(sizeof(ck_frame) == sizeof(ck_frame_ent), "ck_frame must mirror ck
 
 static thread_local std::string g_create_error;
 
+// what ck_gate_create allocates: the key table and the counters, two sets of entries, slots and arena (ck_gate_compact
+// moves the live fan-outs from the set the gate uses into the other), the compaction's old index of every new entry and
+// each record's entry
+struct ck_gate_bufs {
+    ck_buf<unsigned long long> keys, ctr;
+    ck_buf<ck_gate_entry> entries[2]; ck_buf<ck_gate_slot> slots[2]; ck_buf<u8> arena[2];
+    ck_buf<u32> src, rec_entry;
+};
+
 struct ck_handle {
     int device = 0;
     u32 num_sms = 0;                 // grid size of the grid-stride kernels: a fixed number of blocks per SM
@@ -27,76 +37,79 @@ struct ck_handle {
     uint64_t max_in = 0, max_out = 0, max_aux = 0;
     uint32_t max_records = 0, max_payloads = 0, max_pubs = 0;
     // device buffers
-    u8* d_in = nullptr; long long* d_in_off = nullptr;
-    u8* d_out = nullptr; long long* d_out_off = nullptr;
-    u8* d_aux = nullptr; long long* d_aux_off = nullptr; u8* d_glue = nullptr;
-    u8* d_ovl = nullptr; long long* d_ovl_off = nullptr; u32* d_ovl_len = nullptr; ck_canon_ctl* d_canon_ctl = nullptr; u32* d_canon_list = nullptr; ck_elem* d_elems = nullptr; u32 elem_cap = 0; u32* d_cand = nullptr; uint2* d_hist_skip = nullptr;
+    ck_buf<u8> d_in; ck_buf<long long> d_in_off;
+    ck_buf<u8> d_out; ck_buf<long long> d_out_off;
+    ck_buf<u8> d_aux; ck_buf<long long> d_aux_off; ck_buf<u8> d_glue;
+    ck_buf<u8> d_ovl; ck_buf<long long> d_ovl_off; ck_buf<u32> d_ovl_len; ck_buf<ck_canon_ctl> d_canon_ctl; ck_buf<u32> d_canon_list; ck_buf<ck_elem> d_elems; u32 elem_cap = 0; ck_buf<u32> d_cand; ck_buf<uint2> d_hist_skip;
     uint64_t max_ovl = 0;
-    u32* d_cols = nullptr; ck_out_desc* d_descs = nullptr; u32* d_pay_len = nullptr; ck_pub* d_pubs = nullptr;
-    unsigned long long* d_tile_sum = nullptr; unsigned long long* d_grand = nullptr;
-    u8* d_lit = nullptr; ck_tool_cfg* d_tool_cfg = nullptr; ck_agent_cfg* d_agent_cfg = nullptr;
-    u32* d_counts = nullptr; long long* d_slot_base = nullptr; u32* d_agent_tables = nullptr;
+    ck_buf<u32> d_cols; ck_buf<ck_out_desc> d_descs; ck_buf<u32> d_pay_len; ck_buf<ck_pub> d_pubs;
+    ck_buf<unsigned long long> d_tile_sum, d_grand;
+    ck_buf<u8> d_lit; ck_buf<ck_tool_cfg> d_tool_cfg; ck_buf<ck_agent_cfg> d_agent_cfg;
+    ck_buf<u32> d_counts; ck_buf<long long> d_slot_base; ck_buf<u32> d_agent_tables;
     bool agent_set = false; ck_agent_cfg h_agent_cfg{};
-    u32* d_topic_hist = nullptr;
-    // aggregation gate (allocated by ck_gate_create)
-    ck_gate gate{}; bool gate_set = false; u32* d_rec_entry = nullptr;
+    ck_buf<u32> d_topic_hist;
+    // aggregation gate (ck_gate_create): the views the kernels take, over the buffers in gate_bufs
+    ck_gate gate{}; bool gate_set = false;
     ck_gate gate_spare{};               // the entries, slots and arena ck_gate_compact moves the live fan-outs into
-    u32* d_gate_src = nullptr;          // [max_entries] compaction: old index of every new entry
+    ck_gate_bufs gate_bufs;
     unsigned long long gate_reg_seq = 0;    // records registered so far: registration order of the entries
     // peer exchange (ck_comm_create)
-    u8* d_recv = nullptr; ck_xpeers peers{}; void* peer_opened[CK_X_MAXWORLD] = {nullptr}; u32 comm_rank = 0, comm_world = 0, max_fwd = 0, x_nb = 0;
-    unsigned long long region_stride = 0, region_data_cap = 0; u32* d_x_overflow = nullptr; bool comm_ready = false;
+    ck_buf<u8> d_recv; ck_xpeers peers{}; void* peer_opened[CK_X_MAXWORLD] = {nullptr}; u32 comm_rank = 0, comm_world = 0, max_fwd = 0, x_nb = 0;
+    unsigned long long region_stride = 0, region_data_cap = 0; ck_buf<u32> d_x_overflow; bool comm_ready = false;
     // publish grouping (allocated on first use)
-    u32 *d_g_hist = nullptr, *d_g_o1 = nullptr, *d_g_o2 = nullptr, *d_g_keys = nullptr; long long* d_g_base = nullptr; unsigned long long *d_g_tile = nullptr, *d_g_grand = nullptr;
+    ck_buf<u32> d_g_hist, d_g_o1, d_g_o2, d_g_keys; ck_buf<long long> d_g_base; ck_buf<unsigned long long> d_g_tile, d_g_grand;
     bool grouped = false; bool opt_bucket = false; const u32* cur_perm = nullptr;
     // Kafka record-batch framing (allocated on first use)
-    long long *d_rb_batch_off = nullptr, *d_rb_rec_pos = nullptr, *d_rb_key_off = nullptr, *d_rb_corr_off = nullptr;
-    u32 *d_rb_rec_base = nullptr, *d_rb_batch_bad = nullptr, *d_rb_rec_batch = nullptr, *d_rb_val_len = nullptr, *d_rb_rec_bad = nullptr;
-    int *d_rb_key_len = nullptr, *d_rb_corr_len = nullptr; uint32_t rb_n = 0;
-    long long* h_rb_boff = nullptr; u32* h_rb_rbase = nullptr; cudaEvent_t rb_ev = nullptr;   // pinned frame index staging
-    // fetches holding gzip or LZ4 batches (allocated on the first one): the raw bytes, then every such batch's decoded
-    // records section in its slot; per batch its slot (dec_off, n + 1 long, pinned staging h_rb_doff) and its decoded length
-    u8* d_rb_fetch = nullptr; uint64_t rb_fetch_cap = 0; long long *d_rb_dec_off = nullptr, *h_rb_doff = nullptr; u32* d_rb_dec_len = nullptr;
-    uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: no gzip / LZ4 batch)
+    ck_buf<long long> d_rb_batch_off, d_rb_rec_pos, d_rb_key_off, d_rb_corr_off;
+    ck_buf<u32> d_rb_rec_base, d_rb_batch_bad, d_rb_rec_batch, d_rb_val_len, d_rb_rec_bad;
+    ck_buf<int> d_rb_key_len, d_rb_corr_len; uint32_t rb_n = 0;
+    ck_pinned<long long> h_rb_boff; ck_pinned<u32> h_rb_rbase; cudaEvent_t rb_ev = nullptr;   // frame index staging
+    // fetches holding compressed batches (gzip, snappy, LZ4, zstd; allocated on the first one): the raw bytes, then every
+    // such batch's decoded records section in its slot; per batch its slot (dec_off, n + 1 long, staging h_rb_dec_off) and
+    // its decoded length
+    ck_buf<u8> d_rb_fetch; ck_buf<long long> d_rb_dec_off; ck_pinned<long long> h_rb_dec_off; ck_buf<u32> d_rb_dec_len;
+    uint64_t rb_dec_base = 0, rb_dec_bytes = 0;      // the decoded region of the last fetch (0 bytes: no compressed batch)
     // the chunk table of fetches holding snappy batches (ck_snappy.cuh; allocated on the first one, grown as needed): every
     // raw snappy block of the fetch and its place in its batch's slot, staged in page-locked memory
-    ck_sn_chunk *d_rb_sn = nullptr, *h_rb_sn = nullptr; u32 rb_sn_cap = 0, rb_sn_dcap = 0;
+    ck_buf<ck_sn_chunk> d_rb_sn; ck_pinned<ck_sn_chunk> h_rb_sn;
     // per batch the host's flag (ck_txn.h: bad / skipped), uploaded for a fetch that flags any (allocated on the first one);
     // rb_hide: the read_committed mask ck_set_fetch_hidden gave for the next fetch
-    u32 *d_rb_flag = nullptr, *h_rb_flag = nullptr; std::vector<uint8_t> rb_hide; bool rb_hide_set = false;
+    ck_buf<u32> d_rb_flag; ck_pinned<u32> h_rb_flag; std::vector<uint8_t> rb_hide; bool rb_hide_set = false;
     // frame pass (allocated on first use): per slot, then per record in group order; the frames and their table
-    ck_fitem* d_fr_items = nullptr; u32 *d_fr_gkey = nullptr, *d_fr_idx = nullptr, *d_fr_head = nullptr, *d_fr_fstart = nullptr, *d_fr_gfirst = nullptr;
-    u32 *d_fr_ffirst = nullptr, *d_fr_size = nullptr, *d_fr_nlive = nullptr, *d_fr_partial = nullptr;
-    long long *d_fr_gscan = nullptr, *d_fr_S = nullptr, *d_fr_F = nullptr, *d_fr_R = nullptr; unsigned long long *d_fr_tile = nullptr, *d_fr_grand = nullptr;
-    u32 *d_fr_o1 = nullptr, *d_fr_o2 = nullptr;      // its own sort buffers: the per-topic order of ck_group_publishes stays intact
-    ck_frame_ent* d_fr_table = nullptr; u8* d_fr_frames = nullptr; uint64_t fr_cap = 0; u32 fr_max = 0, fr_n = 0; bool fr_info = false, fr_sized = false;
+    ck_buf<ck_fitem> d_fr_items; ck_buf<u32> d_fr_gkey, d_fr_idx, d_fr_head, d_fr_fstart, d_fr_gfirst;
+    ck_buf<u32> d_fr_ffirst, d_fr_size, d_fr_nlive, d_fr_partial;
+    ck_buf<long long> d_fr_gscan, d_fr_S, d_fr_F, d_fr_R; ck_buf<unsigned long long> d_fr_tile, d_fr_grand;
+    ck_buf<u32> d_fr_o1, d_fr_o2;      // its own sort buffers: the per-topic order of ck_group_publishes stays intact
+    // fr_cap: the frames d_fr_frames (and d_fr_partial) have room for, 0 until fr_grow has reserved both
+    ck_buf<ck_frame_ent> d_fr_table; ck_buf<u8> d_fr_frames; uint64_t fr_cap = 0; u32 fr_max = 0, fr_n = 0; bool fr_info = false, fr_sized = false;
     const u32* fr_order = nullptr; long long fr_base = 0, fr_ts = 0;   // what the write half of the last pass needs to run again
-    u8* d_fr_blob = nullptr; long long* d_fr_desc = nullptr; long long* h_fr_info = nullptr;   // h_fr_info: pinned {frames, bytes}
-    int32_t* d_fr_slot = nullptr; u32 fr_nslots = 0, fr_ntopics = 0;
+    ck_buf<u8> d_fr_blob; ck_buf<long long> d_fr_desc; ck_pinned<long long> h_fr_info;   // h_fr_info: {frames, bytes}
+    ck_buf<int32_t> d_fr_slot; u32 fr_nslots = 0, fr_ntopics = 0;
     // idempotent / transactional produce: the producer fields the passes write (ck_set_producer; fr_prod: those of the last
     // pass, which a rewrite into a grown buffer uses again) and, by topic id, the sticky partition of the topic's unkeyed
     // publishes (ck_set_sticky_partitions; host copy for the record form, device copy for the plan's publishes)
     ck_producer prod{-1, -1, 0}, fr_prod{-1, -1, 0};
-    std::vector<int32_t> fr_sticky; int32_t* d_fr_sticky = nullptr; u32 fr_sticky_cap = 0;
+    std::vector<int32_t> fr_sticky; ck_buf<int32_t> d_fr_sticky;
     uint64_t fr_window = 1ull << 20;                 // frame_bytes (ck_set_option 2)
     // LZ4 frames (ck_set_option 3; allocated on the first compressed pass): the uncompressed frames, then the block slots,
-    // each fr_raw_cap bytes; per block slot its size and their scan; the offsets of the compressed frames
+    // each fr_raw_cap bytes (0 until lz_grow has reserved every buffer); per block slot its size and their scan; the
+    // offsets of the compressed frames
     u32 fr_codec = 0, fr_pass_codec = 0;             // option 3, and the codec of the last pass
-    u8* d_fr_raw = nullptr; uint64_t fr_raw_cap = 0; u32 fr_bmax = 0; u32* d_fr_bsize = nullptr;
-    long long *d_fr_bscan = nullptr, *d_fr_zoff = nullptr; unsigned long long* d_fr_btile = nullptr;
+    ck_buf<u8> d_fr_raw; uint64_t fr_raw_cap = 0; u32 fr_bmax = 0; ck_buf<u32> d_fr_bsize;
+    ck_buf<long long> d_fr_bscan, d_fr_zoff; ck_buf<unsigned long long> d_fr_btile;
     // exchange planning (allocated on first use)
-    u32* d_x_hist = nullptr; long long* d_x_base = nullptr; unsigned long long* d_x_nbytes = nullptr;
-    long long *d_x_src_off = nullptr, *d_x_len = nullptr, *d_x_dst_off = nullptr; u32 *d_x_len32 = nullptr, *d_x_pub = nullptr;
-    unsigned long long *d_x_tile = nullptr, *d_x_grand = nullptr, *d_x_grand2 = nullptr; long long* h_x = nullptr;   // h_x: pinned
+    ck_buf<u32> d_x_hist; ck_buf<long long> d_x_base; ck_buf<unsigned long long> d_x_nbytes;
+    ck_buf<long long> d_x_src_off, d_x_len, d_x_dst_off; ck_buf<u32> d_x_len32, d_x_pub;
+    ck_buf<unsigned long long> d_x_tile, d_x_grand, d_x_grand2; ck_pinned<long long> h_x;
     // topic table
-    ck_topic_table tab{}; u32 *d_tab_hash = nullptr, *d_tab_off = nullptr, *d_tab_len = nullptr; int32_t* d_tab_id = nullptr; u8* d_tab_names = nullptr;
+    ck_topic_table tab{}; ck_buf<u32> d_tab_hash, d_tab_off, d_tab_len; ck_buf<int32_t> d_tab_id; ck_buf<u8> d_tab_names;
     uint32_t num_partitions = 0, hist_cap = 0;
     // current batch
     const u8* cur_in = nullptr; const long long* cur_in_off = nullptr; const u32* cur_len = nullptr;
     uint32_t n = 0, n_payloads = 0, n_pubs = 0;
     bool tool_set = false; ck_tool_cfg h_tool_cfg{};
     unsigned long long n_launch = 0;
-    unsigned long long* h_grand = nullptr;   // pinned
+    ck_pinned<unsigned long long> h_grand;
     // profiling: asynchronous event pairs around every kernel, read back (and summed) on demand so
     // that timing the kernels does not serialise the stream during a timed region
     bool profile = false;
@@ -160,43 +173,43 @@ extern "C" int ck_create(int device, uint64_t max_in_bytes, uint64_t max_out_byt
     }
     h->max_in = max_in_bytes; h->max_out = max_out_bytes; h->max_aux = max_aux_bytes; h->max_records = max_records;
     h->max_payloads = max_payloads > max_records ? max_payloads : max_records; h->max_pubs = 2 * h->max_payloads;
-#define ALLOC(p, bytes) if ((e = cudaMalloc((void**)&(p), (bytes))) != cudaSuccess) return bail("cudaMalloc " #p, e)
+#define ALLOC(b, n) if ((e = (b).reserve((n), h->stream)) != cudaSuccess) return bail("allocating " #b, e)
     ALLOC(h->d_in, max_in_bytes + CK_PAD);
-    ALLOC(h->d_in_off, sizeof(long long) * ((size_t)max_records + 1));
+    ALLOC(h->d_in_off, (size_t)max_records + 1);
     ALLOC(h->d_out, max_out_bytes + CK_PAD);
-    ALLOC(h->d_out_off, sizeof(long long) * ((size_t)h->max_payloads + 1));
+    ALLOC(h->d_out_off, (size_t)h->max_payloads + 1);
     ALLOC(h->d_aux, max_aux_bytes + CK_PAD);
-    ALLOC(h->d_aux_off, sizeof(long long) * ((size_t)max_records + 1));
+    ALLOC(h->d_aux_off, (size_t)max_records + 1);
     ALLOC(h->d_glue, (size_t)CK_GLUE_STRIDE * h->max_payloads + CK_PAD);
     h->max_ovl = max_in_bytes;
     ALLOC(h->d_ovl, h->max_ovl + CK_PAD);
-    ALLOC(h->d_ovl_off, sizeof(long long) * ((size_t)max_records + 1));
-    ALLOC(h->d_ovl_len, sizeof(u32) * (size_t)max_records);
-    ALLOC(h->d_canon_ctl, sizeof(ck_canon_ctl));
-    ALLOC(h->d_canon_list, sizeof(u32) * (size_t)max_records);
+    ALLOC(h->d_ovl_off, (size_t)max_records + 1);
+    ALLOC(h->d_ovl_len, (size_t)max_records);
+    ALLOC(h->d_canon_ctl, 1);
+    ALLOC(h->d_canon_list, (size_t)max_records);
     // list elements of long records walked one per thread: a message of a history is rarely shorter than a few hundred bytes
     // (a full list only means the remaining ones are walked inside their record's warp)
     { unsigned long long cap = max_in_bytes / 256 + 1024; if (cap > 0x7fffffffull) cap = 0x7fffffffull; h->elem_cap = (u32)cap; }
-    ALLOC(h->d_elems, sizeof(ck_elem) * (size_t)h->elem_cap);
-    ALLOC(h->d_cand, sizeof(u32) * (size_t)max_records);
-    ALLOC(h->d_hist_skip, sizeof(uint2) * (size_t)max_records);
-    ALLOC(h->d_cols, sizeof(u32) * (size_t)CK_NUM_COLS * max_records);
-    ALLOC(h->d_descs, sizeof(ck_out_desc) * (size_t)h->max_payloads);
-    ALLOC(h->d_pay_len, sizeof(u32) * (size_t)h->max_payloads);
-    ALLOC(h->d_pubs, sizeof(ck_pub) * (size_t)h->max_pubs);
-    ALLOC(h->d_tile_sum, sizeof(unsigned long long) * ((size_t)h->max_payloads / CK_SCAN_TILE + 2));
-    ALLOC(h->d_grand, sizeof(unsigned long long));
+    ALLOC(h->d_elems, (size_t)h->elem_cap);
+    ALLOC(h->d_cand, (size_t)max_records);
+    ALLOC(h->d_hist_skip, (size_t)max_records);
+    ALLOC(h->d_cols, (size_t)CK_NUM_COLS * max_records);
+    ALLOC(h->d_descs, (size_t)h->max_payloads);
+    ALLOC(h->d_pay_len, (size_t)h->max_payloads);
+    ALLOC(h->d_pubs, (size_t)h->max_pubs);
+    ALLOC(h->d_tile_sum, (size_t)h->max_payloads / CK_SCAN_TILE + 2);
+    ALLOC(h->d_grand, 1);
     ALLOC(h->d_lit, CK_LIT_CAP + CK_PAD);
-    ALLOC(h->d_tool_cfg, sizeof(ck_tool_cfg));
-    ALLOC(h->d_agent_cfg, sizeof(ck_agent_cfg));
-    ALLOC(h->d_counts, sizeof(u32) * (size_t)max_records);
-    ALLOC(h->d_slot_base, sizeof(long long) * ((size_t)max_records + 1));
+    ALLOC(h->d_tool_cfg, 1);
+    ALLOC(h->d_agent_cfg, 1);
+    ALLOC(h->d_counts, (size_t)max_records);
+    ALLOC(h->d_slot_base, (size_t)max_records + 1);
     h->hist_cap = 4096;
-    ALLOC(h->d_topic_hist, sizeof(u32) * h->hist_cap);
+    ALLOC(h->d_topic_hist, h->hist_cap);
+    ALLOC(h->h_grand, 1);
 #undef ALLOC
-    cudaMemsetAsync(h->d_in + max_in_bytes, 0, CK_PAD, h->stream);
-    cudaMemsetAsync(h->d_topic_hist, 0, sizeof(u32) * h->hist_cap, h->stream);
-    if ((e = cudaMallocHost((void**)&h->h_grand, sizeof(unsigned long long))) != cudaSuccess) return bail("cudaMallocHost", e);
+    cudaMemsetAsync(h->d_in.p + max_in_bytes, 0, CK_PAD, h->stream);
+    cudaMemsetAsync(h->d_topic_hist.p, 0, sizeof(u32) * h->hist_cap, h->stream);
     if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return bail("init sync", e);
     *out = h;
     return 0;
@@ -206,40 +219,15 @@ extern "C" void ck_destroy(ck_handle* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    void* ptrs[] = {h->d_in, h->d_in_off, h->d_out, h->d_out_off, h->d_aux, h->d_aux_off, h->d_glue, h->d_ovl, h->d_ovl_off, h->d_ovl_len, h->d_canon_ctl, h->d_canon_list, h->d_elems, h->d_cand, h->d_hist_skip, h->d_cols, h->d_descs, h->d_pay_len,
-                    h->d_pubs, h->d_tile_sum, h->d_grand, h->d_lit, h->d_tool_cfg, h->d_agent_cfg, h->d_counts, h->d_slot_base, h->d_agent_tables, h->d_topic_hist, h->d_tab_hash, h->d_tab_off,
-                    h->d_tab_len, h->d_tab_id, h->d_tab_names, h->d_x_hist, h->d_x_base, h->d_x_nbytes, h->d_x_src_off, h->d_x_len, h->d_x_dst_off,
-                    h->d_x_len32, h->d_x_pub, h->d_x_tile, h->d_x_grand, h->d_x_grand2};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    void* gptrs[] = {h->gate.keys, h->gate.entries, h->gate.slots, h->gate.arena, h->gate.ctr, h->d_rec_entry,
-                     h->gate_spare.entries, h->gate_spare.slots, h->gate_spare.arena, h->d_gate_src,
-                     h->d_rb_batch_off, h->d_rb_rec_pos, h->d_rb_key_off, h->d_rb_corr_off, h->d_rb_rec_base, h->d_rb_batch_bad,
-                     h->d_g_hist, h->d_g_o1, h->d_g_o2, h->d_g_keys, h->d_g_base, h->d_g_tile, h->d_g_grand,
-                     h->d_rb_rec_batch, h->d_rb_val_len, h->d_rb_rec_bad, h->d_rb_key_len, h->d_rb_corr_len,
-                     h->d_fr_items, h->d_fr_gkey, h->d_fr_idx, h->d_fr_head, h->d_fr_fstart, h->d_fr_gfirst, h->d_fr_ffirst, h->d_fr_size, h->d_fr_nlive,
-                     h->d_fr_partial, h->d_fr_gscan, h->d_fr_S, h->d_fr_F, h->d_fr_R, h->d_fr_tile, h->d_fr_grand, h->d_fr_table, h->d_fr_frames,
-                     h->d_fr_blob, h->d_fr_desc, h->d_fr_slot, h->d_fr_o1, h->d_fr_o2, h->d_fr_raw, h->d_fr_bsize, h->d_fr_bscan,
-                     h->d_fr_zoff, h->d_fr_btile, h->d_rb_fetch, h->d_rb_dec_off, h->d_rb_dec_len, h->d_rb_flag, h->d_rb_sn,
-                     h->d_fr_sticky};
-    for (void* p : gptrs) if (p) cudaFree(p);
-    if (h->h_rb_doff) cudaFreeHost(h->h_rb_doff);
-    if (h->h_rb_flag) cudaFreeHost(h->h_rb_flag);
-    if (h->h_rb_sn) cudaFreeHost(h->h_rb_sn);
+    if (h->xstream) cudaStreamSynchronize(h->xstream);
     for (u32 d = 0; d < CK_X_MAXWORLD; d++) if (h->peer_opened[d]) cudaIpcCloseMemHandle(h->peer_opened[d]);
-    if (h->d_recv) cudaFree(h->d_recv);
-    if (h->d_x_overflow) cudaFree(h->d_x_overflow);
-    if (h->h_grand) cudaFreeHost(h->h_grand);
-    if (h->h_x) cudaFreeHost(h->h_x);
-    if (h->h_fr_info) cudaFreeHost(h->h_fr_info);
-    if (h->h_rb_boff) cudaFreeHost(h->h_rb_boff);
-    if (h->h_rb_rbase) cudaFreeHost(h->h_rb_rbase);
     if (h->rb_ev) cudaEventDestroy(h->rb_ev);
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
-    if (h->xstream) { cudaStreamSynchronize(h->xstream); cudaStreamDestroy(h->xstream); }
     if (h->x_ev0) cudaEventDestroy(h->x_ev0);
     if (h->x_ev1) cudaEventDestroy(h->x_ev1);
+    if (h->xstream) cudaStreamDestroy(h->xstream);
     if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
+    delete h;                                          // the buffers free themselves
 }
 
 static u32 host_fnv1a(const u8* p, u32 n) { u32 h = 2166136261u; for (u32 i = 0; i < n; i++) h = (h ^ p[i]) * 16777619u; return h ? h : 1u; }
@@ -262,23 +250,22 @@ extern "C" int ck_register_topics(ck_handle* h, const uint8_t* names, const uint
         }
         th[slot] = hh; toff[slot] = offsets[i]; tlen[slot] = len; tid[slot] = ids[i];
     }
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    void* olds[] = {h->d_tab_hash, h->d_tab_off, h->d_tab_len, h->d_tab_id, h->d_tab_names};
-    for (void* p : olds) if (p) cudaFree(p);
-    h->d_tab_hash = h->d_tab_off = h->d_tab_len = nullptr; h->d_tab_id = nullptr; h->d_tab_names = nullptr;
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));    // the kernels queued so far may read the old table
     u32 total = n ? offsets[n] : 0;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_tab_hash, sizeof(u32) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_tab_off, sizeof(u32) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_tab_len, sizeof(u32) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_tab_id, sizeof(int32_t) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_tab_names, (size_t)total + CK_PAD));
-    CUDA_TRY(h, cudaMemcpy(h->d_tab_hash, th.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_tab_off, toff.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_tab_len, tlen.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_tab_id, tid.data(), sizeof(int32_t) * cap, cudaMemcpyHostToDevice));
-    if (total) CUDA_TRY(h, cudaMemcpy(h->d_tab_names, names, total, cudaMemcpyHostToDevice));
-    h->tab.cap = cap; h->tab.hash = h->d_tab_hash; h->tab.id = h->d_tab_id; h->tab.name_off = h->d_tab_off;
-    h->tab.name_len = h->d_tab_len; h->tab.names = h->d_tab_names;
+    ck_buf<u32> d_hash, d_off, d_len; ck_buf<int32_t> d_id; ck_buf<u8> d_names;
+    CUDA_TRY(h, d_hash.reserve(cap, h->stream));
+    CUDA_TRY(h, d_off.reserve(cap, h->stream));
+    CUDA_TRY(h, d_len.reserve(cap, h->stream));
+    CUDA_TRY(h, d_id.reserve(cap, h->stream));
+    CUDA_TRY(h, d_names.reserve((size_t)total + CK_PAD, h->stream));
+    CUDA_TRY(h, cudaMemcpy(d_hash.p, th.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(d_off.p, toff.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(d_len.p, tlen.data(), sizeof(u32) * cap, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(d_id.p, tid.data(), sizeof(int32_t) * cap, cudaMemcpyHostToDevice));
+    if (total) CUDA_TRY(h, cudaMemcpy(d_names.p, names, total, cudaMemcpyHostToDevice));
+    h->tab.cap = cap; h->tab.hash = d_hash.p; h->tab.id = d_id.p; h->tab.name_off = d_off.p; h->tab.name_len = d_len.p; h->tab.names = d_names.p;
+    h->d_tab_hash = std::move(d_hash); h->d_tab_off = std::move(d_off); h->d_tab_len = std::move(d_len);
+    h->d_tab_id = std::move(d_id); h->d_tab_names = std::move(d_names);
     h->num_partitions = num_partitions;
     return 0;
 }
@@ -301,15 +288,15 @@ extern "C" int ck_set_tool_node(ck_handle* h, int32_t publish_topic_id, uint32_t
     }
     if (pool.size() > CK_LIT_CAP) return fail(h, "ck_set_tool_node: literal pool overflow");
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    CUDA_TRY(h, cudaMemcpy(h->d_lit, pool.data(), pool.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_tool_cfg, &c, sizeof c, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_lit.p, pool.data(), pool.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_tool_cfg.p, &c, sizeof c, cudaMemcpyHostToDevice));
     h->h_tool_cfg = c; h->tool_set = true;
     return 0;
 }
 
 static ck_view view_of(ck_handle* h) {
-    ck_view v; v.in = h->cur_in; v.off = h->cur_in_off; v.ovl = h->d_ovl; v.ovl_off = h->d_ovl_off; v.ovl_len = h->d_ovl_len;
-    v.canon_ctl = h->d_canon_ctl; v.canon_list = h->d_canon_list; v.len = h->cur_len; v.perm = h->cur_perm; v.elems = h->d_elems; v.elem_cap = h->elem_cap; v.hist_skip = h->d_hist_skip;
+    ck_view v; v.in = h->cur_in; v.off = h->cur_in_off; v.ovl = h->d_ovl.p; v.ovl_off = h->d_ovl_off.p; v.ovl_len = h->d_ovl_len.p;
+    v.canon_ctl = h->d_canon_ctl.p; v.canon_list = h->d_canon_list.p; v.len = h->cur_len; v.perm = h->cur_perm; v.elems = h->d_elems.p; v.elem_cap = h->elem_cap; v.hist_skip = h->d_hist_skip.p;
     return v;
 }
 
@@ -317,17 +304,14 @@ static int run_scan(ck_handle* h, const u32* len, u32 n, long long* out_off, u32
                     unsigned long long* tile_sum = nullptr, unsigned long long* grand = nullptr, int timer = CK_K_SCAN);
 
 static int group_alloc(ck_handle* h) {
-    u32 nb_max = (h->max_pubs + CK_G_BLOCK - 1) / CK_G_BLOCK;
-    if (!h->d_g_hist) {
-        size_t nh = 64 * (size_t)nb_max;
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_hist, sizeof(u32) * nh));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_base, sizeof(long long) * (nh + 1)));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_o1, sizeof(u32) * ((size_t)h->max_pubs + 1)));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_o2, sizeof(u32) * ((size_t)h->max_pubs + 1)));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_keys, sizeof(u32) * CK_G_KEYS));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_tile, sizeof(unsigned long long) * (nh / CK_SCAN_TILE + 2)));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_g_grand, sizeof(unsigned long long)));
-    }
+    size_t nh = 64 * (size_t)((h->max_pubs + CK_G_BLOCK - 1) / CK_G_BLOCK);
+    CUDA_TRY(h, h->d_g_hist.reserve(nh, h->stream));
+    CUDA_TRY(h, h->d_g_base.reserve(nh + 1, h->stream));
+    CUDA_TRY(h, h->d_g_o1.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_g_o2.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_g_keys.reserve(CK_G_KEYS, h->stream));
+    CUDA_TRY(h, h->d_g_tile.reserve(nh / CK_SCAN_TILE + 2, h->stream));
+    CUDA_TRY(h, h->d_g_grand.reserve(1, h->stream));
     return 0;
 }
 
@@ -336,8 +320,8 @@ static int group_alloc(ck_handle* h) {
 // counts, for keys below CK_G_KEYS
 template <int SHIFT, class KeyFn>
 static void group_pass(ck_handle* h, KeyFn keyf, const u32* in, u32 n, u32 nb, u32* key_hist, bool count, u32* dst) {
-    if (count) CKL(h) ck_group_count_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_hist, key_hist);
-    else CKL(h) ck_group_scatter_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_base, dst);
+    if (count) CKL(h) ck_group_count_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_hist.p, key_hist);
+    else CKL(h) ck_group_scatter_kernel<SHIFT, KeyFn><<<nb, CK_G_BLOCK, 0, h->stream>>>(keyf, in, n, h->d_g_base.p, dst);
 }
 template <class KeyFn>
 static void group_launch(ck_handle* h, KeyFn keyf, u32 p, const u32* in, u32 n, u32 nb, u32* key_hist, bool count, u32* dst) {
@@ -352,7 +336,7 @@ static void group_launch(ck_handle* h, KeyFn keyf, u32 p, const u32* in, u32 n, 
 template <class KeyFn>
 static int group_sort(ck_handle* h, KeyFn keyf, u32 n, int timer, u32 passes = 2, u32* key_hist = nullptr, const u32** result = nullptr,
                       u32* o1 = nullptr, u32* o2 = nullptr) {
-    if (!o1) { o1 = h->d_g_o1; o2 = h->d_g_o2; }
+    if (!o1) { o1 = h->d_g_o1.p; o2 = h->d_g_o2.p; }
     if (key_hist) CUDA_TRY(h, cudaMemsetAsync(key_hist, 0, sizeof(u32) * CK_G_KEYS, h->stream));
     if (result) *result = (passes & 1) ? o1 : o2;
     if (!n) return 0;
@@ -366,7 +350,7 @@ static int group_sort(ck_handle* h, KeyFn keyf, u32 n, int timer, u32 passes = 2
             group_launch(h, keyf, p, p ? out_of(p - 1) : nullptr, n, nb, key_hist, true, nullptr);
             CUDA_TRY(h, cudaGetLastError());
         }
-        if (run_scan(h, h->d_g_hist, 64 * nb, h->d_g_base, 0, h->d_g_tile, h->d_g_grand)) return 1;
+        if (run_scan(h, h->d_g_hist.p, 64 * nb, h->d_g_base.p, 0, h->d_g_tile.p, h->d_g_grand.p)) return 1;
     }
     {
         KTimer t(h, timer);
@@ -382,14 +366,14 @@ static int launch_decode(ck_handle* h) {
     u32 n = h->n;
     if (!n) return 0;
     ck_view v = view_of(h);
-    CUDA_TRY(h, cudaMemsetAsync(h->d_ovl_off, 0xff, sizeof(long long) * (size_t)n, h->stream));      // no overlays yet
-    CUDA_TRY(h, cudaMemsetAsync(h->d_canon_ctl, 0, sizeof(ck_canon_ctl), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_ovl_off.p, 0xff, sizeof(long long) * (size_t)n, h->stream));      // no overlays yet
+    CUDA_TRY(h, cudaMemsetAsync(h->d_canon_ctl.p, 0, sizeof(ck_canon_ctl), h->stream));
     h->cur_perm = nullptr;
     if (h->opt_bucket && n > 64) {
         if (group_alloc(h)) return 1;
         ck_key_len kf; kf.v = v;
-        if (group_sort(h, kf, n, CK_K_WALK, 2, h->d_g_keys)) return 1;
-        h->cur_perm = h->d_g_o2;
+        if (group_sort(h, kf, n, CK_K_WALK, 2, h->d_g_keys.p)) return 1;
+        h->cur_perm = h->d_g_o2.p;
         v = view_of(h);
     }
     {
@@ -397,21 +381,21 @@ static int launch_decode(ck_handle* h) {
         // for the element pass, or (long records that are long for another reason) the whole record walked by the warp.
         // Both kernels exit at once when there are no such records.
         KTimer t(h, CK_K_WALK_LONG);
-        CKL(h) ck_classify_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(v, n, h->d_cand);
+        CKL(h) ck_classify_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(v, n, h->d_cand.p);
         u32 lblocks = (n + CK_LONG_WARPS - 1) / CK_LONG_WARPS; if (lblocks > h->num_sms * CK_LONG_MINB) lblocks = h->num_sms * CK_LONG_MINB;
-        CKL(h) ck_walk_long_kernel<<<lblocks, 32 * CK_LONG_WARPS, CK_LONG_WARPS * sizeof(ck_long_index), h->stream>>>(v, h->d_cols, n, h->d_cand, h->d_hist_skip);
+        CKL(h) ck_walk_long_kernel<<<lblocks, 32 * CK_LONG_WARPS, CK_LONG_WARPS * sizeof(ck_long_index), h->stream>>>(v, h->d_cols.p, n, h->d_cand.p, h->d_hist_skip.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     {
         KTimer t(h, CK_K_WALK);
-        CKL(h) ck_walk_kernel<<<(n + 127) / 128, 128, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, n, h->d_cols, n);
+        CKL(h) ck_walk_kernel<<<(n + 127) / 128, 128, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, n, h->d_cols.p, n);
         CUDA_TRY(h, cudaGetLastError());
     }
     {
         // the history messages listed by the pre-scan or deferred by the long walker, one thread each (exits at once when
         // there are none)
         KTimer t(h, CK_K_WALK_ELEMS);
-        CKL(h) ck_walk_elems_kernel<<<h->num_sms * CK_WALK_MINB, CK_WALK_THREADS, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, h->d_cols, n);
+        CKL(h) ck_walk_elems_kernel<<<h->num_sms * CK_WALK_MINB, CK_WALK_THREADS, CK_WALK_THREADS * CK_WIN_STRIDE, h->stream>>>(v, h->d_cols.p, n);
         CUDA_TRY(h, cudaGetLastError());
     }
     {
@@ -419,8 +403,8 @@ static int launch_decode(ck_handle* h) {
         // overlay and walked again in that spelling
         KTimer t(h, CK_K_CANON);
         u32 blocks = (n + 63) / 64; if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
-        CKL(h) ck_canon_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols, n, h->d_ovl, (long long)h->max_ovl, h->d_ovl_off, h->d_ovl_len);
-        CKL(h) ck_rewalk_list_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols, n);
+        CKL(h) ck_canon_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols.p, n, h->d_ovl.p, (long long)h->max_ovl, h->d_ovl_off.p, h->d_ovl_len.p);
+        CKL(h) ck_rewalk_list_kernel<<<blocks, 64, 0, h->stream>>>(v, n, h->d_cols.p, n);
         CUDA_TRY(h, cudaGetLastError());
     }
     return 0;
@@ -432,10 +416,10 @@ extern "C" int ck_submit(ck_handle* h, const uint8_t* host_in, const int64_t* ho
     uint64_t nbytes = n ? (uint64_t)(host_off[n] - host_off[0]) : 0;
     if (n && host_off[0] != 0) return fail(h, "ck_submit: offsets must start at 0");
     if (nbytes > h->max_in) return fail(h, "ck_submit: batch larger than max_in_bytes");
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_in, host_in, nbytes, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_in_off, host_off, sizeof(long long) * ((size_t)n + 1), cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_in + nbytes, 0, 16, h->stream));
-    h->cur_in = h->d_in; h->cur_in_off = h->d_in_off; h->cur_len = nullptr; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_in.p, host_in, nbytes, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_in_off.p, host_off, sizeof(long long) * ((size_t)n + 1), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_in.p + nbytes, 0, 16, h->stream));
+    h->cur_in = h->d_in.p; h->cur_in_off = h->d_in_off.p; h->cur_len = nullptr; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
     return launch_decode(h);
 }
 
@@ -449,7 +433,7 @@ extern "C" int ck_submit_device(ck_handle* h, const uint8_t* dev_in, const int64
 static int run_scan(ck_handle* h, const u32* len, u32 n, long long* out_off, u32 pad,
                     unsigned long long* tile_sum, unsigned long long* grand, int timer) {
     KTimer t(h, timer);
-    if (!tile_sum) { tile_sum = h->d_tile_sum; grand = h->d_grand; }
+    if (!tile_sum) { tile_sum = h->d_tile_sum.p; grand = h->d_grand.p; }
     u32 ntiles = (n + CK_SCAN_TILE - 1) / CK_SCAN_TILE;
     if (n) {
         CKL(h) ck_scan_tiles_kernel<<<ntiles, CK_SCAN_BLOCK, 0, h->stream>>>(len, n, tile_sum, pad);
@@ -461,13 +445,13 @@ static int run_scan(ck_handle* h, const u32* len, u32 n, long long* out_off, u32
 }
 
 static int scan_emit(ck_handle* h, u32 npay, const u8* aux) {
-    if (run_scan(h, h->d_pay_len, npay, h->d_out_off, 15)) return 1;   // payloads start 16-byte aligned
+    if (run_scan(h, h->d_pay_len.p, npay, h->d_out_off.p, 15)) return 1;   // payloads start 16-byte aligned
     {
         KTimer t(h, CK_K_EMIT);
         if (npay) {
             u32 warps_per_block = 256 / 32;
             CKL(h) ck_emit_kernel<<<(npay + warps_per_block - 1) / warps_per_block, 256, 0, h->stream>>>(
-                view_of(h), h->d_lit, aux, h->d_glue, h->d_descs, h->d_out_off, npay, h->d_out, (long long)h->max_out);
+                view_of(h), h->d_lit.p, aux, h->d_glue.p, h->d_descs.p, h->d_out_off.p, npay, h->d_out.p, (long long)h->max_out);
         }
         CUDA_TRY(h, cudaGetLastError());
     }
@@ -484,8 +468,8 @@ static int launch_plan(ck_handle* h, const long long* aux_off, int mode) {
     }
     KTimer t(h, CK_K_PLAN);
     if (h->n) CKL(h) ck_plan_tool_kernel<<<(h->n + CK_P2_THREADS - 1) / CK_P2_THREADS, CK_P2_THREADS, CK_P2_SMEM, h->stream>>>(
-        view_of(h), h->n, h->d_cols, h->n, h->d_tool_cfg, h->d_lit, aux_off, mode, h->d_descs, h->d_pay_len, h->d_pubs,
-        h->tab, h->num_partitions, h->d_topic_hist, h->hist_cap);
+        view_of(h), h->n, h->d_cols.p, h->n, h->d_tool_cfg.p, h->d_lit.p, aux_off, mode, h->d_descs.p, h->d_pay_len.p, h->d_pubs.p,
+        h->tab, h->num_partitions, h->d_topic_hist.p, h->hist_cap);
     CUDA_TRY(h, cudaGetLastError());
     return 0;
 }
@@ -513,9 +497,9 @@ extern "C" int ck_tool_plan(ck_handle* h, const uint8_t* host_aux, const int64_t
     if (host_aux_off) {
         uint64_t nb = (uint64_t)host_aux_off[h->n];
         if (nb > h->max_aux) return fail(h, "ck_tool_plan: results larger than max_aux_bytes");
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_aux, host_aux, nb, cudaMemcpyHostToDevice, h->stream));
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_aux_off, host_aux_off, sizeof(long long) * ((size_t)h->n + 1), cudaMemcpyHostToDevice, h->stream));
-        return tool_plan_common(h, h->d_aux, h->d_aux_off);
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_aux.p, host_aux, nb, cudaMemcpyHostToDevice, h->stream));
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_aux_off.p, host_aux_off, sizeof(long long) * ((size_t)h->n + 1), cudaMemcpyHostToDevice, h->stream));
+        return tool_plan_common(h, h->d_aux.p, h->d_aux_off.p);
     }
     return tool_plan_common(h, nullptr, nullptr);
 }
@@ -537,8 +521,8 @@ extern "C" int ck_reply_plan(ck_handle* h, uint32_t mode) {
     if (mode > 2) return fail(h, "ck_reply_plan: mode must be 0 (auto), 1 (text) or 2 (data)");
     {
         KTimer t(h, CK_K_PLAN);
-        if (h->n) CKL(h) ck_reply_plan_kernel<<<(h->n + 127) / 128, 128, 0, h->stream>>>(view_of(h), h->n, h->d_cols, h->n, mode, h->d_glue,
-                                                                               h->d_descs, h->d_pay_len);
+        if (h->n) CKL(h) ck_reply_plan_kernel<<<(h->n + 127) / 128, 128, 0, h->stream>>>(view_of(h), h->n, h->d_cols.p, h->n, mode, h->d_glue.p,
+                                                                               h->d_descs.p, h->d_pay_len.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (scan_emit(h, h->n, nullptr)) return 1;
@@ -587,15 +571,16 @@ extern "C" int ck_set_agent_node(ck_handle* h, int32_t publish_topic_id, const u
           tab[5 * ntools + k] = ck_hash_span(hr, 0, (u32)nm.size()); }    // the device compares it with ck_hash_span of the name in the record
     }
     if (pool.size() > CK_LIT_CAP) return fail(h, "ck_set_agent_node: literal pool overflow");
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (h->d_agent_tables) { cudaFree(h->d_agent_tables); h->d_agent_tables = nullptr; }
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_agent_tables, sizeof(u32) * (tab.size() + 1)));
-    CUDA_TRY(h, cudaMemcpy(h->d_agent_tables, tab.data(), sizeof(u32) * tab.size(), cudaMemcpyHostToDevice));
-    c.tool_name_off = h->d_agent_tables; c.tool_name_len = h->d_agent_tables + ntools;
-    c.tool_lit_off = h->d_agent_tables + 2 * ntools; c.tool_lit_len = h->d_agent_tables + 3 * ntools;
-    c.tool_topic_id = h->d_agent_tables + 4 * ntools;
-    CUDA_TRY(h, cudaMemcpy(h->d_lit, pool.data(), pool.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_agent_cfg, &c, sizeof c, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));    // the kernels queued so far may read the old tables
+    ck_buf<u32> tables;
+    CUDA_TRY(h, tables.reserve(tab.size() + 1, h->stream));
+    CUDA_TRY(h, cudaMemcpy(tables.p, tab.data(), sizeof(u32) * tab.size(), cudaMemcpyHostToDevice));
+    c.tool_name_off = tables.p; c.tool_name_len = tables.p + ntools;
+    c.tool_lit_off = tables.p + 2 * ntools; c.tool_lit_len = tables.p + 3 * ntools;
+    c.tool_topic_id = tables.p + 4 * ntools;
+    CUDA_TRY(h, cudaMemcpy(h->d_lit.p, pool.data(), pool.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_agent_cfg.p, &c, sizeof c, cudaMemcpyHostToDevice));
+    h->d_agent_tables = std::move(tables);
     h->h_agent_cfg = c; h->agent_set = true;
     return 0;
 }
@@ -604,9 +589,9 @@ extern "C" int ck_set_agent_tool_topic_ids(ck_handle* h, int32_t self_topic_id, 
     cudaSetDevice(h->device);
     if (!h->agent_set || ntools != h->h_agent_cfg.ntools) return fail(h, "ck_set_agent_tool_topic_ids: agent node not set / size mismatch");
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (ntools) CUDA_TRY(h, cudaMemcpy(h->d_agent_tables + 4 * (size_t)ntools, ids, sizeof(u32) * ntools, cudaMemcpyHostToDevice));
+    if (ntools) CUDA_TRY(h, cudaMemcpy(h->d_agent_tables.p + 4 * (size_t)ntools, ids, sizeof(u32) * ntools, cudaMemcpyHostToDevice));
     h->h_agent_cfg.self_topic_id = self_topic_id;
-    CUDA_TRY(h, cudaMemcpy(h->d_agent_cfg, &h->h_agent_cfg, sizeof h->h_agent_cfg, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_agent_cfg.p, &h->h_agent_cfg, sizeof h->h_agent_cfg, cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -618,16 +603,16 @@ extern "C" int ck_tailcall_plan(ck_handle* h, uint64_t unix_ms, uint64_t seed) {
     if (n > h->max_payloads) return fail(h, "ck_tailcall_plan: more payloads than max_payloads");
     {
         KTimer t(h, CK_K_FANOUT);
-        if (n) CKL(h) ck_tailcall_plan_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->d_agent_cfg, h->d_lit,
-            unix_ms, seed, h->d_aux, h->d_glue, h->d_descs, h->d_pay_len, h->d_pubs);
+        if (n) CKL(h) ck_tailcall_plan_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->d_agent_cfg.p, h->d_lit.p,
+            unix_ms, seed, h->d_aux.p, h->d_glue.p, h->d_descs.p, h->d_pay_len.p, h->d_pubs.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (scan_emit(h, n, h->d_aux)) return 1;
+    if (scan_emit(h, n, h->d_aux.p)) return 1;
     {
         KTimer t(h, CK_K_ROUTE);
         u32 npubs = 2 * n;
-        if (npubs) CKL(h) ck_route_kernel<<<(npubs + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_cols, n, h->d_pubs, npubs,
-            h->tab, h->num_partitions, h->d_topic_hist, h->hist_cap);
+        if (npubs) CKL(h) ck_route_kernel<<<(npubs + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_cols.p, n, h->d_pubs.p, npubs,
+            h->tab, h->num_partitions, h->d_topic_hist.p, h->hist_cap);
         CUDA_TRY(h, cudaGetLastError());
         h->n_pubs = npubs;
     }
@@ -646,28 +631,28 @@ extern "C" int ck_fanout_plan(ck_handle* h, uint64_t unix_ms, uint64_t seed, uin
             CUDA_TRY(h, cudaFuncSetAttribute(ck_fanout2_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CK_F2_SMEM));
             f2_attr = true;
         }
-        if (n) CKL(h) ck_fanout2_count_kernel<<<(n + CK_F2_WARPS - 1) / CK_F2_WARPS, 32 * CK_F2_WARPS, CK_F2_SMEM, h->stream>>>(view_of(h), n, h->d_cols, n, h->d_agent_cfg,
-                                                                                                             max_fanout, sequential, h->d_counts);
+        if (n) CKL(h) ck_fanout2_count_kernel<<<(n + CK_F2_WARPS - 1) / CK_F2_WARPS, 32 * CK_F2_WARPS, CK_F2_SMEM, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->d_agent_cfg.p,
+                                                                                                             max_fanout, sequential, h->d_counts.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_counts, n, h->d_slot_base, 0)) return 1;
-    *h->h_grand = 0;
-    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->h_grand, h->d_grand, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    if (run_scan(h, h->d_counts.p, n, h->d_slot_base.p, 0)) return 1;
+    *h->h_grand.p = 0;
+    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->h_grand.p, h->d_grand.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    unsigned long long slots = *h->h_grand;
+    unsigned long long slots = *h->h_grand.p;
     if (slots > h->max_payloads) return fail(h, "ck_fanout_plan: more payloads than max_payloads");
     {
         KTimer t(h, CK_K_FANOUT);
-        if (n) CKL(h) ck_fanout2_plan_kernel<<<(n + CK_F2_WARPS - 1) / CK_F2_WARPS, 32 * CK_F2_WARPS, CK_F2_SMEM, h->stream>>>(view_of(h), n, h->d_cols, n, h->d_agent_cfg, h->d_lit,
-            h->d_agent_tables + 5 * (size_t)h->h_agent_cfg.ntools, h->d_slot_base, unix_ms, seed, h->d_aux, h->d_glue, h->d_descs, h->d_pay_len, h->d_pubs);
+        if (n) CKL(h) ck_fanout2_plan_kernel<<<(n + CK_F2_WARPS - 1) / CK_F2_WARPS, 32 * CK_F2_WARPS, CK_F2_SMEM, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->d_agent_cfg.p, h->d_lit.p,
+            h->d_agent_tables.p + 5 * (size_t)h->h_agent_cfg.ntools, h->d_slot_base.p, unix_ms, seed, h->d_aux.p, h->d_glue.p, h->d_descs.p, h->d_pay_len.p, h->d_pubs.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (scan_emit(h, (u32)slots, h->d_aux)) return 1;
+    if (scan_emit(h, (u32)slots, h->d_aux.p)) return 1;
     {
         KTimer t(h, CK_K_ROUTE);
         u32 npubs = 2 * (u32)slots;
-        if (npubs) CKL(h) ck_route_kernel<<<(npubs + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_cols, n, h->d_pubs, npubs,
-            h->tab, h->num_partitions, h->d_topic_hist, h->hist_cap);
+        if (npubs) CKL(h) ck_route_kernel<<<(npubs + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_cols.p, n, h->d_pubs.p, npubs,
+            h->tab, h->num_partitions, h->d_topic_hist.p, h->hist_cap);
         CUDA_TRY(h, cudaGetLastError());
         h->n_pubs = npubs;
     }
@@ -679,8 +664,8 @@ extern "C" int ck_group_publishes(ck_handle* h) {
     cudaSetDevice(h->device);
     if (group_alloc(h)) return 1;
     h->grouped = true;
-    ck_key_pub kf; kf.pubs = h->d_pubs; kf.rank = h->comm_rank; kf.world = h->comm_ready ? h->comm_world : 1;
-    return group_sort(h, kf, h->n_pubs, CK_K_ROUTE, 2, h->d_g_keys);
+    ck_key_pub kf; kf.pubs = h->d_pubs.p; kf.rank = h->comm_rank; kf.world = h->comm_ready ? h->comm_world : 1;
+    return group_sort(h, kf, h->n_pubs, CK_K_ROUTE, 2, h->d_g_keys.p);
 }
 
 // engine options.  CK_OPT_BUCKET (1): bucket every submitted batch by record length before the thread-per-record walk —
@@ -701,68 +686,19 @@ extern "C" int ck_set_option(ck_handle* h, uint32_t option, uint64_t value) {
 extern "C" int ck_fetch_groups(ck_handle* h, uint32_t* host_order, uint32_t* host_key_counts, int wait) {
     cudaSetDevice(h->device);
     if (!h->grouped) return fail(h, "ck_fetch_groups: call ck_group_publishes first");
-    if (h->n_pubs) CUDA_TRY(h, cudaMemcpyAsync(host_order, h->d_g_o2, sizeof(u32) * (size_t)h->n_pubs, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(host_key_counts, h->d_g_keys, sizeof(u32) * CK_G_KEYS, cudaMemcpyDeviceToHost, h->stream));
+    if (h->n_pubs) CUDA_TRY(h, cudaMemcpyAsync(host_order, h->d_g_o2.p, sizeof(u32) * (size_t)h->n_pubs, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_key_counts, h->d_g_keys.p, sizeof(u32) * CK_G_KEYS, cudaMemcpyDeviceToHost, h->stream));
     if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
 
 // ---- Kafka RecordBatch v2 framing (csrc/ck_kafka.cuh) -------------------------------------------------------------------
-static int rb_alloc(ck_handle* h) {
-    if (h->d_rb_batch_off) return 0;
-    size_t mr = (size_t)h->max_records + 1;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_batch_off, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_base, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_batch_bad, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_pos, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_batch, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_val_len, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_key_off, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_key_len, sizeof(int) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_corr_off, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_corr_len, sizeof(int) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_rec_bad, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_boff, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_rbase, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaEventCreateWithFlags(&h->rb_ev, cudaEventDisableTiming));
-    return 0;
-}
 static inline uint32_t host_be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
 
-// the per-batch arrays of fetches holding gzip or LZ4 batches, on the first such fetch
-static int rb_lz_alloc(ck_handle* h) {
-    if (h->d_rb_dec_off) return 0;
-    size_t mr = (size_t)h->max_records + 1;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_dec_off, sizeof(long long) * mr));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_dec_len, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_doff, sizeof(long long) * mr));
-    return 0;
-}
-// the per-batch flags of fetches holding a control batch or under a read_committed mask, on the first such fetch
-static int rb_flag_alloc(ck_handle* h) {
-    if (h->d_rb_flag) return 0;
-    size_t mr = (size_t)h->max_records + 1;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_flag, sizeof(u32) * mr));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_rb_flag, sizeof(u32) * mr));
-    return 0;
-}
-// room for n entries in the chunk table's staging, its first `used` entries kept (the caller has waited for rb_ev: no copy
-// reads the staging)
+// room for n entries in the chunk table's staging, at least doubling it, its first `used` entries kept
 static int rb_sn_reserve(ck_handle* h, u32 n, u32 used) {
-    if (n <= h->rb_sn_cap) return 0;
-    u32 cap = std::max(n, std::max(1024u, h->rb_sn_cap * 2u));
-    ck_sn_chunk* p = nullptr;
-    CUDA_TRY(h, cudaMallocHost((void**)&p, sizeof(ck_sn_chunk) * cap));
-    if (h->h_rb_sn) { memcpy(p, h->h_rb_sn, sizeof(ck_sn_chunk) * used); cudaFreeHost(h->h_rb_sn); }
-    h->h_rb_sn = p; h->rb_sn_cap = cap;
-    return 0;
-}
-// the fetch buffer: raw bytes, then the decoded slots.  Grown as fr_grow grows the frame buffer (waits for the stream once)
-static int rb_fetch_grow(ck_handle* h, uint64_t cap) {
-    if (h->d_rb_fetch) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_rb_fetch); }
-    h->d_rb_fetch = nullptr; h->rb_fetch_cap = 0;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_fetch, cap + CK_PAD));
-    h->rb_fetch_cap = cap;
+    if (n <= h->h_rb_sn.cap) return 0;
+    CUDA_TRY(h, h->h_rb_sn.reserve(std::max<size_t>(n, std::max<size_t>(1024, 2 * h->h_rb_sn.cap)), h->stream, used));
     return 0;
 }
 
@@ -788,13 +724,21 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     bool hide = h->rb_hide_set;                        // the mask given for this fetch, consumed by it whatever happens
     h->rb_hide_set = false;
     if (nbytes > h->max_in) return fail(h, "ck_submit_recordbatch: buffer larger than max_in_bytes");
-    if (rb_alloc(h)) return 1;
+    size_t mr = (size_t)h->max_records + 1;
+    CUDA_TRY(h, h->d_rb_batch_off.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_rec_base.reserve(mr, h->stream));
+    CUDA_TRY(h, h->d_rb_batch_bad.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_rec_pos.reserve(mr, h->stream));
+    CUDA_TRY(h, h->d_rb_rec_batch.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_val_len.reserve(mr, h->stream));
+    CUDA_TRY(h, h->d_rb_key_off.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_key_len.reserve(mr, h->stream));
+    CUDA_TRY(h, h->d_rb_corr_off.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_corr_len.reserve(mr, h->stream));
+    CUDA_TRY(h, h->d_rb_rec_bad.reserve(mr, h->stream));
+    CUDA_TRY(h, h->h_rb_boff.reserve(mr, h->stream)); CUDA_TRY(h, h->h_rb_rbase.reserve(mr, h->stream));
+    if (!h->rb_ev) CUDA_TRY(h, cudaEventCreateWithFlags(&h->rb_ev, cudaEventDisableTiming));
     // the frame index is staged in page-locked memory the handle owns: its copies are asynchronous.  The staging is reused
     // once the copies of the previous call have been done (normally long ago: it waits for those copies only)
     CUDA_TRY(h, cudaEventSynchronize(h->rb_ev));
-    long long* boff = h->h_rb_boff; u32* rbase = h->h_rb_rbase;
+    long long* boff = h->h_rb_boff.p; u32* rbase = h->h_rb_rbase.p;
     uint64_t pos = 0; uint64_t total = 0; u32 nb = 0;
-    bool lz = false, has_lz4 = false, has_gz = false, has_zs = false, has_sn = false;   // lz: the fetch holds a decoded batch
+    bool decoded = false, has_lz4 = false, has_gz = false, has_zs = false, has_sn = false;   // decoded: a batch is decoded into a slot
     u32 nsn = 0;                                       // entries of the snappy chunk table
     bool flagged = false;                              // some batch is flagged bad or skipped by the host
     uint64_t dbytes = 0;                               // slot bytes so far (the LZ4 and zstd bounds, the gzip ISIZEs, the snappy lengths)
@@ -807,16 +751,17 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
         u32 flag = (host_buf[pos + 22] & CK_TXN_CONTROL) ? (u32)ck_txn_control(host_buf + pos, end - pos, &type)
                  : hide && nb < h->rb_hide.size() && h->rb_hide[nb] ? (u32)CK_TXN_HIDE : (u32)CK_TXN_SHOW;
         if (flag && !flagged) {                        // the batches before the first flagged one are delivered
-            if (rb_flag_alloc(h)) return 1;
-            for (u32 b = 0; b < nb; b++) h->h_rb_flag[b] = 0;
+            CUDA_TRY(h, h->d_rb_flag.reserve(mr, h->stream)); CUDA_TRY(h, h->h_rb_flag.reserve(mr, h->stream));
+            for (u32 b = 0; b < nb; b++) h->h_rb_flag.p[b] = 0;
             flagged = true;
         }
-        if (flagged) h->h_rb_flag[nb] = flag;
+        if (flagged) h->h_rb_flag.p[nb] = flag;
         if (!flag && (codec == CK_RB_LZ4 || codec == CK_RB_GZIP || codec == CK_RB_ZSTD || codec == CK_RB_SNAPPY)) {
-            if (!lz) {                                 // the batches before the first decoded one have empty slots
-                if (rb_lz_alloc(h)) return 1;
-                for (u32 b = 0; b <= nb; b++) h->h_rb_doff[b] = 0;
-                lz = true;
+            if (!decoded) {                            // the batches before the first decoded one have empty slots
+                CUDA_TRY(h, h->d_rb_dec_off.reserve(mr, h->stream)); CUDA_TRY(h, h->d_rb_dec_len.reserve(mr, h->stream));
+                CUDA_TRY(h, h->h_rb_dec_off.reserve(mr, h->stream));
+                for (u32 b = 0; b <= nb; b++) h->h_rb_dec_off.p[b] = 0;
+                decoded = true;
             }
             // the slot: LZ4, what the block chain decodes to at most; gzip, the member's ISIZE; zstd, what the blocks
             // decode to at most (compressed ones Block_Maximum_Size, even when Frame_Content_Size says less: their literals
@@ -846,13 +791,13 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
                 while ((r = ck_sn_next(z, end - pos - CK_RB_HEADER, w, &off, &len, &dl)) > 0) {
                     if (CK_RB_HEADER + o + dl > 0x7fffffffull) { r = -1; break; }
                     if (rb_sn_reserve(h, nsn + 1, nsn)) return 1;
-                    h->h_rb_sn[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER + off), nb, len, (u32)o, dl};
+                    h->h_rb_sn.p[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER + off), nb, len, (u32)o, dl};
                     o += dl;
                 }
                 if (r < 0) {
                     nsn = first;
                     if (rb_sn_reserve(h, nsn + 1, nsn)) return 1;
-                    h->h_rb_sn[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER), nb, 0u, 0u, 0u};
+                    h->h_rb_sn.p[nsn++] = ck_sn_chunk{(long long)(pos + CK_RB_HEADER), nb, 0u, 0u, 0u};
                 }
                 bound = r < 0 ? 0 : o;
                 has_sn = true;
@@ -861,9 +806,9 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
                 if (ck_gz_member(z, end - pos - CK_RB_HEADER, &hdr, &isize) && CK_RB_HEADER + (unsigned long long)isize <= 0x7fffffffull) bound = isize;
                 has_gz = true;
             }
-            h->h_rb_doff[nb] = (long long)dbytes;
+            h->h_rb_dec_off.p[nb] = (long long)dbytes;
             dbytes += bound;
-        } else if (lz) h->h_rb_doff[nb] = (long long)dbytes;
+        } else if (decoded) h->h_rb_dec_off.p[nb] = (long long)dbytes;
         boff[nb] = (long long)pos; rbase[nb] = (u32)total; nb++;
         total += cnt; pos = end;
     }
@@ -871,53 +816,48 @@ extern "C" int ck_submit_recordbatch(ck_handle* h, const uint8_t* host_buf, uint
     if (hide && h->rb_hide.size() != nb) return fail(h, "ck_submit_recordbatch: the mask of ck_set_fetch_hidden does not cover the fetch's batches");
     u32 n = (u32)total;
     if (n_records) *n_records = n;
-    u8* buf = h->d_in;
+    u8* buf = h->d_in.p;
     uint64_t base = 0, used = pos;
-    if (lz) {                                          // slots in value-offset space: behind the raw bytes, 16-byte aligned
+    if (decoded) {                                     // slots in value-offset space: behind the raw bytes, 16-byte aligned
         base = (pos + 15) & ~15ull; used = base + dbytes;
-        for (u32 b = 0; b < nb; b++) h->h_rb_doff[b] += (long long)base;
-        h->h_rb_doff[nb] = (long long)used;
-        if (used > h->rb_fetch_cap && rb_fetch_grow(h, used + used / 8 + 4096)) return 1;
-        buf = h->d_rb_fetch;
+        for (u32 b = 0; b < nb; b++) h->h_rb_dec_off.p[b] += (long long)base;
+        h->h_rb_dec_off.p[nb] = (long long)used;
+        // the fetch buffer, grown as fr_grow grows the frame buffer
+        if (used + CK_PAD > h->d_rb_fetch.cap) CUDA_TRY(h, h->d_rb_fetch.reserve(used + used / 8 + 4096 + CK_PAD, h->stream));
+        buf = h->d_rb_fetch.p;
     }
     CUDA_TRY(h, cudaMemcpyAsync(buf, host_buf, pos, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(buf + pos, 0, lz ? used - pos + 16 : 16, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
-    if (lz) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_dec_off, h->h_rb_doff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(buf + pos, 0, decoded ? used - pos + 16 : 16, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_batch_off.p, boff, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_rec_base.p, rbase, sizeof(u32) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    if (decoded) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_dec_off.p, h->h_rb_dec_off.p, sizeof(long long) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
     if (nsn) {
-        if (nsn > h->rb_sn_dcap) {                     // the last fetch's decode may still read the table: wait for it once
-            CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-            if (h->d_rb_sn) cudaFree(h->d_rb_sn);
-            h->d_rb_sn = nullptr; h->rb_sn_dcap = 0;
-            CUDA_TRY(h, cudaMalloc((void**)&h->d_rb_sn, sizeof(ck_sn_chunk) * h->rb_sn_cap));
-            h->rb_sn_dcap = h->rb_sn_cap;
-        }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_sn, h->h_rb_sn, sizeof(ck_sn_chunk) * nsn, cudaMemcpyHostToDevice, h->stream));
+        CUDA_TRY(h, h->d_rb_sn.reserve(h->h_rb_sn.cap, h->stream));   // the size of the staging
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_sn.p, h->h_rb_sn.p, sizeof(ck_sn_chunk) * nsn, cudaMemcpyHostToDevice, h->stream));
     }
-    if (flagged) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_flag, h->h_rb_flag, sizeof(u32) * nb, cudaMemcpyHostToDevice, h->stream));
+    if (flagged) CUDA_TRY(h, cudaMemcpyAsync(h->d_rb_flag.p, h->h_rb_flag.p, sizeof(u32) * nb, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaEventRecord(h->rb_ev, h->stream));
-    h->rb_n = n; h->rb_dec_base = lz ? base : 0; h->rb_dec_bytes = lz ? dbytes : 0;
+    h->rb_n = n; h->rb_dec_base = decoded ? base : 0; h->rb_dec_bytes = decoded ? dbytes : 0;
     if (nb) {
         KTimer t(h, CK_K_WALK);
-        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, flagged ? h->d_rb_flag : nullptr, nb, h->d_rb_batch_bad);
-        if (has_lz4) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb, h->d_rb_batch_bad, h->d_rb_dec_len);
-        if (has_gz) CKL(h) ck_rb_gzip_kernel<<<(nb + CK_GZ_WARPS - 1) / CK_GZ_WARPS, 32 * CK_GZ_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
-                                                                                                          h->d_rb_batch_bad, h->d_rb_dec_len);
-        if (has_zs) CKL(h) ck_rb_zstd_kernel<<<(nb + CK_ZS_WARPS - 1) / CK_ZS_WARPS, 32 * CK_ZS_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off, h->d_rb_dec_off, nb,
-                                                                                                          h->d_rb_batch_bad, h->d_rb_dec_len);
-        if (has_sn) CKL(h) ck_rb_snappy_kernel<<<(nsn + CK_SN_WARPS - 1) / CK_SN_WARPS, 32 * CK_SN_WARPS, 0, h->stream>>>(buf, h->d_rb_sn, nsn, h->d_rb_dec_off,
-                                                                                                              h->d_rb_batch_bad, h->d_rb_dec_len);
-        CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off, lz ? h->d_rb_dec_off : nullptr,
-                                                                        lz ? h->d_rb_dec_len : nullptr, h->d_rb_rec_base, nb,
-                                                                        h->d_rb_batch_bad, h->d_rb_rec_pos, h->d_rb_rec_batch);
-        if (n) CKL(h) ck_rb_fields_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(buf, (long long)used, h->d_rb_rec_pos, h->d_rb_rec_batch, h->d_rb_batch_bad, n,
-            h->d_in_off, h->d_rb_val_len, h->d_rb_key_off, h->d_rb_key_len, h->d_rb_corr_off, h->d_rb_corr_len, h->d_rb_rec_bad);
+        CKL(h) ck_rb_crc_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off.p, flagged ? h->d_rb_flag.p : nullptr, nb, h->d_rb_batch_bad.p);
+        if (has_lz4) CKL(h) ck_rb_lz4_kernel<<<(nb + 7) / 8, 256, 0, h->stream>>>(buf, h->d_rb_batch_off.p, h->d_rb_dec_off.p, nb, h->d_rb_batch_bad.p, h->d_rb_dec_len.p);
+        if (has_gz) CKL(h) ck_rb_gzip_kernel<<<(nb + CK_GZ_WARPS - 1) / CK_GZ_WARPS, 32 * CK_GZ_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off.p, h->d_rb_dec_off.p, nb,
+                                                                                                          h->d_rb_batch_bad.p, h->d_rb_dec_len.p);
+        if (has_zs) CKL(h) ck_rb_zstd_kernel<<<(nb + CK_ZS_WARPS - 1) / CK_ZS_WARPS, 32 * CK_ZS_WARPS, 0, h->stream>>>(buf, h->d_rb_batch_off.p, h->d_rb_dec_off.p, nb,
+                                                                                                          h->d_rb_batch_bad.p, h->d_rb_dec_len.p);
+        if (has_sn) CKL(h) ck_rb_snappy_kernel<<<(nsn + CK_SN_WARPS - 1) / CK_SN_WARPS, 32 * CK_SN_WARPS, 0, h->stream>>>(buf, h->d_rb_sn.p, nsn, h->d_rb_dec_off.p,
+                                                                                                              h->d_rb_batch_bad.p, h->d_rb_dec_len.p);
+        CKL(h) ck_rb_split_kernel<<<(nb + 127) / 128, 128, 0, h->stream>>>(buf, h->d_rb_batch_off.p, decoded ? h->d_rb_dec_off.p : nullptr,
+                                                                        decoded ? h->d_rb_dec_len.p : nullptr, h->d_rb_rec_base.p, nb,
+                                                                        h->d_rb_batch_bad.p, h->d_rb_rec_pos.p, h->d_rb_rec_batch.p);
+        if (n) CKL(h) ck_rb_fields_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(buf, (long long)used, h->d_rb_rec_pos.p, h->d_rb_rec_batch.p, h->d_rb_batch_bad.p, n,
+            h->d_in_off.p, h->d_rb_val_len.p, h->d_rb_key_off.p, h->d_rb_key_len.p, h->d_rb_corr_off.p, h->d_rb_corr_len.p, h->d_rb_rec_bad.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    h->cur_in = buf; h->cur_in_off = h->d_in_off; h->cur_len = h->d_rb_val_len; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
+    h->cur_in = buf; h->cur_in_off = h->d_in_off.p; h->cur_len = h->d_rb_val_len.p; h->n = n; h->n_payloads = 0; h->n_pubs = 0;
     if (launch_decode(h)) return 1;
-    if (n) { CKL(h) ck_rb_mark_bad_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_rb_rec_bad, n, h->d_cols, n); CUDA_TRY(h, cudaGetLastError()); }
+    if (n) { CKL(h) ck_rb_mark_bad_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_rb_rec_bad.p, n, h->d_cols.p, n); CUDA_TRY(h, cudaGetLastError()); }
     return 0;
 }
 
@@ -976,13 +916,13 @@ static int fetch_rb_index_impl(ck_handle* h, int64_t* val_off, uint32_t* val_len
     cudaSetDevice(h->device);
     u32 n = h->rb_n;
     if (!n) return 0;
-    if (val_off) CUDA_TRY(h, cudaMemcpyAsync(val_off, h->d_in_off, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (val_len) CUDA_TRY(h, cudaMemcpyAsync(val_len, h->d_rb_val_len, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (key_off) CUDA_TRY(h, cudaMemcpyAsync(key_off, h->d_rb_key_off, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (key_len) CUDA_TRY(h, cudaMemcpyAsync(key_len, h->d_rb_key_len, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (corr_off) CUDA_TRY(h, cudaMemcpyAsync(corr_off, h->d_rb_corr_off, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (corr_len) CUDA_TRY(h, cudaMemcpyAsync(corr_len, h->d_rb_corr_len, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
-    if (bad) CUDA_TRY(h, cudaMemcpyAsync(bad, h->d_rb_rec_bad, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (val_off) CUDA_TRY(h, cudaMemcpyAsync(val_off, h->d_in_off.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (val_len) CUDA_TRY(h, cudaMemcpyAsync(val_len, h->d_rb_val_len.p, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (key_off) CUDA_TRY(h, cudaMemcpyAsync(key_off, h->d_rb_key_off.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (key_len) CUDA_TRY(h, cudaMemcpyAsync(key_len, h->d_rb_key_len.p, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (corr_off) CUDA_TRY(h, cudaMemcpyAsync(corr_off, h->d_rb_corr_off.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (corr_len) CUDA_TRY(h, cudaMemcpyAsync(corr_len, h->d_rb_corr_len.p, sizeof(int) * n, cudaMemcpyDeviceToHost, h->stream));
+    if (bad) CUDA_TRY(h, cudaMemcpyAsync(bad, h->d_rb_rec_bad.p, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
     if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -995,60 +935,57 @@ extern "C" int ck_fetch_rb_decoded_async(ck_handle* h, uint8_t* dst, uint64_t ca
     if (nbytes) *nbytes = h->rb_dec_bytes;
     if (!dst || !h->rb_dec_bytes) return 0;
     if (cap < h->rb_dec_bytes) return fail(h, "ck_fetch_rb_decoded_async: host buffer too small");
-    CUDA_TRY(h, cudaMemcpyAsync(dst, h->d_rb_fetch + h->rb_dec_base, h->rb_dec_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(dst, h->d_rb_fetch.p + h->rb_dec_base, h->rb_dec_bytes, cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 
 // ---- frame pass: the publishes of a step (or host-produced records) as RecordBatch v2 frames (csrc/ck_kafka.cuh) -------
 static int fr_grow(ck_handle* h, uint64_t cap) {
-    if (h->d_fr_frames) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_fr_frames); cudaFree(h->d_fr_partial); }
-    h->d_fr_frames = nullptr; h->d_fr_partial = nullptr; h->fr_cap = 0;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_frames, cap + CK_PAD));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_partial, sizeof(u32) * (cap / CK_RB_CRC_CHUNK + (size_t)h->max_pubs + 2)));
+    h->fr_cap = 0;
+    CUDA_TRY(h, h->d_fr_frames.reserve(cap + CK_PAD, h->stream));
+    CUDA_TRY(h, h->d_fr_partial.reserve(cap / CK_RB_CRC_CHUNK + (size_t)h->max_pubs + 2, h->stream));
     h->fr_cap = cap;
     return 0;
 }
 // the scratch of the LZ4 stage, sized for uncompressed frames of `cap` bytes: those frames, the block slots (a block's
 // compressed bytes lie at its own offset, and are never longer), and a size per 64 KB block slot
 static int lz_grow(ck_handle* h, uint64_t cap) {
-    if (h->d_fr_raw) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_fr_raw); cudaFree(h->d_fr_bsize); cudaFree(h->d_fr_bscan); cudaFree(h->d_fr_btile); }
-    h->d_fr_raw = nullptr; h->d_fr_bsize = nullptr; h->d_fr_bscan = nullptr; h->d_fr_btile = nullptr; h->fr_raw_cap = 0;
+    h->fr_raw_cap = 0;
     uint64_t bmax = cap / CK_LZ_BLOCK + (uint64_t)h->fr_max + 2;
     if (bmax > 0xffffffffull) return fail(h, "lz_grow: more than 2^32 LZ4 blocks");
-    if (!h->d_fr_zoff) CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_zoff, sizeof(long long) * ((size_t)h->fr_max + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_raw, 2 * (cap + CK_PAD)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_bsize, sizeof(u32) * bmax));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_bscan, sizeof(long long) * (bmax + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_btile, sizeof(unsigned long long) * (bmax / CK_SCAN_TILE + 2)));
+    CUDA_TRY(h, h->d_fr_zoff.reserve((size_t)h->fr_max + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_raw.reserve(2 * (cap + CK_PAD), h->stream));
+    CUDA_TRY(h, h->d_fr_bsize.reserve(bmax, h->stream));
+    CUDA_TRY(h, h->d_fr_bscan.reserve(bmax + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_btile.reserve(bmax / CK_SCAN_TILE + 2, h->stream));
     h->fr_raw_cap = cap; h->fr_bmax = (u32)bmax;
     return 0;
 }
 static int fr_alloc(ck_handle* h) {
-    if (h->d_fr_items) return 0;
     size_t m = (size_t)h->max_pubs;
     h->fr_max = h->max_pubs;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_items, sizeof(ck_fitem) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gkey, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_idx, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_head, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_fstart, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gfirst, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_ffirst, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_size, sizeof(u32) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_nlive, sizeof(u32)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_gscan, sizeof(long long) * (m + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_S, sizeof(long long) * (m + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_F, sizeof(long long) * (m + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_R, sizeof(long long) * (m + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_tile, sizeof(unsigned long long) * (m / CK_SCAN_TILE + 2)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_grand, sizeof(unsigned long long)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_table, sizeof(ck_frame_ent) * m));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o1, sizeof(u32) * (m + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_o2, sizeof(u32) * (m + 1)));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_fr_info, sizeof(long long) * 3));
+    CUDA_TRY(h, h->d_fr_items.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_gkey.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_idx.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_head.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_fstart.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_gfirst.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_ffirst.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_size.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_nlive.reserve(1, h->stream));
+    CUDA_TRY(h, h->d_fr_gscan.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_S.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_F.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_R.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_tile.reserve(m / CK_SCAN_TILE + 2, h->stream));
+    CUDA_TRY(h, h->d_fr_grand.reserve(1, h->stream));
+    CUDA_TRY(h, h->d_fr_table.reserve(m, h->stream));
+    CUDA_TRY(h, h->d_fr_o1.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->d_fr_o2.reserve(m + 1, h->stream));
+    CUDA_TRY(h, h->h_fr_info.reserve(3, h->stream));
     // first size of the frame buffer: every payload framed twice (a payload slot carries at most two publishes) plus the
     // record and frame overhead of a publish with an id of up to 40 bytes.  A pass that needs more grows it (ck_frames_size)
-    return fr_grow(h, 2 * h->max_out + 160ull * m + 4096);
+    return h->fr_cap ? 0 : fr_grow(h, 2 * h->max_out + 160ull * m + 4096);
 }
 
 // group -> split -> size -> table + headers -> write -> CRC over items[0..n) that a source kernel built (gkey: group keys of
@@ -1058,47 +995,47 @@ static int lz_compress(ck_handle* h);
 static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long long window, long long base_offset, long long ts) {
     h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec; h->fr_prod = h->prod;
     if (!n) return 0;
-    if (h->fr_pass_codec && !h->d_fr_raw && lz_grow(h, h->fr_cap)) return 1;
+    if (h->fr_pass_codec && !h->fr_raw_cap && lz_grow(h, h->fr_cap)) return 1;
     const u32* order = nullptr;
     if (passes) {
         if (group_alloc(h)) return 1;
-        ck_key_arr kf; kf.k = h->d_fr_gkey;
-        if (group_sort(h, kf, n, CK_K_FRAME, passes, nullptr, &order, h->d_fr_o1, h->d_fr_o2)) return 1;
+        ck_key_arr kf; kf.k = h->d_fr_gkey.p;
+        if (group_sort(h, kf, n, CK_K_FRAME, passes, nullptr, &order, h->d_fr_o1.p, h->d_fr_o2.p)) return 1;
     }
     h->fr_order = order; h->fr_base = base_offset; h->fr_ts = ts;
     u32 nb = (n + 255) / 256;
-    unsigned long long* tile = h->d_fr_tile; unsigned long long* grand = h->d_fr_grand;
+    unsigned long long* tile = h->d_fr_tile.p; unsigned long long* grand = h->d_fr_grand.p;
     {
         KTimer t(h, CK_K_FRAME);
-        CUDA_TRY(h, cudaMemsetAsync(h->d_fr_nlive, 0, sizeof(u32), h->stream));
-        CKL(h) ck_fr_heads_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_gkey, n, excl, h->d_fr_head, h->d_fr_nlive);
+        CUDA_TRY(h, cudaMemsetAsync(h->d_fr_nlive.p, 0, sizeof(u32), h->stream));
+        CKL(h) ck_fr_heads_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_gkey.p, n, excl, h->d_fr_head.p, h->d_fr_nlive.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_head, n, h->d_fr_gscan, 0, tile, grand, CK_K_FRAME)) return 1;
+    if (run_scan(h, h->d_fr_head.p, n, h->d_fr_gscan.p, 0, tile, grand, CK_K_FRAME)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
-        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head, h->d_fr_gscan, n, h->d_fr_gfirst);
-        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_head, h->d_fr_gscan, h->d_fr_gfirst, n, h->d_fr_nlive, h->d_fr_size);
+        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head.p, h->d_fr_gscan.p, n, h->d_fr_gfirst.p);
+        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items.p, h->d_fr_head.p, h->d_fr_gscan.p, h->d_fr_gfirst.p, n, h->d_fr_nlive.p, h->d_fr_size.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_size, n, h->d_fr_S, 0, tile, grand, CK_K_FRAME)) return 1;
+    if (run_scan(h, h->d_fr_size.p, n, h->d_fr_S.p, 0, tile, grand, CK_K_FRAME)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
-        CKL(h) ck_fr_split_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head, h->d_fr_gscan, h->d_fr_gfirst, h->d_fr_S, n, h->d_fr_nlive, window, h->d_fr_fstart);
+        CKL(h) ck_fr_split_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_head.p, h->d_fr_gscan.p, h->d_fr_gfirst.p, h->d_fr_S.p, n, h->d_fr_nlive.p, window, h->d_fr_fstart.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_fstart, n, h->d_fr_F, 0, tile, grand, CK_K_FRAME)) return 1;
+    if (run_scan(h, h->d_fr_fstart.p, n, h->d_fr_F.p, 0, tile, grand, CK_K_FRAME)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
-        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_fstart, h->d_fr_F, n, h->d_fr_ffirst);
-        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_fstart, h->d_fr_F, h->d_fr_ffirst, n, h->d_fr_nlive, h->d_fr_size);
+        CKL(h) ck_fr_first_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_fstart.p, h->d_fr_F.p, n, h->d_fr_ffirst.p);
+        CKL(h) ck_fr_size_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items.p, h->d_fr_fstart.p, h->d_fr_F.p, h->d_fr_ffirst.p, n, h->d_fr_nlive.p, h->d_fr_size.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_size, n, h->d_fr_R, 0, tile, grand, CK_K_FRAME)) return 1;
+    if (run_scan(h, h->d_fr_size.p, n, h->d_fr_R.p, 0, tile, grand, CK_K_FRAME)) return 1;
     if (frame_write(h)) return 1;
     // frames and bytes, copied back with the step's results (ck_frames_size reads them)
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info, h->d_fr_F + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info + 1, h->d_fr_R + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info.p, h->d_fr_F.p + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info.p + 1, h->d_fr_R.p + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
     h->fr_info = true;
     return 0;
 }
@@ -1110,27 +1047,27 @@ static int frame_write(ck_handle* h) {
     u32 n = h->fr_n, nb = (n + 255) / 256;
     const u32* order = h->fr_order;
     bool lz = h->fr_pass_codec != 0;
-    u8* dst = lz ? h->d_fr_raw : h->d_fr_frames;
+    u8* dst = lz ? h->d_fr_raw.p : h->d_fr_frames.p;
     uint64_t cap = lz ? h->fr_raw_cap : h->fr_cap;
     {
         KTimer t(h, CK_K_FRAME);   // chunk counts per frame go to d_fr_head (free again), their scan to d_fr_S
-        CKL(h) ck_fr_table_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_ffirst, h->d_fr_F, h->d_fr_R, n, h->d_fr_nlive,
-                                                          h->fr_base, h->fr_ts, h->fr_prod, cap, h->d_fr_table, dst, h->d_fr_head);
+        CKL(h) ck_fr_table_kernel<<<nb, 256, 0, h->stream>>>(order, h->d_fr_items.p, h->d_fr_ffirst.p, h->d_fr_F.p, h->d_fr_R.p, n, h->d_fr_nlive.p,
+                                                          h->fr_base, h->fr_ts, h->fr_prod, cap, h->d_fr_table.p, dst, h->d_fr_head.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (!lz && run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
+    if (!lz && run_scan(h, h->d_fr_head.p, n, h->d_fr_S.p, 0, h->d_fr_tile.p, h->d_fr_grand.p, CK_K_FRAME)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
-        CKL(h) ck_fr_write_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(order, h->d_fr_items, h->d_fr_fstart, h->d_fr_F, h->d_fr_ffirst, h->d_fr_R, n,
-                                                                   h->d_fr_nlive, cap, dst);
+        CKL(h) ck_fr_write_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(order, h->d_fr_items.p, h->d_fr_fstart.p, h->d_fr_F.p, h->d_fr_ffirst.p, h->d_fr_R.p, n,
+                                                                   h->d_fr_nlive.p, cap, dst);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (lz && lz_compress(h)) return 1;
     {
         KTimer t(h, CK_K_FRAME);
         u32 cblocks = (n + 7) / 8; if (cblocks > h->num_sms * 8) cblocks = h->num_sms * 8;
-        CKL(h) ck_fr_crc_chunks_kernel<<<cblocks, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_frames, h->d_fr_partial);
-        CKL(h) ck_fr_crc_fold_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_S, h->d_fr_F, n, h->d_fr_partial, h->d_fr_frames);
+        CKL(h) ck_fr_crc_chunks_kernel<<<cblocks, 256, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_S.p, h->d_fr_F.p, n, h->d_fr_frames.p, h->d_fr_partial.p);
+        CKL(h) ck_fr_crc_fold_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_S.p, h->d_fr_F.p, n, h->d_fr_partial.p, h->d_fr_frames.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     return 0;
@@ -1141,37 +1078,37 @@ static int frame_write(ck_handle* h) {
 // d_fr_gscan and frame lengths in d_fr_size: the first half of the pass is done with both
 static int lz_compress(ck_handle* h) {
     u32 n = h->fr_n, nb = (n + 255) / 256;
-    u8* slots = h->d_fr_raw + h->fr_raw_cap + CK_PAD;
+    u8* slots = h->d_fr_raw.p + h->fr_raw_cap + CK_PAD;
     {
         KTimer t(h, CK_K_LZ4);
-        CKL(h) ck_lz_blocks_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_F, n, h->fr_raw_cap, h->d_fr_head);
+        CKL(h) ck_lz_blocks_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_F.p, n, h->fr_raw_cap, h->d_fr_head.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_head, n, h->d_fr_gscan, 0, h->d_fr_tile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    if (run_scan(h, h->d_fr_head.p, n, h->d_fr_gscan.p, 0, h->d_fr_tile.p, h->d_fr_grand.p, CK_K_LZ4)) return 1;
     {
         KTimer t(h, CK_K_LZ4);
         u32 blocks = h->num_sms * 8;
-        CKL(h) ck_lz_compress_kernel<<<blocks, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table, h->d_fr_gscan, h->d_fr_F, n, h->d_fr_raw, slots,
-                                                                              h->fr_bmax, h->d_fr_bsize);
+        CKL(h) ck_lz_compress_kernel<<<blocks, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_gscan.p, h->d_fr_F.p, n, h->d_fr_raw.p, slots,
+                                                                              h->fr_bmax, h->d_fr_bsize.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_bsize, h->fr_bmax, h->d_fr_bscan, 0, h->d_fr_btile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    if (run_scan(h, h->d_fr_bsize.p, h->fr_bmax, h->d_fr_bscan.p, 0, h->d_fr_btile.p, h->d_fr_grand.p, CK_K_LZ4)) return 1;
     {
         KTimer t(h, CK_K_LZ4);
-        CKL(h) ck_lz_size_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_gscan, h->d_fr_bscan, n, h->d_fr_size);
+        CKL(h) ck_lz_size_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_gscan.p, h->d_fr_bscan.p, n, h->d_fr_size.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_size, n, h->d_fr_zoff, 0, h->d_fr_tile, h->d_fr_grand, CK_K_LZ4)) return 1;
+    if (run_scan(h, h->d_fr_size.p, n, h->d_fr_zoff.p, 0, h->d_fr_tile.p, h->d_fr_grand.p, CK_K_LZ4)) return 1;
     {
         KTimer t(h, CK_K_LZ4);
-        CKL(h) ck_lz_gather_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_gscan, h->d_fr_F, n, h->d_fr_bscan, h->d_fr_bsize,
-                                                                         h->d_fr_zoff, h->d_fr_size, h->d_fr_raw, slots, h->fr_cap, h->d_fr_frames);
-        CKL(h) ck_lz_head_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table, h->d_fr_F, n, h->d_fr_zoff, h->d_fr_size, h->d_fr_raw, h->fr_cap,
-                                                           h->d_fr_frames, h->d_fr_head);
+        CKL(h) ck_lz_gather_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_gscan.p, h->d_fr_F.p, n, h->d_fr_bscan.p, h->d_fr_bsize.p,
+                                                                         h->d_fr_zoff.p, h->d_fr_size.p, h->d_fr_raw.p, slots, h->fr_cap, h->d_fr_frames.p);
+        CKL(h) ck_lz_head_kernel<<<nb, 256, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_F.p, n, h->d_fr_zoff.p, h->d_fr_size.p, h->d_fr_raw.p, h->fr_cap,
+                                                           h->d_fr_frames.p, h->d_fr_head.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_fr_head, n, h->d_fr_S, 0, h->d_fr_tile, h->d_fr_grand, CK_K_FRAME)) return 1;
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info + 2, h->d_fr_zoff + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    if (run_scan(h, h->d_fr_head.p, n, h->d_fr_S.p, 0, h->d_fr_tile.p, h->d_fr_grand.p, CK_K_FRAME)) return 1;
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_fr_info.p + 2, h->d_fr_zoff.p + n, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 
@@ -1184,13 +1121,13 @@ extern "C" int ck_set_frame_topics(ck_handle* h, const int32_t* topic_ids, uint3
     for (u32 i = 0; i < n; i++) { if (topic_ids[i] < 0) return fail(h, "ck_set_frame_topics: ids must be >= 0"); if (topic_ids[i] > top) top = topic_ids[i]; }
     std::vector<int32_t> slot((size_t)top + 1, -1);
     for (u32 i = 0; i < n; i++) if (slot[topic_ids[i]] < 0) slot[topic_ids[i]] = (int32_t)i;
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (h->d_fr_slot) { cudaFree(h->d_fr_slot); h->d_fr_slot = nullptr; }
-    h->fr_nslots = (u32)slot.size(); h->fr_ntopics = n;
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));    // the passes queued so far may read the old table
+    ck_buf<int32_t> d_slot;
     if (n) {
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_slot, sizeof(int32_t) * slot.size()));
-        CUDA_TRY(h, cudaMemcpy(h->d_fr_slot, slot.data(), sizeof(int32_t) * slot.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(h, d_slot.reserve(slot.size(), h->stream));
+        CUDA_TRY(h, cudaMemcpy(d_slot.p, slot.data(), sizeof(int32_t) * slot.size(), cudaMemcpyHostToDevice));
     }
+    h->d_fr_slot = std::move(d_slot); h->fr_nslots = (u32)slot.size(); h->fr_ntopics = n;
     return 0;
 }
 
@@ -1205,9 +1142,9 @@ extern "C" int ck_encode_frames(ck_handle* h, int64_t timestamp_ms) {
     u32 n = h->n_pubs, excl = (u32)((1ull << (6 * passes)) - 1);
     {
         KTimer t(h, CK_K_FRAME);
-        if (n) CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, nullptr, n, h->d_pay_len, h->d_out_off, h->d_out,
-            h->d_cols, h->n, h->d_fr_slot, h->fr_nslots, h->num_partitions, excl, h->fr_sticky.empty() ? nullptr : h->d_fr_sticky,
-            (u32)h->fr_sticky.size(), h->d_fr_items, h->d_fr_gkey);
+        if (n) CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs.p, nullptr, n, h->d_pay_len.p, h->d_out_off.p, h->d_out.p,
+            h->d_cols.p, h->n, h->d_fr_slot.p, h->fr_nslots, h->num_partitions, excl, h->fr_sticky.empty() ? nullptr : h->d_fr_sticky.p,
+            (u32)h->fr_sticky.size(), h->d_fr_items.p, h->d_fr_gkey.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     return frame_pass(h, n, passes, excl, h->fr_window, 0, timestamp_ms);
@@ -1230,14 +1167,15 @@ extern "C" int ck_set_sticky_partitions(ck_handle* h, const int32_t* parts, uint
     for (u32 i = 0; i < n; i++)
         if (parts[i] < -1 || (parts[i] >= 0 && (u32)parts[i] >= h->num_partitions))
             return fail(h, "ck_set_sticky_partitions: a partition outside [0, num_partitions)");
-    if (n > h->fr_sticky_cap) {
-        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-        if (h->d_fr_sticky) { cudaFree(h->d_fr_sticky); h->d_fr_sticky = nullptr; }
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_sticky, sizeof(int32_t) * n));
-        h->fr_sticky_cap = n;
+    std::vector<int32_t> host(parts, parts + n);
+    ck_buf<int32_t> grown;                             // a larger table replaces the old one once its copy is queued
+    if (n > h->d_fr_sticky.cap) {
+        CUDA_TRY(h, cudaStreamSynchronize(h->stream));    // the passes queued so far may read the old table
+        CUDA_TRY(h, grown.reserve(n, h->stream));
     }
-    h->fr_sticky.assign(parts, parts + n);
-    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_sticky, h->fr_sticky.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    if (n) CUDA_TRY(h, cudaMemcpyAsync(grown.p ? grown.p : h->d_fr_sticky.p, host.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+    if (grown.p) h->d_fr_sticky = std::move(grown);
+    h->fr_sticky = std::move(host);
     return 0;
 }
 
@@ -1257,26 +1195,24 @@ extern "C" int ck_encode_frames_records(ck_handle* h, int32_t topic_id, const ui
     u32 passes = fr_passes((unsigned long long)h->num_partitions + 1);
     if (passes > 5) return fail(h, "ck_encode_frames_records: too many partitions");
     if (fr_alloc(h)) return 1;
-    if (!h->d_fr_blob) {
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_blob, h->max_in + CK_PAD));
-        CUDA_TRY(h, cudaMalloc((void**)&h->d_fr_desc, sizeof(long long) * 6 * (size_t)h->max_pubs));
-    }
-    if (nbytes) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_blob, host_blob, nbytes, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_fr_blob + nbytes, 0, 16, h->stream));
-    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_desc, host_desc, sizeof(long long) * 6 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, h->d_fr_blob.reserve(h->max_in + CK_PAD, h->stream));
+    CUDA_TRY(h, h->d_fr_desc.reserve(6 * (size_t)h->max_pubs, h->stream));
+    if (nbytes) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_blob.p, host_blob, nbytes, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_fr_blob.p + nbytes, 0, 16, h->stream));
+    if (n) CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_desc.p, host_desc, sizeof(long long) * 6 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
     {
         KTimer t(h, CK_K_FRAME);
         int32_t sticky = topic_id >= 0 && (size_t)topic_id < h->fr_sticky.size() ? h->fr_sticky[topic_id] : -1;
-        if (n) CKL(h) ck_fr_src_recs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_fr_blob, h->d_fr_desc, n, topic_id, h->num_partitions,
-                                                                                   sticky, h->d_fr_items, h->d_fr_gkey);
+        if (n) CKL(h) ck_fr_src_recs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_fr_blob.p, h->d_fr_desc.p, n, topic_id, h->num_partitions,
+                                                                                   sticky, h->d_fr_items.p, h->d_fr_gkey.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     return frame_pass(h, n, passes, (u32)((1ull << (6 * passes)) - 1), h->fr_window, 0, timestamp_ms);
 }
 
 // bytes of the last pass's frames: uncompressed (as the table kernel lays them out) and as they go out
-static uint64_t fr_raw_bytes(ck_handle* h) { return h->fr_info ? (uint64_t)(h->h_fr_info[1] + (long long)CK_RB_HEADER * h->h_fr_info[0]) : 0; }
-static uint64_t fr_bytes(ck_handle* h) { return !h->fr_info ? 0 : h->fr_pass_codec ? (uint64_t)h->h_fr_info[2] : fr_raw_bytes(h); }
+static uint64_t fr_raw_bytes(ck_handle* h) { return h->fr_info ? (uint64_t)(h->h_fr_info.p[1] + (long long)CK_RB_HEADER * h->h_fr_info.p[0]) : 0; }
+static uint64_t fr_bytes(ck_handle* h) { return !h->fr_info ? 0 : h->fr_pass_codec ? (uint64_t)h->h_fr_info.p[2] : fr_raw_bytes(h); }
 
 // frames and bytes of the last pass (waits for it).  Frames that did not fit the frame buffer (or, compressed, the scratch
 // buffer of the uncompressed frames) are written again into buffers grown to their size (one more wait each): a step is
@@ -1294,7 +1230,7 @@ extern "C" int ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     }
     h->fr_sized = true;
-    if (n_frames) *n_frames = h->fr_info ? (u32)h->h_fr_info[0] : 0u;
+    if (n_frames) *n_frames = h->fr_info ? (u32)h->h_fr_info.p[0] : 0u;
     if (nbytes) *nbytes = fr_bytes(h);
     return 0;
 }
@@ -1304,11 +1240,11 @@ extern "C" int ck_frames_size(ck_handle* h, uint32_t* n_frames, uint64_t* nbytes
 extern "C" int ck_fetch_frames_async(ck_handle* h, ck_frame* host_table, uint32_t table_cap, uint8_t* host_frames, uint64_t cap) {
     cudaSetDevice(h->device);
     if (h->fr_info && !h->fr_sized) return fail(h, "ck_fetch_frames_async: call ck_frames_size after the frame pass first");
-    uint64_t nf = h->fr_info ? (uint64_t)h->h_fr_info[0] : 0, nb = fr_bytes(h);
+    uint64_t nf = h->fr_info ? (uint64_t)h->h_fr_info.p[0] : 0, nb = fr_bytes(h);
     if (nb > h->fr_cap) return fail(h, "ck_fetch_frames_async: frames larger than the frame buffer");
     if (nf > table_cap || nb > cap) return fail(h, "ck_fetch_frames_async: host buffers too small");
-    if (nf) CUDA_TRY(h, cudaMemcpyAsync(host_table, h->d_fr_table, sizeof(ck_frame) * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
-    if (nb) CUDA_TRY(h, cudaMemcpyAsync(host_frames, h->d_fr_frames, (size_t)nb, cudaMemcpyDeviceToHost, h->stream));
+    if (nf) CUDA_TRY(h, cudaMemcpyAsync(host_table, h->d_fr_table.p, sizeof(ck_frame) * (size_t)nf, cudaMemcpyDeviceToHost, h->stream));
+    if (nb) CUDA_TRY(h, cudaMemcpyAsync(host_frames, h->d_fr_frames.p, (size_t)nb, cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 
@@ -1319,11 +1255,11 @@ extern "C" int ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uin
     cudaSetDevice(h->device);
     if (!n || n > h->n_pubs) return fail(h, "ck_encode_recordbatch: index list empty or longer than the publish table");
     if (fr_alloc(h)) return 1;
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_idx, host_idx, sizeof(u32) * n, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_fr_idx.p, host_idx, sizeof(u32) * n, cudaMemcpyHostToDevice, h->stream));
     {
         KTimer t(h, CK_K_FRAME);
-        CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs, h->d_fr_idx, n, h->d_pay_len, h->d_out_off, h->d_out,
-            h->d_cols, h->n, nullptr, 0, 0, CK_RB_NONE, nullptr, 0, h->d_fr_items, h->d_fr_gkey);
+        CKL(h) ck_fr_src_pubs_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(view_of(h), h->d_pubs.p, h->d_fr_idx.p, n, h->d_pay_len.p, h->d_out_off.p, h->d_out.p,
+            h->d_cols.p, h->n, nullptr, 0, 0, CK_RB_NONE, nullptr, 0, h->d_fr_items.p, h->d_fr_gkey.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (frame_pass(h, n, 0, CK_RB_NONE, ~0ull, base_offset, timestamp_ms)) return 1;
@@ -1331,7 +1267,7 @@ extern "C" int ck_encode_recordbatch(ck_handle* h, const uint32_t* host_idx, uin
     if (ck_frames_size(h, &nf, &total)) return 1;
     if (nf != 1) return fail(h, "ck_encode_recordbatch: the index list holds no live publish");
     if (total > cap) return fail(h, "ck_encode_recordbatch: host buffer too small");
-    CUDA_TRY(h, cudaMemcpyAsync(host_frame, h->d_fr_frames, total, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_frame, h->d_fr_frames.p, total, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (frame_len) *frame_len = total;
     return 0;
@@ -1343,26 +1279,27 @@ extern "C" int ck_gate_create(ck_handle* h, uint32_t max_entries, uint32_t max_s
     if (h->gate_set) return fail(h, "ck_gate_create: already created");
     if (arena_bytes >= (1ull << 32)) return fail(h, "ck_gate_create: arena must be smaller than 4 GiB (32-bit segment offsets)");
     if (max_entries == 0 || max_entries > (1u << 28)) return fail(h, "ck_gate_create: max_entries must be in [1, 2^28]");
-    ck_gate g{};
     u32 cap = 64; while (cap < 4 * (uint64_t)max_entries) cap <<= 1;
-    g.cap = cap; g.max_entries = max_entries; g.max_slots = max_slots; g.arena_cap = arena_bytes;
-    ck_gate s = g;
-    CUDA_TRY(h, cudaMalloc((void**)&g.keys, sizeof(unsigned long long) * cap));
-    CUDA_TRY(h, cudaMalloc((void**)&g.entries, sizeof(ck_gate_entry) * (size_t)max_entries));
-    CUDA_TRY(h, cudaMalloc((void**)&g.slots, sizeof(ck_gate_slot) * (size_t)max_slots));
-    CUDA_TRY(h, cudaMalloc((void**)&g.arena, arena_bytes + CK_PAD));
-    CUDA_TRY(h, cudaMalloc((void**)&g.ctr, sizeof(unsigned long long) * 8));
-    // the second set of buffers for ck_gate_compact: the gate holds twice the entries, slots and arena it is sized for
-    CUDA_TRY(h, cudaMalloc((void**)&s.entries, sizeof(ck_gate_entry) * (size_t)max_entries));
-    CUDA_TRY(h, cudaMalloc((void**)&s.slots, sizeof(ck_gate_slot) * (size_t)max_slots));
-    CUDA_TRY(h, cudaMalloc((void**)&s.arena, arena_bytes + CK_PAD));
-    s.keys = g.keys; s.ctr = g.ctr;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_gate_src, sizeof(u32) * (size_t)max_entries));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_rec_entry, sizeof(u32) * (size_t)h->max_records));
-    CUDA_TRY(h, cudaMemsetAsync(g.keys, 0, sizeof(unsigned long long) * cap, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(g.ctr, 0, sizeof(unsigned long long) * 8, h->stream));
+    ck_gate_bufs b;
+    CUDA_TRY(h, b.keys.reserve(cap, h->stream));
+    CUDA_TRY(h, b.ctr.reserve(8, h->stream));
+    // two sets of entries, slots and arena for ck_gate_compact: the gate holds twice what it is sized for
+    for (int k = 0; k < 2; k++) {
+        CUDA_TRY(h, b.entries[k].reserve((size_t)max_entries, h->stream));
+        CUDA_TRY(h, b.slots[k].reserve((size_t)max_slots, h->stream));
+        CUDA_TRY(h, b.arena[k].reserve(arena_bytes + CK_PAD, h->stream));
+    }
+    CUDA_TRY(h, b.src.reserve((size_t)max_entries, h->stream));
+    CUDA_TRY(h, b.rec_entry.reserve((size_t)h->max_records, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(b.keys.p, 0, sizeof(unsigned long long) * cap, h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(b.ctr.p, 0, sizeof(unsigned long long) * 8, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    h->gate = g; h->gate_spare = s; h->gate_set = true;
+    ck_gate g{};
+    g.keys = b.keys.p; g.cap = cap; g.max_entries = max_entries; g.max_slots = max_slots; g.arena_cap = arena_bytes; g.ctr = b.ctr.p;
+    ck_gate s = g;
+    g.entries = b.entries[0].p; g.slots = b.slots[0].p; g.arena = b.arena[0].p;
+    s.entries = b.entries[1].p; s.slots = b.slots[1].p; s.arena = b.arena[1].p;
+    h->gate_bufs = std::move(b); h->gate = g; h->gate_spare = s; h->gate_set = true;
     return 0;
 }
 
@@ -1382,8 +1319,8 @@ extern "C" int ck_gate_compact(ck_handle* h) {
     if (!h->gate_set) return fail(h, "ck_gate_compact: call ck_gate_create first");
     ck_gate g = h->gate, d = h->gate_spare;
     CUDA_TRY(h, cudaMemsetAsync(g.keys, 0, sizeof(unsigned long long) * g.cap, h->stream));
-    CKL(h) ck_gate_compact_plan_kernel<<<1, 1024, 0, h->stream>>>(g, d, h->d_gate_src);
-    CKL(h) ck_gate_compact_move_kernel<<<(g.max_entries + 7) / 8, 256, 0, h->stream>>>(g, d, h->d_gate_src);
+    CKL(h) ck_gate_compact_plan_kernel<<<1, 1024, 0, h->stream>>>(g, d, h->gate_bufs.src.p);
+    CKL(h) ck_gate_compact_move_kernel<<<(g.max_entries + 7) / 8, 256, 0, h->stream>>>(g, d, h->gate_bufs.src.p);
     CUDA_TRY(h, cudaGetLastError());
     h->gate = d; h->gate_spare = g;
     return 0;
@@ -1405,10 +1342,10 @@ extern "C" int ck_gate_register(ck_handle* h, uint32_t min_pending) {
     CUDA_TRY(h, cudaMemsetAsync(h->gate.ctr + 4, 0, sizeof(unsigned long long), h->stream));   // failures of this call
     if (!n) return 0;
     KTimer t(h, CK_K_FANOUT);
-    CKL(h) ck_gate_register_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, min_pending,
-                                                                              h->gate_reg_seq, h->d_rec_entry);
+    CKL(h) ck_gate_register_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->gate, min_pending,
+                                                                              h->gate_reg_seq, h->gate_bufs.rec_entry.p);
     h->gate_reg_seq += n;
-    CKL(h) ck_gate_copy_base_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(view_of(h), n, h->gate, h->d_rec_entry);
+    CKL(h) ck_gate_copy_base_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(view_of(h), n, h->gate, h->gate_bufs.rec_entry.p);
     CUDA_TRY(h, cudaGetLastError());
     return 0;
 }
@@ -1425,10 +1362,10 @@ extern "C" int ck_gate_arrive(ck_handle* h, uint64_t stamp_base) {
     {
         KTimer t(h, CK_K_PLAN);
         if (n) {
-            CKL(h) ck_gate_probe_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, stamp_base, h->d_rec_entry);
-            CKL(h) ck_gate_resolve_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, stamp_base, h->d_rec_entry,
-                h->h_tool_cfg.publish_topic_id, h->d_glue, h->d_descs, h->d_pay_len, h->d_pubs);
-            CKL(h) ck_gate_merge_kernel<<<(n + 3) / 4, 128, 0, h->stream>>>(view_of(h), n, h->d_cols, n, h->gate, h->d_rec_entry, h->d_glue, h->d_descs, h->d_pay_len);
+            CKL(h) ck_gate_probe_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->gate, stamp_base, h->gate_bufs.rec_entry.p);
+            CKL(h) ck_gate_resolve_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->gate, stamp_base, h->gate_bufs.rec_entry.p,
+                h->h_tool_cfg.publish_topic_id, h->d_glue.p, h->d_descs.p, h->d_pay_len.p, h->d_pubs.p);
+            CKL(h) ck_gate_merge_kernel<<<(n + 3) / 4, 128, 0, h->stream>>>(view_of(h), n, h->d_cols.p, n, h->gate, h->gate_bufs.rec_entry.p, h->d_glue.p, h->d_descs.p, h->d_pay_len.p);
         }
         CUDA_TRY(h, cudaGetLastError());
     }
@@ -1439,22 +1376,21 @@ extern "C" int ck_gate_arrive(ck_handle* h, uint64_t stamp_base) {
 
 // ---- cross-partition forward over peer memory (csrc/ck_xsend.cuh) --------------------------------------------------------
 static int x_alloc(ck_handle* h) {
-    if (h->d_x_hist) return 0;
     u32 nb_max = (h->max_pubs + CK_X_BLOCK - 1) / CK_X_BLOCK;
     size_t nh = (size_t)CK_X_MAXWORLD * nb_max;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_hist, sizeof(u32) * nh));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_base, sizeof(long long) * (nh + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_nbytes, sizeof(unsigned long long) * CK_X_MAXWORLD));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_src_off, sizeof(long long) * ((size_t)h->max_pubs + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_len, sizeof(long long) * ((size_t)h->max_pubs + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_dst_off, sizeof(long long) * ((size_t)h->max_pubs + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_len32, sizeof(u32) * ((size_t)h->max_pubs + 1)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_pub, sizeof(u32) * ((size_t)h->max_pubs + 1)));
+    CUDA_TRY(h, h->d_x_hist.reserve(nh, h->stream));
+    CUDA_TRY(h, h->d_x_base.reserve(nh + 1, h->stream));
+    CUDA_TRY(h, h->d_x_nbytes.reserve(CK_X_MAXWORLD, h->stream));
+    CUDA_TRY(h, h->d_x_src_off.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_x_len.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_x_dst_off.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_x_len32.reserve((size_t)h->max_pubs + 1, h->stream));
+    CUDA_TRY(h, h->d_x_pub.reserve((size_t)h->max_pubs + 1, h->stream));
     size_t nt = (nh > h->max_pubs ? nh : h->max_pubs) / CK_SCAN_TILE + 2;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_tile, sizeof(unsigned long long) * nt));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_grand, sizeof(unsigned long long)));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_grand2, sizeof(unsigned long long)));
-    CUDA_TRY(h, cudaMallocHost((void**)&h->h_x, sizeof(long long) * (2 * CK_X_MAXWORLD + 2)));
+    CUDA_TRY(h, h->d_x_tile.reserve(nt, h->stream));
+    CUDA_TRY(h, h->d_x_grand.reserve(1, h->stream));
+    CUDA_TRY(h, h->d_x_grand2.reserve(1, h->stream));
+    CUDA_TRY(h, h->h_x.reserve(2 * CK_X_MAXWORLD + 2, h->stream));
     return 0;
 }
 
@@ -1463,34 +1399,42 @@ static int x_alloc(ck_handle* h) {
 extern "C" int ck_comm_create(ck_handle* h, uint32_t rank, uint32_t world, uint32_t max_fwd, uint64_t data_cap, uint8_t* ipc_handle_out) {
     cudaSetDevice(h->device);
     if (world < 1 || world > CK_X_MAXWORLD || rank >= world) return fail(h, "ck_comm_create: world must be 1..16 and rank < world");
-    if (h->d_recv) return fail(h, "ck_comm_create: already created");
+    if (h->d_recv.p) return fail(h, "ck_comm_create: already created");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "ipc handle size");
-    h->comm_rank = rank; h->comm_world = world; h->max_fwd = max_fwd;
-    h->region_data_cap = (data_cap + 15) & ~15ull;
-    h->region_stride = (CK_X_HDR + (unsigned long long)max_fwd * sizeof(ck_xmeta) + h->region_data_cap + 255) & ~255ull;
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_recv, h->region_stride * world + CK_X_FLAGS_BYTES + CK_PAD));
-    CUDA_TRY(h, cudaMemset(h->d_recv, 0, h->region_stride * world + CK_X_FLAGS_BYTES));
-    CUDA_TRY(h, cudaMalloc((void**)&h->d_x_overflow, sizeof(u32) * (CK_X_MAXWORLD + 1)));
-    CUDA_TRY(h, cudaMemset(h->d_x_overflow, 0, sizeof(u32) * (CK_X_MAXWORLD + 1)));     // [world]: barrier timeout flag
+    unsigned long long data = (data_cap + 15) & ~15ull;
+    unsigned long long stride = (CK_X_HDR + (unsigned long long)max_fwd * sizeof(ck_xmeta) + data + 255) & ~255ull;
+    ck_buf<u8> recv; ck_buf<u32> overflow;
+    CUDA_TRY(h, recv.reserve(stride * world + CK_X_FLAGS_BYTES + CK_PAD, h->stream));
+    CUDA_TRY(h, cudaMemset(recv.p, 0, stride * world + CK_X_FLAGS_BYTES));
+    CUDA_TRY(h, overflow.reserve(CK_X_MAXWORLD + 1, h->stream));
+    CUDA_TRY(h, cudaMemset(overflow.p, 0, sizeof(u32) * (CK_X_MAXWORLD + 1)));     // [world]: barrier timeout flag
     cudaIpcMemHandle_t ih;
-    CUDA_TRY(h, cudaIpcGetMemHandle(&ih, h->d_recv));
-    memcpy(ipc_handle_out, &ih, 64);
+    CUDA_TRY(h, cudaIpcGetMemHandle(&ih, recv.p));
     // the exchange is a dozen small dependent kernels: on a highest-priority stream their blocks are scheduled as soon as
     // any SM slot frees up instead of queueing behind the other lane's million-record kernels
     int lo = 0, hi = 0;
     CUDA_TRY(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    CUDA_TRY(h, cudaStreamCreateWithPriority(&h->xstream, cudaStreamNonBlocking, hi));
-    CUDA_TRY(h, cudaEventCreateWithFlags(&h->x_ev0, cudaEventDisableTiming));
-    CUDA_TRY(h, cudaEventCreateWithFlags(&h->x_ev1, cudaEventDisableTiming));
+    cudaStream_t xs = nullptr; cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaError_t stream_err = cudaStreamCreateWithPriority(&xs, cudaStreamNonBlocking, hi);
+    if (stream_err == cudaSuccess) stream_err = cudaEventCreateWithFlags(&ev0, cudaEventDisableTiming);
+    if (stream_err == cudaSuccess) stream_err = cudaEventCreateWithFlags(&ev1, cudaEventDisableTiming);
+    if (stream_err != cudaSuccess) {
+        if (ev0) cudaEventDestroy(ev0);
+        if (xs) cudaStreamDestroy(xs);
+        CUDA_TRY(h, stream_err);
+    }
+    memcpy(ipc_handle_out, &ih, 64);
+    h->comm_rank = rank; h->comm_world = world; h->max_fwd = max_fwd; h->region_data_cap = data; h->region_stride = stride;
+    h->d_recv = std::move(recv); h->d_x_overflow = std::move(overflow); h->xstream = xs; h->x_ev0 = ev0; h->x_ev1 = ev1;
     return 0;
 }
 
 // handles[world][64]: every rank's ck_comm_create output, in rank order (this rank's own entry is ignored)
 extern "C" int ck_comm_connect(ck_handle* h, const uint8_t* handles) {
     cudaSetDevice(h->device);
-    if (!h->d_recv) return fail(h, "ck_comm_connect: call ck_comm_create first");
+    if (!h->d_recv.p) return fail(h, "ck_comm_connect: call ck_comm_create first");
     for (u32 d = 0; d < h->comm_world; d++) {
-        if (d == h->comm_rank) { h->peers.recv[d] = h->d_recv; continue; }
+        if (d == h->comm_rank) { h->peers.recv[d] = h->d_recv.p; continue; }
         cudaIpcMemHandle_t ih; memcpy(&ih, handles + 64 * (size_t)d, 64);
         void* p = nullptr;
         CUDA_TRY(h, cudaIpcOpenMemHandle(&p, ih, cudaIpcMemLazyEnablePeerAccess));
@@ -1529,31 +1473,31 @@ static int exchange_send_on_stream(ck_handle* h, uint64_t step) {
     u32 nh = world * nb;
     {
         KTimer t(h, CK_K_ROUTE);
-        CUDA_TRY(h, cudaMemsetAsync(h->d_x_nbytes, 0, sizeof(unsigned long long) * CK_X_MAXWORLD, h->stream));
-        CKL(h) ck_xplan_count_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs, npubs, h->d_pay_len, rank, world, h->d_x_hist, h->d_x_nbytes);
+        CUDA_TRY(h, cudaMemsetAsync(h->d_x_nbytes.p, 0, sizeof(unsigned long long) * CK_X_MAXWORLD, h->stream));
+        CKL(h) ck_xplan_count_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs.p, npubs, h->d_pay_len.p, rank, world, h->d_x_hist.p, h->d_x_nbytes.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_x_hist, nh, h->d_x_base, 0, h->d_x_tile, h->d_x_grand)) return 1;       // d_x_grand = payloads selected
+    if (run_scan(h, h->d_x_hist.p, nh, h->d_x_base.p, 0, h->d_x_tile.p, h->d_x_grand.p)) return 1;       // d_x_grand = payloads selected
     {
         KTimer t(h, CK_K_ROUTE);
-        CUDA_TRY(h, cudaMemsetAsync(h->d_x_len32, 0, sizeof(u32) * ((size_t)npubs + 1), h->stream));
-        CKL(h) ck_xplan_scatter_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs, npubs, h->d_pay_len, h->d_out_off, rank, world, h->d_x_base,
-                                                                  h->d_x_src_off, h->d_x_len, h->d_x_len32, h->d_x_pub);
+        CUDA_TRY(h, cudaMemsetAsync(h->d_x_len32.p, 0, sizeof(u32) * ((size_t)npubs + 1), h->stream));
+        CKL(h) ck_xplan_scatter_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs.p, npubs, h->d_pay_len.p, h->d_out_off.p, rank, world, h->d_x_base.p,
+                                                                  h->d_x_src_off.p, h->d_x_len.p, h->d_x_len32.p, h->d_x_pub.p);
         CUDA_TRY(h, cudaGetLastError());
     }
     // byte offsets of the (16-byte padded) payloads in destination order; scanned over all publish slots so that the
     // launch does not need the selected count on the host (unselected tail entries are zero)
-    if (run_scan(h, h->d_x_len32, npubs ? npubs : 1, h->d_x_dst_off, 15, h->d_x_tile, h->d_x_grand2)) return 1;
+    if (run_scan(h, h->d_x_len32.p, npubs ? npubs : 1, h->d_x_dst_off.p, 15, h->d_x_tile.p, h->d_x_grand2.p)) return 1;
     unsigned long long flags_off = h->region_stride * world;
     {
         KTimer t(h, CK_K_EMIT);
         // barrier 1: every peer has consumed what it received last time (its own stream order puts that before this point)
-        CKL(h) ck_xbarrier_kernel<<<1, 32, 0, h->stream>>>(h->peers, rank, world, flags_off, 0, step, h->d_x_overflow + CK_X_MAXWORLD);
-        if (npubs) CKL(h) ck_xsend_kernel<<<h->num_sms * 4, 256, 0, h->stream>>>(h->d_pubs, h->d_x_pub, h->d_x_src_off, h->d_x_len32, h->d_x_dst_off, h->d_x_base, nb,
-            h->d_x_grand, h->d_out, h->peers, rank, world, h->region_stride, h->max_fwd, h->region_data_cap, h->d_x_overflow);
-        CKL(h) ck_xhdr_kernel<<<1, 32, 0, h->stream>>>(h->d_x_dst_off, h->d_x_base, nb, h->d_x_grand, h->peers, rank, world, h->region_stride, step, h->d_x_overflow);
+        CKL(h) ck_xbarrier_kernel<<<1, 32, 0, h->stream>>>(h->peers, rank, world, flags_off, 0, step, h->d_x_overflow.p + CK_X_MAXWORLD);
+        if (npubs) CKL(h) ck_xsend_kernel<<<h->num_sms * 4, 256, 0, h->stream>>>(h->d_pubs.p, h->d_x_pub.p, h->d_x_src_off.p, h->d_x_len32.p, h->d_x_dst_off.p, h->d_x_base.p, nb,
+            h->d_x_grand.p, h->d_out.p, h->peers, rank, world, h->region_stride, h->max_fwd, h->region_data_cap, h->d_x_overflow.p);
+        CKL(h) ck_xhdr_kernel<<<1, 32, 0, h->stream>>>(h->d_x_dst_off.p, h->d_x_base.p, nb, h->d_x_grand.p, h->peers, rank, world, h->region_stride, step, h->d_x_overflow.p);
         // barrier 2: everybody's stores (to everybody) have landed
-        CKL(h) ck_xbarrier_kernel<<<1, 32, 0, h->stream>>>(h->peers, rank, world, flags_off, 1, step, h->d_x_overflow + CK_X_MAXWORLD);
+        CKL(h) ck_xbarrier_kernel<<<1, 32, 0, h->stream>>>(h->peers, rank, world, flags_off, 1, step, h->d_x_overflow.p + CK_X_MAXWORLD);
         CUDA_TRY(h, cudaGetLastError());
     }
     return 0;
@@ -1562,8 +1506,8 @@ static int exchange_send_on_stream(ck_handle* h, uint64_t step) {
 // what this rank received (after the caller's closing barrier): per source rank the header {step, count, overflow, bytes};
 // ck_recv_buffer gives the device address and layout for in-place use, ck_fetch_received copies region `src` to the host
 extern "C" int ck_recv_info(ck_handle* h, void** dev_recv, uint64_t* region_stride, uint32_t* max_fwd, uint64_t* data_cap) {
-    if (!h->d_recv) return fail(h, "ck_recv_info: call ck_comm_create first");
-    if (dev_recv) *dev_recv = h->d_recv;
+    if (!h->d_recv.p) return fail(h, "ck_recv_info: call ck_comm_create first");
+    if (dev_recv) *dev_recv = h->d_recv.p;
     if (region_stride) *region_stride = h->region_stride;
     if (max_fwd) *max_fwd = h->max_fwd;
     if (data_cap) *data_cap = h->region_data_cap;
@@ -1571,13 +1515,13 @@ extern "C" int ck_recv_info(ck_handle* h, void** dev_recv, uint64_t* region_stri
 }
 extern "C" int ck_fetch_received(ck_handle* h, uint32_t src, uint64_t* hdr4 /* step, count, overflow, nbytes */, uint8_t* host_meta, uint8_t* host_data, uint64_t data_cap) {
     cudaSetDevice(h->device);
-    if (!h->d_recv || src >= h->comm_world) return fail(h, "ck_fetch_received: no such region");
-    const u8* region = h->d_recv + (size_t)src * h->region_stride;
+    if (!h->d_recv.p || src >= h->comm_world) return fail(h, "ck_fetch_received: no such region");
+    const u8* region = h->d_recv.p + (size_t)src * h->region_stride;
     ck_xregion_hdr hd{};
     CUDA_TRY(h, cudaMemcpyAsync(&hd, region, sizeof hd, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     hdr4[0] = hd.step; hdr4[1] = hd.count; hdr4[2] = hd.overflow; hdr4[3] = hd.nbytes;
-    { u32 to = 0; CUDA_TRY(h, cudaMemcpy(&to, h->d_x_overflow + CK_X_MAXWORLD, sizeof to, cudaMemcpyDeviceToHost)); if (to) return fail(h, "exchange barrier timed out: a peer did not arrive"); }
+    { u32 to = 0; CUDA_TRY(h, cudaMemcpy(&to, h->d_x_overflow.p + CK_X_MAXWORLD, sizeof to, cudaMemcpyDeviceToHost)); if (to) return fail(h, "exchange barrier timed out: a peer did not arrive"); }
     if (hd.nbytes > data_cap) return fail(h, "ck_fetch_received: host buffer too small");
     if (host_meta && hd.count) CUDA_TRY(h, cudaMemcpyAsync(host_meta, region + CK_X_HDR, sizeof(ck_xmeta) * (size_t)hd.count, cudaMemcpyDeviceToHost, h->stream));
     if (host_data && hd.nbytes) CUDA_TRY(h, cudaMemcpyAsync(host_data, region + CK_X_HDR + (size_t)h->max_fwd * sizeof(ck_xmeta), hd.nbytes, cudaMemcpyDeviceToHost, h->stream));
@@ -1590,12 +1534,12 @@ extern "C" int ck_fetch_received(ck_handle* h, uint32_t src, uint64_t* hdr4 /* s
 // page-locked memory and returns; they are complete after the next ck_sync
 extern "C" int ck_peek_received(ck_handle* h, uint64_t* hdr4 /* [world][4]: step, count, overflow, nbytes */) {
     cudaSetDevice(h->device);
-    if (!h->d_recv) return fail(h, "ck_peek_received: call ck_comm_create first");
+    if (!h->d_recv.p) return fail(h, "ck_peek_received: call ck_comm_create first");
     ck_xregion_hdr hd[CK_X_MAXWORLD];
-    CUDA_TRY(h, cudaMemcpy2DAsync(hd, sizeof(ck_xregion_hdr), h->d_recv, h->region_stride, sizeof(ck_xregion_hdr), h->comm_world,
+    CUDA_TRY(h, cudaMemcpy2DAsync(hd, sizeof(ck_xregion_hdr), h->d_recv.p, h->region_stride, sizeof(ck_xregion_hdr), h->comm_world,
                                   cudaMemcpyDeviceToHost, h->stream));
     u32 to = 0;
-    CUDA_TRY(h, cudaMemcpyAsync(&to, h->d_x_overflow + CK_X_MAXWORLD, sizeof to, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&to, h->d_x_overflow.p + CK_X_MAXWORLD, sizeof to, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (to) return fail(h, "exchange barrier timed out: a peer did not arrive");
     for (u32 r = 0; r < h->comm_world; r++) {
@@ -1605,9 +1549,9 @@ extern "C" int ck_peek_received(ck_handle* h, uint64_t* hdr4 /* [world][4]: step
 }
 extern "C" int ck_fetch_received_async(ck_handle* h, uint32_t src, uint64_t count, uint64_t nbytes, uint8_t* host_meta, uint8_t* host_data) {
     cudaSetDevice(h->device);
-    if (!h->d_recv || src >= h->comm_world) return fail(h, "ck_fetch_received_async: no such region");
+    if (!h->d_recv.p || src >= h->comm_world) return fail(h, "ck_fetch_received_async: no such region");
     if (count > h->max_fwd || nbytes > h->region_data_cap) return fail(h, "ck_fetch_received_async: count / nbytes beyond the region");
-    const u8* region = h->d_recv + (size_t)src * h->region_stride;
+    const u8* region = h->d_recv.p + (size_t)src * h->region_stride;
     if (host_meta && count) CUDA_TRY(h, cudaMemcpyAsync(host_meta, region + CK_X_HDR, sizeof(ck_xmeta) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
     if (host_data && nbytes) CUDA_TRY(h, cudaMemcpyAsync(host_data, region + CK_X_HDR + (size_t)h->max_fwd * sizeof(ck_xmeta), nbytes, cudaMemcpyDeviceToHost, h->stream));
     return 0;
@@ -1625,39 +1569,39 @@ extern "C" int ck_exchange_plan(ck_handle* h, uint32_t rank, uint32_t world, con
     u32 nb = (npubs + CK_X_BLOCK - 1) / CK_X_BLOCK;
     for (u32 d = 0; d < world; d++) { host_counts[d] = 0; host_nbytes[d] = 0; }
     *n_sel = 0;
-    if (dev_src_off) *dev_src_off = (const int64_t*)h->d_x_src_off;
-    if (dev_len) *dev_len = (const int64_t*)h->d_x_len;
-    if (dev_dst_off) *dev_dst_off = (const int64_t*)h->d_x_dst_off;
-    if (dev_pub) *dev_pub = h->d_x_pub;
+    if (dev_src_off) *dev_src_off = (const int64_t*)h->d_x_src_off.p;
+    if (dev_len) *dev_len = (const int64_t*)h->d_x_len.p;
+    if (dev_dst_off) *dev_dst_off = (const int64_t*)h->d_x_dst_off.p;
+    if (dev_pub) *dev_pub = h->d_x_pub.p;
     if (!nb) return 0;
     u32 nh = world * nb;
     {
         KTimer t(h, CK_K_ROUTE);
-        CUDA_TRY(h, cudaMemsetAsync(h->d_x_nbytes, 0, sizeof(unsigned long long) * CK_X_MAXWORLD, h->stream));
-        CKL(h) ck_xplan_count_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs, npubs, h->d_pay_len, rank, world, h->d_x_hist, h->d_x_nbytes);
+        CUDA_TRY(h, cudaMemsetAsync(h->d_x_nbytes.p, 0, sizeof(unsigned long long) * CK_X_MAXWORLD, h->stream));
+        CKL(h) ck_xplan_count_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs.p, npubs, h->d_pay_len.p, rank, world, h->d_x_hist.p, h->d_x_nbytes.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (run_scan(h, h->d_x_hist, nh, h->d_x_base, 0, h->d_x_tile, h->d_x_grand)) return 1;
+    if (run_scan(h, h->d_x_hist.p, nh, h->d_x_base.p, 0, h->d_x_tile.p, h->d_x_grand.p)) return 1;
     // first slot of every destination (= base[d * nb]), the total, and the bytes per destination
-    CUDA_TRY(h, cudaMemcpy2DAsync(h->h_x, sizeof(long long), h->d_x_base, sizeof(long long) * nb, sizeof(long long), world,
+    CUDA_TRY(h, cudaMemcpy2DAsync(h->h_x.p, sizeof(long long), h->d_x_base.p, sizeof(long long) * nb, sizeof(long long), world,
                                   cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_x + CK_X_MAXWORLD, h->d_x_nbytes, sizeof(long long) * world, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_x + 2 * CK_X_MAXWORLD, h->d_x_grand, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_x.p + CK_X_MAXWORLD, h->d_x_nbytes.p, sizeof(long long) * world, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->h_x.p + 2 * CK_X_MAXWORLD, h->d_x_grand.p, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    long long total = h->h_x[2 * CK_X_MAXWORLD];
+    long long total = h->h_x.p[2 * CK_X_MAXWORLD];
     for (u32 d = 0; d < world; d++) {
-        long long next = d + 1 < world ? h->h_x[d + 1] : total;
-        host_counts[d] = next - h->h_x[d];
-        host_nbytes[d] = h->h_x[CK_X_MAXWORLD + d];
+        long long next = d + 1 < world ? h->h_x.p[d + 1] : total;
+        host_counts[d] = next - h->h_x.p[d];
+        host_nbytes[d] = h->h_x.p[CK_X_MAXWORLD + d];
     }
     *n_sel = (u32)total;
     {
         KTimer t(h, CK_K_ROUTE);
-        CKL(h) ck_xplan_scatter_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs, npubs, h->d_pay_len, h->d_out_off, rank, world, h->d_x_base,
-                                                                  h->d_x_src_off, h->d_x_len, h->d_x_len32, h->d_x_pub);
+        CKL(h) ck_xplan_scatter_kernel<<<nb, CK_X_BLOCK, 0, h->stream>>>(h->d_pubs.p, npubs, h->d_pay_len.p, h->d_out_off.p, rank, world, h->d_x_base.p,
+                                                                  h->d_x_src_off.p, h->d_x_len.p, h->d_x_len32.p, h->d_x_pub.p);
         CUDA_TRY(h, cudaGetLastError());
     }
-    if (total && run_scan(h, h->d_x_len32, (u32)total, h->d_x_dst_off, 0, h->d_x_tile, h->d_x_grand)) return 1;
+    if (total && run_scan(h, h->d_x_len32.p, (u32)total, h->d_x_dst_off.p, 0, h->d_x_tile.p, h->d_x_grand.p)) return 1;
     return 0;
 }
 
@@ -1671,12 +1615,12 @@ extern "C" int ck_sync(ck_handle* h) {
 
 extern "C" int ck_out_size(ck_handle* h, uint64_t* out_bytes, uint32_t* n_payloads, uint32_t* n_publishes) {
     cudaSetDevice(h->device);
-    *h->h_grand = 0;
+    *h->h_grand.p = 0;
     if (h->n_payloads) {
-        CUDA_TRY(h, cudaMemcpyAsync(h->h_grand, h->d_grand, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+        CUDA_TRY(h, cudaMemcpyAsync(h->h_grand.p, h->d_grand.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
     }
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (out_bytes) *out_bytes = *h->h_grand;
+    if (out_bytes) *out_bytes = *h->h_grand.p;
     if (n_payloads) *n_payloads = h->n_payloads;
     if (n_publishes) *n_publishes = h->n_pubs;
     return 0;
@@ -1684,7 +1628,7 @@ extern "C" int ck_out_size(ck_handle* h, uint64_t* out_bytes, uint32_t* n_payloa
 
 extern "C" int ck_fetch_columns(ck_handle* h, uint32_t* host_cols) {
     cudaSetDevice(h->device);
-    CUDA_TRY(h, cudaMemcpyAsync(host_cols, h->d_cols, sizeof(u32) * (size_t)CK_NUM_COLS * h->n, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_cols, h->d_cols.p, sizeof(u32) * (size_t)CK_NUM_COLS * h->n, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1697,7 +1641,7 @@ static int fetch_cols_impl(ck_handle* h, const uint32_t* which, uint32_t k, uint
     cudaSetDevice(h->device);
     for (uint32_t j = 0; j < k; j++) {
         if (which[j] >= CK_NUM_COLS) return fail(h, "ck_fetch_cols: no such column");
-        if (h->n) CUDA_TRY(h, cudaMemcpyAsync(host_rows + (size_t)j * h->n, h->d_cols + (size_t)which[j] * h->n, sizeof(u32) * (size_t)h->n,
+        if (h->n) CUDA_TRY(h, cudaMemcpyAsync(host_rows + (size_t)j * h->n, h->d_cols.p + (size_t)which[j] * h->n, sizeof(u32) * (size_t)h->n,
                                              cudaMemcpyDeviceToHost, h->stream));
     }
     if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1708,7 +1652,7 @@ static int fetch_cols_impl(ck_handle* h, const uint32_t* which, uint32_t k, uint
 extern "C" int ck_canon_stats(ck_handle* h, uint32_t* n_listed, uint64_t* overlay_bytes) {
     cudaSetDevice(h->device);
     ck_canon_ctl c{};
-    if (h->n) CUDA_TRY(h, cudaMemcpyAsync(&c, h->d_canon_ctl, sizeof c, cudaMemcpyDeviceToHost, h->stream));
+    if (h->n) CUDA_TRY(h, cudaMemcpyAsync(&c, h->d_canon_ctl.p, sizeof c, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (n_listed) *n_listed = c.count;
     if (overlay_bytes) *overlay_bytes = c.cursor;
@@ -1732,10 +1676,10 @@ static int fetch_output_impl(ck_handle* h, uint8_t* host_out, uint64_t cap, int6
     if (ck_out_size(h, &total, nullptr, nullptr)) return 1;
     if (total > cap) return fail(h, "ck_fetch_output: host buffer too small");
     if (total > h->max_out) return fail(h, "ck_fetch_output: device output buffer overflowed (raise max_out_bytes)");
-    if (host_out && total) CUDA_TRY(h, cudaMemcpyAsync(host_out, h->d_out, total, cudaMemcpyDeviceToHost, h->stream));
-    if (host_out_off && h->n_payloads) CUDA_TRY(h, cudaMemcpyAsync(host_out_off, h->d_out_off, sizeof(long long) * ((size_t)h->n_payloads + 1), cudaMemcpyDeviceToHost, h->stream));
-    if (host_out_len && h->n_payloads) CUDA_TRY(h, cudaMemcpyAsync(host_out_len, h->d_pay_len, sizeof(u32) * (size_t)h->n_payloads, cudaMemcpyDeviceToHost, h->stream));
-    if (host_pubs && h->n_pubs) CUDA_TRY(h, cudaMemcpyAsync(host_pubs, h->d_pubs, sizeof(ck_pub) * (size_t)h->n_pubs, cudaMemcpyDeviceToHost, h->stream));
+    if (host_out && total) CUDA_TRY(h, cudaMemcpyAsync(host_out, h->d_out.p, total, cudaMemcpyDeviceToHost, h->stream));
+    if (host_out_off && h->n_payloads) CUDA_TRY(h, cudaMemcpyAsync(host_out_off, h->d_out_off.p, sizeof(long long) * ((size_t)h->n_payloads + 1), cudaMemcpyDeviceToHost, h->stream));
+    if (host_out_len && h->n_payloads) CUDA_TRY(h, cudaMemcpyAsync(host_out_len, h->d_pay_len.p, sizeof(u32) * (size_t)h->n_payloads, cudaMemcpyDeviceToHost, h->stream));
+    if (host_pubs && h->n_pubs) CUDA_TRY(h, cudaMemcpyAsync(host_pubs, h->d_pubs.p, sizeof(ck_pub) * (size_t)h->n_pubs, cudaMemcpyDeviceToHost, h->stream));
     if (wait) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1754,13 +1698,13 @@ extern "C" int ck_fetch_overlay(ck_handle* h, uint8_t* host_ovl, uint64_t cap, i
     cudaSetDevice(h->device);
     if (!h->n) { if (used) *used = 0; return 0; }
     long long total = 0;
-    CUDA_TRY(h, cudaMemcpyAsync(&total, &h->d_canon_ctl->cursor, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(host_off, h->d_ovl_off, sizeof(long long) * (size_t)h->n, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(host_len, h->d_ovl_len, sizeof(u32) * (size_t)h->n, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&total, &h->d_canon_ctl.p->cursor, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_off, h->d_ovl_off.p, sizeof(long long) * (size_t)h->n, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_len, h->d_ovl_len.p, sizeof(u32) * (size_t)h->n, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if ((uint64_t)total > h->max_ovl) total = (long long)h->max_ovl;
     if ((uint64_t)total > cap) return fail(h, "ck_fetch_overlay: host buffer too small");
-    if (total) CUDA_TRY(h, cudaMemcpyAsync(host_ovl, h->d_ovl, (size_t)total, cudaMemcpyDeviceToHost, h->stream));
+    if (total) CUDA_TRY(h, cudaMemcpyAsync(host_ovl, h->d_ovl.p, (size_t)total, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (used) *used = (uint64_t)total;
     return 0;
@@ -1769,7 +1713,7 @@ extern "C" int ck_fetch_overlay(ck_handle* h, uint8_t* host_ovl, uint64_t cap, i
 extern "C" int ck_fetch_topic_hist(ck_handle* h, uint32_t* host_hist, uint32_t n) {
     cudaSetDevice(h->device);
     if (n > h->hist_cap) n = h->hist_cap;
-    CUDA_TRY(h, cudaMemcpyAsync(host_hist, h->d_topic_hist, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(host_hist, h->d_topic_hist.p, sizeof(u32) * n, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1777,18 +1721,18 @@ extern "C" int ck_fetch_topic_hist(ck_handle* h, uint32_t* host_hist, uint32_t n
 extern "C" void* ck_stream(ck_handle* h) { return (void*)h->stream; }
 
 extern "C" int ck_device_buffers2(ck_handle* h, void** pubs, void** pay_len, void** descs) {
-    if (pubs) *pubs = h->d_pubs;
-    if (pay_len) *pay_len = h->d_pay_len;
-    if (descs) *descs = h->d_descs;
+    if (pubs) *pubs = h->d_pubs.p;
+    if (pay_len) *pay_len = h->d_pay_len.p;
+    if (descs) *descs = h->d_descs.p;
     return 0;
 }
 
 extern "C" int ck_device_buffers(ck_handle* h, void** in, void** in_off, void** out, void** out_off, void** cols) {
-    if (in) *in = h->d_in;
-    if (in_off) *in_off = h->d_in_off;
-    if (out) *out = h->d_out;
-    if (out_off) *out_off = h->d_out_off;
-    if (cols) *cols = h->d_cols;
+    if (in) *in = h->d_in.p;
+    if (in_off) *in_off = h->d_in_off.p;
+    if (out) *out = h->d_out.p;
+    if (out_off) *out_off = h->d_out_off.p;
+    if (cols) *cols = h->d_cols.p;
     return 0;
 }
 
