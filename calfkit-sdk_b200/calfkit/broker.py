@@ -30,7 +30,8 @@ Kafka's own granularity — record batches — at both ends:
     the engine's record form at `flush_frames` (the Worker calls it once per step and installs the `framer`).  There is no
     CPU encoder: without a framer, flushing them fails loudly.  `MemoryBroker(compression_type="lz4")` (the keyword a
     FastStream KafkaBroker takes) makes every frame an LZ4-compressed batch, compressed on the device; other codecs are
-    refused by the Worker when frame sinks are registered.
+    refused by the Worker when frame sinks are registered.  `compression_level=` (Kafka's compression.lz4.level, 1 .. 17)
+    trades compressor time for smaller LZ4 frames: 1 and 2 build the default frames, 3 and up search deeper per level.
 Idempotent and transactional produce (KIP-98), as aiokafka and the Java producer apply `enable_idempotence=True` and
 `transactional_id="..."` (which implies idempotence): `init_producer_id` hands out producer ids and epochs; every frame
 carries its producer's id and epoch, and the broker writes its baseSequence when it hands the frame to its sink, from one
@@ -100,6 +101,9 @@ class MemoryBroker:
         # the codec of the frames handed to frame sinks, as KafkaBroker(compression_type=...) takes it: None or "lz4"
         # (compressed on the device); the Worker refuses any other codec when frame sinks are registered
         self.compression_type: str | None = kwargs.get("compression_type")
+        # compression.lz4.level (KIP-390) as KafkaBroker(compression_level=...) would take it: 1 .. 17, None the default;
+        # the Worker checks it and applies it to LZ4 frames only, as Kafka ignores it for other codecs
+        self.compression_level: int | None = kwargs.get("compression_level")
         self.num_partitions = num_partitions       # partitions per topic (Kafka's default partitioner: murmur2(key) % partitions)
         # idempotent / transactional produce (frame sinks): KafkaBroker(enable_idempotence=True) / (transactional_id="...")
         self.transactional_id: str | None = kwargs.get("transactional_id")

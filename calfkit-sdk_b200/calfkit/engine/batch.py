@@ -23,6 +23,15 @@ from calfkit.exceptions import EngineError
 
 # frame codecs the device builds, by the name Kafka clients use (KafkaBroker(compression_type=...)) -> Kafka's codec id
 FRAME_CODECS = {None: 0, "lz4": 3}
+# the levels of LZ4 frames (Kafka's compression.lz4.level, KIP-390): 1 .. 17; None is the default parse
+LZ4_LEVELS = range(1, 18)
+
+
+def check_compression_level(level) -> int | None:
+    """`level` when it is None or an int in LZ4_LEVELS; else EngineError naming it"""
+    if level is not None and (type(level) is not int or level not in LZ4_LEVELS):
+        raise EngineError(f"compression level {level!r} is not supported (None or an int in 1 .. 17)")
+    return level
 
 # what a Kafka consumer's `isolation_level` takes: read_committed hides the records of aborted transactions (csrc/ck_txn.h)
 ISOLATION_LEVELS = ("read_uncommitted", "read_committed")
@@ -514,12 +523,16 @@ class BatchEngine:
         """the frame split window W: a frame holds at most 61 + W + one record bytes (default 1 MiB)"""
         self._check(self.lib.ck_set_option(self.h, 2, window))
 
-    def set_frame_compression(self, codec: str | None) -> None:
+    def set_frame_compression(self, codec: str | None, level: int | None = None) -> None:
         """the codec of the frames the frame passes build: None (uncompressed, the default) or "lz4" (Kafka codec 3: the
-        records section of every frame is one LZ4 frame of independent 64 KB blocks, compressed on the device)"""
+        records section of every frame is one LZ4 frame of independent 64 KB blocks, compressed on the device).  `level`
+        (compression.lz4.level, 1 .. 17; None: the default parse) picks the LZ4 parse: 1 and 2 give the default's bytes,
+        3 and up a hash-chain search that deepens with the level (ck_set_option 4).  It has no effect on other codecs"""
+        check_compression_level(level)
         if codec not in FRAME_CODECS:
             raise EngineError(f"frame compression {codec!r} is not supported (None or 'lz4')")
         self._check(self.lib.ck_set_option(self.h, 3, FRAME_CODECS[codec]))
+        self._check(self.lib.ck_set_option(self.h, 4, level or 0))
 
     def set_producer(self, pid: int, epoch: int, transactional: bool = False) -> None:
         """the producer fields of the frames the following passes build (ck_set_producer): pid -1 none (producerId and

@@ -45,7 +45,7 @@ import numpy as np
 from calfkit.broker import Record
 from calfkit.client import Client
 from calfkit.engine import BatchEngine
-from calfkit.engine.batch import FRAME_CODECS, ISOLATION_LEVELS
+from calfkit.engine.batch import FRAME_CODECS, ISOLATION_LEVELS, check_compression_level
 from calfkit.engine._lib import CK_ACT_RAISES, CK_OK, CK_SKIPPED, CK_UNSUPPORTED, STATUS_NAMES
 from calfkit.exceptions import EngineError
 from calfkit.engine.lane import FetchArena, FetchRecords, LanePipeline, PublishBatch
@@ -166,6 +166,7 @@ class Worker:
             frame_topics = list(self._client._connection.frame_sinks)
             topics = list(node.subscribe_topics) + ([node.publish_topic] if node.publish_topic else []) + self._route_topics + frame_topics
             codec = self._frame_codec() if frame_topics else None
+            clevel = self._frame_level(codec) if frame_topics else None
             level = self._levels.get(id(node), "read_uncommitted")
             producer = self._producer_of(self._client._connection) if frame_topics else None
 
@@ -175,7 +176,7 @@ class Worker:
                 eng.set_isolation_level(level)
                 if frame_topics:
                     eng.set_frame_topics(frame_topics)
-                    eng.set_frame_compression(codec)
+                    eng.set_frame_compression(codec, clevel)
                     if producer is not None:
                         eng.set_producer(*producer)
             pipe = LanePipeline(self._device, configure, lanes=self._lanes, max_records=self._batch_records,
@@ -301,6 +302,12 @@ class Worker:
             raise EngineError(f"frame sinks: compression_type {codec!r} is not built on the device (None or 'lz4')")
         return codec
 
+    def _frame_level(self, codec: str | None) -> int | None:
+        """the broker's compression_level for the frames of `codec`: checked whatever the codec, applied to LZ4 frames
+        only (Kafka ignores compression.lz4.level for other codecs)"""
+        level = check_compression_level(getattr(self._client._connection, "compression_level", None))
+        return level if codec == "lz4" else None
+
     def _frame_records(self, topic: str, records: list[Record]):
         """the engine's record form over Records produced to a frame-sink topic by host paths, in engine-sized chunks"""
         broker = self._client._connection
@@ -308,7 +315,8 @@ class Worker:
             from calfkit.engine.lane import PinnedPool
             self._framer_eng = BatchEngine(self._device, max_records=self._batch_records, max_in_bytes=self._batch_bytes)
             self._framer_eng.register_topics(list(broker.frame_sinks), num_partitions=getattr(broker, "num_partitions", 0))
-            self._framer_eng.set_frame_compression(self._frame_codec())
+            codec = self._frame_codec()
+            self._framer_eng.set_frame_compression(codec, self._frame_level(codec))
             producer = self._producer_of(broker)
             if producer is not None:
                 self._framer_eng.set_producer(*producer)

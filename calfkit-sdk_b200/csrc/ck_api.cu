@@ -95,6 +95,9 @@ struct ck_handle {
     // each fr_raw_cap bytes (0 until lz_grow has reserved every buffer); per block slot its size and their scan; the
     // offsets of the compressed frames
     u32 fr_codec = 0, fr_pass_codec = 0;             // option 3, and the codec of the last pass
+    // compression level (option 4; 0 = the default parse) and the level of the last pass; the chains of the hash-chain
+    // parse (ck_lz4_block_hc), one per warp of its fixed grid (allocated on the first pass at a level that uses it)
+    u32 fr_level = 0, fr_pass_level = 0; ck_buf<uint16_t> d_fr_chain;
     ck_buf<u8> d_fr_raw; uint64_t fr_raw_cap = 0; u32 fr_bmax = 0; ck_buf<u32> d_fr_bsize;
     ck_buf<long long> d_fr_bscan, d_fr_zoff; ck_buf<unsigned long long> d_fr_btile;
     // exchange planning (allocated on first use)
@@ -678,6 +681,14 @@ extern "C" int ck_set_option(ck_handle* h, uint32_t option, uint64_t value) {
         if (value != 0 && value != 3) return fail(h, "ck_set_option: frame codec must be 0 (none) or 3 (lz4)");
         h->fr_codec = (u32)value; return 0;
     }
+    if (option == 4) {
+        if (value > CK_LZ_LEVEL_MAX) {
+            char b[128];
+            snprintf(b, sizeof b, "ck_set_option: compression level %llu is outside 0 (default) .. %u", (unsigned long long)value, CK_LZ_LEVEL_MAX);
+            return fail(h, b);
+        }
+        h->fr_level = (u32)value; return 0;
+    }
     return fail(h, "ck_set_option: unknown option");
 }
 
@@ -993,9 +1004,11 @@ static int fr_alloc(ck_handle* h) {
 static int frame_write(ck_handle* h);
 static int lz_compress(ck_handle* h);
 static int frame_pass(ck_handle* h, u32 n, u32 passes, u32 excl, unsigned long long window, long long base_offset, long long ts) {
-    h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec; h->fr_prod = h->prod;
+    h->fr_n = n; h->fr_info = false; h->fr_sized = false; h->fr_pass_codec = h->fr_codec; h->fr_pass_level = h->fr_level; h->fr_prod = h->prod;
     if (!n) return 0;
     if (h->fr_pass_codec && !h->fr_raw_cap && lz_grow(h, h->fr_cap)) return 1;
+    if (h->fr_pass_codec && ck_lz_hc_depth[h->fr_pass_level])
+        CUDA_TRY(h, h->d_fr_chain.reserve((size_t)h->num_sms * CK_LZ_HC_CTAS_PER_SM * CK_LZ_WARPS * CK_LZ_BLOCK, h->stream));
     const u32* order = nullptr;
     if (passes) {
         if (group_alloc(h)) return 1;
@@ -1087,9 +1100,11 @@ static int lz_compress(ck_handle* h) {
     if (run_scan(h, h->d_fr_head.p, n, h->d_fr_gscan.p, 0, h->d_fr_tile.p, h->d_fr_grand.p, CK_K_LZ4)) return 1;
     {
         KTimer t(h, CK_K_LZ4);
-        u32 blocks = h->num_sms * 8;
-        CKL(h) ck_lz_compress_kernel<<<blocks, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_gscan.p, h->d_fr_F.p, n, h->d_fr_raw.p, slots,
-                                                                              h->fr_bmax, h->d_fr_bsize.p);
+        u32 depth = ck_lz_hc_depth[h->fr_pass_level];
+        if (!depth) CKL(h) ck_lz_compress_kernel<<<h->num_sms * 8, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_gscan.p, h->d_fr_F.p, n,
+                                                                                                  h->d_fr_raw.p, slots, h->fr_bmax, h->d_fr_bsize.p);
+        else CKL(h) ck_lz_compress_hc_kernel<<<h->num_sms * CK_LZ_HC_CTAS_PER_SM, CK_LZ_WARPS * 32, 0, h->stream>>>(h->d_fr_table.p, h->d_fr_gscan.p,
+            h->d_fr_F.p, n, h->d_fr_raw.p, slots, h->fr_bmax, h->d_fr_bsize.p, h->d_fr_chain.p, depth);
         CUDA_TRY(h, cudaGetLastError());
     }
     if (run_scan(h, h->d_fr_bsize.p, h->fr_bmax, h->d_fr_bscan.p, 0, h->d_fr_btile.p, h->d_fr_grand.p, CK_K_LZ4)) return 1;

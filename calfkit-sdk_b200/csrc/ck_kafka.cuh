@@ -641,8 +641,9 @@ ck_fr_crc_fold_kernel(const ck_frame_ent* __restrict__ table, const long long* _
 // turns each into a batch with attributes 3 (LZ4): header | 7-byte LZ4 frame header | blocks | end mark 00000000, where
 // the records section [61, end) of the uncompressed frame is cut into independent blocks of 64 KB (the last one shorter):
 //   blocks   thread per frame: block count; its scan gives every frame its first block
-//   lz4      warp per block (ck_lz4_block): compressed bytes into a slot at the block's own offset in a second scratch
-//            region, or none when they would not be smaller (the block is then stored raw, bit 31 of its size set)
+//   lz4      warp per block (ck_lz4_block, or ck_lz4_block_hc at a compression level of 3 and up, ck_set_option 4):
+//            compressed bytes into a slot at the block's own offset in a second scratch region, or none when they would not
+//            be smaller (the block is then stored raw, bit 31 of its size set)
 //   size     block sizes -> scan; frame lengths -> scan -> offsets of the compressed frames
 //   gather   warp per block: size word + bytes into the frame buffer; then thread per frame: header (attributes 3,
 //            batchLength), LZ4 frame header, end mark, the frame table's offset / length and the CRC chunk count
@@ -671,10 +672,14 @@ ck_lz_blocks_kernel(const ck_frame_ent* __restrict__ table, const long long* __r
     }
     nblk[f] = k;
 }
-// warps stride over the block slots 0 .. bmax: bsize[b] = 4 + bytes of block b as it goes out (0 past the last block)
-__global__ void __launch_bounds__(CK_LZ_WARPS * 32)
-ck_lz_compress_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B, const long long* __restrict__ F, u32 n,
-                      const u8* __restrict__ raw, u8* __restrict__ slots, u32 bmax, u32* __restrict__ bsize) {
+// warps stride over the block slots 0 .. bmax: bsize[b] = 4 + bytes of block b as it goes out (0 past the last block).
+// depth 0: the greedy parse (ck_lz4_block); else the hash-chain parse (ck_lz4_block_hc) with the chain of warp slot w at
+// chains + w * CK_LZ_BLOCK
+template <bool HC>
+__device__ __forceinline__ void ck_lz_compress_warps(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B,
+                                                     const long long* __restrict__ F, u32 n, const u8* __restrict__ raw,
+                                                     u8* __restrict__ slots, u32 bmax, u32* __restrict__ bsize,
+                                                     uint16_t* __restrict__ chains, u32 depth) {
     __shared__ uint16_t tabs[CK_LZ_WARPS][1u << CK_LZ_HBITS];
     u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = gridDim.x * CK_LZ_WARPS;
     u32 nf = (u32)F[n];
@@ -685,9 +690,23 @@ ck_lz_compress_kernel(const ck_frame_ent* __restrict__ table, const long long* _
         ck_frame_ent e = table[f];
         unsigned long long at = (unsigned long long)e.offset + CK_RB_HEADER + (b - (unsigned long long)B[f]) * CK_LZ_BLOCK;
         u32 len = (u32)min((unsigned long long)CK_LZ_BLOCK, (unsigned long long)(e.offset + e.length) - at);
-        u32 z = ck_lz4_block(raw + at, len, slots + at, tabs[wid], lane);
+        u32 z = HC ? ck_lz4_block_hc(raw + at, len, slots + at, tabs[wid], chains + (size_t)(blockIdx.x * CK_LZ_WARPS + wid) * CK_LZ_BLOCK, depth, lane)
+                   : ck_lz4_block(raw + at, len, slots + at, tabs[wid], lane);
         if (lane == 0) bsize[b] = 4u + (z ? z : len);
     }
+}
+__global__ void __launch_bounds__(CK_LZ_WARPS * 32)
+ck_lz_compress_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B, const long long* __restrict__ F, u32 n,
+                      const u8* __restrict__ raw, u8* __restrict__ slots, u32 bmax, u32* __restrict__ bsize) {
+    ck_lz_compress_warps<false>(table, B, F, n, raw, slots, bmax, bsize, nullptr, 0);
+}
+// the hash-chain parse runs on a fixed grid of CK_LZ_HC_CTAS_PER_SM CTAs per SM: one chain of CK_LZ_BLOCK u16 per warp
+#define CK_LZ_HC_CTAS_PER_SM 2u
+__global__ void __launch_bounds__(CK_LZ_WARPS * 32)
+ck_lz_compress_hc_kernel(const ck_frame_ent* __restrict__ table, const long long* __restrict__ B, const long long* __restrict__ F, u32 n,
+                         const u8* __restrict__ raw, u8* __restrict__ slots, u32 bmax, u32* __restrict__ bsize,
+                         uint16_t* __restrict__ chains, u32 depth) {
+    ck_lz_compress_warps<true>(table, B, F, n, raw, slots, bmax, bsize, chains, depth);
 }
 // thread per frame: compressed length (0: the frame has no blocks, it did not fit the scratch buffer); S = scan of bsize
 __global__ void __launch_bounds__(256)

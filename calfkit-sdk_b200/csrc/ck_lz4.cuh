@@ -39,6 +39,38 @@ __device__ __forceinline__ u32 ck_lz_put_seq(u8* __restrict__ d, const u8* __res
     return pos;
 }
 
+// The block rules a decoder enforces (both parses below keep them through the two helpers that follow): a match starts at
+// most at len - 12 and ends at most at len - 5 (the last 5 bytes are literals), the last sequence holds literals only,
+// offsets are 1 .. 65535 (a block holds at most 65536 positions).  ck_lz_room: the most a match at ms may run
+__device__ __forceinline__ u32 ck_lz_room(u32 len, u32 ms) { return len - 5u - ms; }
+// length of the match src[ms ..] = src[mc ..] of which ml bytes are known equal, extended by the warp 128 bytes per round
+// and held to the block rules
+__device__ __forceinline__ u32 ck_lz_extend(const u8* __restrict__ src, u32 len, u32 ms, u32 mc, u32 ml, u32 lane) {
+    u32 maxlen = ck_lz_room(len, ms);
+    while (ml < maxlen) {
+        u32 o = ml + 4u * lane;
+        bool in = o < maxlen;
+        u32 x = in ? ck_ld32u(src + ms + o) ^ ck_ld32u(src + mc + o) : 0u;
+        u32 stop = __ballot_sync(0xffffffffu, x != 0u || !in);
+        if (stop) {
+            u32 l = (u32)__ffs(stop) - 1u, xl = __shfl_sync(0xffffffffu, x, l);
+            ml += 4u * l + (xl ? ((u32)__ffs(xl) - 1u) >> 3 : 0u);
+            break;
+        }
+        ml += 128u;
+    }
+    return min(ml, maxlen);
+}
+// the sequence literals src[anchor, ms) + match (ms - off, ml; ml 0: the last sequence, literals only) appended at dst[op];
+// false when the block would reach cap bytes (it is then stored raw)
+__device__ __forceinline__ bool ck_lz_emit(u8* __restrict__ dst, u32& op, u32 cap, const u8* __restrict__ src, u32 anchor, u32 ms,
+                                           u32 off, u32 ml, u32 lane) {
+    u32 ll = ms - anchor;
+    if (op + 1u + ck_lz_len_bytes(ll) + ll + (ml ? 2u + ck_lz_len_bytes(ml - 4u) : 0u) > cap) return false;
+    op += ck_lz_put_seq(dst + op, src + anchor, ll, off, ml, lane);
+    return true;
+}
+
 // One LZ4 block of src[0, len), len <= 64 KB, compressed by one warp into dst (at most len - 1 bytes are written).  Returns
 // the compressed size, or 0 when it would not be smaller than len (the caller stores the block raw).
 // Greedy parse: the warp looks at the 32 positions p .. p+31 at once; each lane hashes its 4 bytes and takes the table's
@@ -46,8 +78,6 @@ __device__ __forceinline__ u32 ck_lz_put_seq(u8* __restrict__ d, const u8* __res
 // candidate matches starts the match; positions up to it enter the table (one writer per hash: the highest position),
 // the match is extended 128 bytes per round, and the literals before it and the match are written.  Every step is a
 // fixed function of the input: the output is deterministic.
-// Block rules a decoder enforces: a match starts at most len - 12, ends at most len - 5 (the last 5 bytes are literals),
-// the last sequence holds literals only, offsets are 1 .. 65535 (a block holds at most 65536 positions)
 __device__ __forceinline__ u32 ck_lz4_block(const u8* __restrict__ src, u32 len, u8* __restrict__ dst, uint16_t* __restrict__ tab, u32 lane) {
     if (len < 13u) return 0;                                   // no match can start: literals only, one byte longer
     for (u32 i = lane; i < (1u << CK_LZ_HBITS) / 2; i += 32) ((u32*)tab)[i] = 0u;
@@ -69,29 +99,86 @@ __device__ __forceinline__ u32 ck_lz4_block(const u8* __restrict__ src, u32 len,
         __syncwarp();
         if (!hits) { p += 32; continue; }
         u32 ms = p + f, mc = __shfl_sync(0xffffffffu, c, f);
-        u32 maxlen = len - 5u - ms, ml = 4;
-        while (ml < maxlen) {
-            u32 o = ml + 4u * lane;
-            bool in = o < maxlen;
-            u32 x = in ? ck_ld32u(src + ms + o) ^ ck_ld32u(src + mc + o) : 0u;
-            u32 stop = __ballot_sync(0xffffffffu, x != 0u || !in);
-            if (stop) {
-                u32 l = (u32)__ffs(stop) - 1u, xl = __shfl_sync(0xffffffffu, x, l);
-                ml += 4u * l + (xl ? ((u32)__ffs(xl) - 1u) >> 3 : 0u);
-                break;
-            }
-            ml += 128u;
-        }
-        ml = min(ml, maxlen);
-        u32 ll = ms - anchor;
-        if (op + 3u + ck_lz_len_bytes(ll) + ll + ck_lz_len_bytes(ml - 4u) > cap) return 0;
-        op += ck_lz_put_seq(dst + op, src + anchor, ll, ms - mc, ml, lane);
+        u32 ml = ck_lz_extend(src, len, ms, mc, 4u, lane);
+        if (!ck_lz_emit(dst, op, cap, src, anchor, ms, ms - mc, ml, lane)) return 0;
         anchor = p = ms + ml;
     }
-    u32 ll = len - anchor;
-    if (op + 1u + ck_lz_len_bytes(ll) + ll > cap) return 0;
-    op += ck_lz_put_seq(dst + op, src + anchor, ll, 0, 0, lane);
-    return op;
+    return ck_lz_emit(dst, op, cap, src, anchor, len, 0, 0, lane) ? op : 0;
+}
+
+// ---- hash-chain parse (compression levels 3 and up) ----------------------------------------------------------------------
+// Search depth by compression level (ck_set_option 4, Kafka's compression.lz4.level 1 .. 17): 0 = the greedy parse above
+// (levels 1 and 2 are liblz4's fast compressor, so they stay the default parse).  From level 3 the depth doubles per level,
+// as liblz4's HC levels 3 .. 9 search 4 .. 256 candidates, up to CK_LZ_HC_DEPTH_CAP at level 9; levels 10 .. 17 search as
+// level 9 does (liblz4 runs its optimal parser there; this parse stays the chain walk with the lazy step)
+#define CK_LZ_LEVEL_MAX 17u
+#define CK_LZ_HC_DEPTH_CAP 256u
+static const uint16_t ck_lz_hc_depth[CK_LZ_LEVEL_MAX + 1] = {0, 0, 0, 4, 8, 16, 32, 64, 128, 256, 256, 256, 256, 256, 256, 256, 256, 256};
+// a lane stops probing a candidate at this many equal bytes, and stops its walk at such a candidate (the nearest one of
+// that length): the chosen match is then extended by the warp (ck_lz_extend)
+#define CK_LZ_HC_NICE 64u
+
+// positions [from, to) (at most 32) enter the head table and the chain: chain[q] = q - the previous position with q's hash
+// (an earlier lane of the same round, else the head), 0 = none.  Every lane reads the head before any lane writes it
+__device__ __forceinline__ void ck_lz_hc_insert(const u8* __restrict__ src, u32 from, u32 to, uint16_t* __restrict__ tab,
+                                                uint16_t* __restrict__ chain, u32 lane) {
+    u32 q = from + lane;
+    bool valid = q < to;
+    u32 h = valid ? ck_lz_hash(ck_ld32u(src + q)) : ~0u;
+    u32 same = __match_any_sync(0xffffffffu, h) & __ballot_sync(0xffffffffu, valid);
+    u32 t = valid ? tab[h] : 0u, below = same & ((1u << lane) - 1u);
+    u32 prev = below ? from + 31u - (u32)__clz(below) : t ? t - 1u : q;
+    if (valid) chain[q] = (uint16_t)(q - prev);
+    __syncwarp();
+    if (valid && lane == 31u - (u32)__clz(same)) tab[h] = (uint16_t)(q + 1u);
+    __syncwarp();
+}
+
+// The same block contract as ck_lz4_block (one warp, len <= 64 KB, 0 = store raw, deterministic, the block rules) with a
+// hash-chain search: chain (CK_LZ_BLOCK entries, global memory of this warp alone) links each position to the previous one
+// with its hash, tab holds the last position per hash.  The warp looks at 32 positions per round, after every position up
+// to them has entered the chain; each lane walks its own position's chain through at most `depth` candidates and keeps the
+// longest match (the nearest among equals).  The first lane with a match starts it, unless the lane after it has a longer
+// one (the lazy step, taken again while it holds); the chosen match is extended by the warp and written.  Positions
+// inside a match enter the chain too, so later positions find them.  depth >= 1
+__device__ __forceinline__ u32 ck_lz4_block_hc(const u8* __restrict__ src, u32 len, u8* __restrict__ dst, uint16_t* __restrict__ tab,
+                                               uint16_t* __restrict__ chain, u32 depth, u32 lane) {
+    if (len < 13u) return 0;
+    for (u32 i = lane; i < (1u << CK_LZ_HBITS) / 2; i += 32) ((u32*)tab)[i] = 0u;
+    __syncwarp();
+    const u32 last = len - 12u, cap = len - 1u;
+    u32 p = 0, anchor = 0, op = 0, ins = 0;                    // positions below ins are in the chain
+    while (p <= last) {
+        for (u32 end = min(p + 32u, last + 1u); ins < end; ins = min(ins + 32u, end)) ck_lz_hc_insert(src, ins, min(ins + 32u, end), tab, chain, lane);
+        u32 q = p + lane, ml = 0, off = 0;
+        if (q <= last) {
+            u32 v = ck_ld32u(src + q), nice = min(ck_lz_room(len, q), CK_LZ_HC_NICE), c = q, d = chain[q];
+            for (u32 k = 0; k < depth && d; k++) {
+                c -= d;
+                if (ck_ld32u(src + c) == v) {
+                    u32 l = 4;
+                    while (l < nice) {
+                        u32 x = ck_ld32u(src + q + l) ^ ck_ld32u(src + c + l);
+                        if (x) { l += ((u32)__ffs(x) - 1u) >> 3; break; }
+                        l += 4u;
+                    }
+                    l = min(l, nice);
+                    if (l > ml) { ml = l; off = q - c; if (ml == nice) break; }
+                }
+                d = chain[c];
+            }
+        }
+        u32 hits = __ballot_sync(0xffffffffu, ml != 0u);
+        if (!hits) { p += 32; continue; }
+        u32 longer = __ballot_sync(0xffffffffu, __shfl_down_sync(0xffffffffu, ml, 1) > ml && lane < 31u);
+        u32 f = (u32)__ffs(hits) - 1u;
+        f += (u32)__ffs(~(longer >> f)) - 1u;                  // the lazy step: on while the next position's match is longer
+        u32 ms = p + f, mo = __shfl_sync(0xffffffffu, off, f);
+        u32 mlen = ck_lz_extend(src, len, ms, ms - mo, __shfl_sync(0xffffffffu, ml, f), lane);
+        if (!ck_lz_emit(dst, op, cap, src, anchor, ms, mo, mlen, lane)) return 0;
+        anchor = p = ms + mlen;
+    }
+    return ck_lz_emit(dst, op, cap, src, anchor, len, 0, 0, lane) ? op : 0;
 }
 
 // ---- decoding (lz4's doc/lz4_Frame_format.md and doc/lz4_Block_format.md) ------------------------------------------------

@@ -90,7 +90,12 @@ int  ck_submit_device(ck_handle* h, const uint8_t* dev_in, const int64_t* dev_of
  * attributes 3 whose records section is one LZ4 frame (descriptor 04224D18 60 40 82: independent 64 KB blocks, no
  * checksums), compressed on the device; a block that would not shrink is stored raw.  The split rule and the frame table
  * keep their meaning (W applies to the uncompressed records); ck_frames_size, ck_fetch_frames_async and the frame table
- * report the compressed frames, each at most its uncompressed length + 4 bytes per 64 KB block + 11 */
+ * report the compressed frames, each at most its uncompressed length + 4 bytes per 64 KB block + 11
+ * option 4 (compression level, Kafka's compression.lz4.level): the LZ4 parse of the following passes.  0 (default), 1 and 2:
+ * the greedy parse; 3 .. 17: a hash-chain search of 4 candidates per position at level 3, doubling per level up to 256 at
+ * level 9 and above, with a lazy step.  Any other value is refused.  It applies to LZ4 passes only; the frame format, and
+ * output that is byte-identical at 0, 1 and 2, do not change.  A pass keeps the level it was queued with (a rewrite into
+ * grown buffers uses it again) */
 int  ck_set_option(ck_handle* h, uint32_t option, uint64_t value);
 
 /* group the publish table of the current plan by destination topic on the device (stable two-pass radix sort over 12-bit
