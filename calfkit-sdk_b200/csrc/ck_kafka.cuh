@@ -144,11 +144,14 @@ ck_rb_crc_kernel(const u8* __restrict__ buf, const long long* __restrict__ batch
     if (lane == 0) batch_bad[w] = bad ? 1u : flag ? flag[w] : 0u;
 }
 
+// a zig-zag varint of at most 10 bytes whose unsigned value fits in 64 bits (a 10th byte above 1 is refused, as an exact
+// 64-bit reader refuses it); non-minimal encodings are accepted
 __device__ __forceinline__ bool ck_varint(const u8* __restrict__ p, u32& pos, u32 end, long long& out) {
     unsigned long long u = 0; u32 shift = 0;
     for (;;) {
-        if (pos >= end || shift > 63) return false;
+        if (pos >= end) return false;
         u8 b = p[pos++];
+        if (shift == 63 && b > 1) return false;
         u |= (unsigned long long)(b & 0x7f) << shift;
         if (!(b & 0x80)) break;
         shift += 7;
@@ -299,14 +302,17 @@ ck_rb_split_kernel(const u8* __restrict__ buf, const long long* __restrict__ bat
         if (!ok) { rec_pos[r0 + k] = -1; continue; }
         rec_pos[r0 + k] = lo + pos;
         long long len;
-        if (!ck_varint(f, pos, flen, len) || len < 0 || pos + (u32)len > flen) { ok = false; rec_pos[r0 + k] = -1; continue; }
+        // the length compared in 64 bits: narrowed first, 2^32 + L would pass as L
+        if (!ck_varint(f, pos, flen, len) || len < 0 || (unsigned long long)len > flen - pos) { ok = false; rec_pos[r0 + k] = -1; continue; }
         pos += (u32)len;
     }
     if (ok && pos != flen) ok = false;
     if (!ok && !st) batch_bad[b] = 1;
 }
 
-// thread per record
+// thread per record.  Every length is compared with the bytes left in the record as a 64-bit quantity before it is
+// narrowed; a negative key or value length is null, a negative header count or header key length is refused.  A refused
+// record keeps no span
 __global__ void __launch_bounds__(128)
 ck_rb_fields_kernel(const u8* __restrict__ buf, long long buf_len, const long long* __restrict__ rec_pos, const u32* __restrict__ rec_batch,
                     const u32* __restrict__ batch_bad, u32 n,
@@ -326,28 +332,30 @@ ck_rb_fields_kernel(const u8* __restrict__ buf, long long buf_len, const long lo
     if (ok) end = rec_end;
     pos += 1;                                                   // attributes
     ok = ok && ck_varint(p, pos, end, t) && ck_varint(p, pos, end, t);       // timestampDelta, offsetDelta
+    // after a varint is read, pos <= end
     ok = ok && ck_varint(p, pos, end, t);                       // key
+    ok = ok && (t < 0 || (unsigned long long)t <= end - pos);
     if (ok && t >= 0) { key_off[i] = rp + pos; key_len[i] = (int)t; pos += (u32)t; }
-    ok = ok && pos <= end && ck_varint(p, pos, end, t);         // value
+    ok = ok && ck_varint(p, pos, end, t);                       // value
+    ok = ok && (t < 0 || (unsigned long long)t <= end - pos);
     if (ok && t >= 0) { val_off[i] = rp + pos; val_len[i] = (u32)t; pos += (u32)t; }
     long long nh = 0;
-    ok = ok && pos <= end && ck_varint(p, pos, end, nh);
+    ok = ok && ck_varint(p, pos, end, nh) && nh >= 0;
     for (long long hcount = 0; ok && hcount < nh; hcount++) {
         long long kl, vl;
-        ok = ck_varint(p, pos, end, kl) && kl >= 0 && pos + (u32)kl <= end;
+        ok = ck_varint(p, pos, end, kl) && kl >= 0 && (unsigned long long)kl <= end - pos;
         if (!ok) break;
         u32 kpos = pos; pos += (u32)kl;
-        ok = ck_varint(p, pos, end, vl);
+        ok = ck_varint(p, pos, end, vl) && (vl < 0 || (unsigned long long)vl <= end - pos);
         if (!ok) break;
         bool is_corr = (kl == 14);                              // "correlation_id" (FastStream's header)
         const char* want = "correlation_id";
         for (u32 b = 0; is_corr && b < 14; b++) is_corr = (p[kpos + b] == (u8)want[b]);
         if (vl >= 0) { if (is_corr) { corr_off[i] = rp + pos; corr_len[i] = (int)vl; } pos += (u32)vl; }
-        ok = pos <= end;
     }
     ok = ok && pos == rec_end;
     rec_bad[i] = ok ? 0u : 1u;
-    if (!ok) { val_len[i] = 0; }
+    if (!ok) { val_off[i] = 0; val_len[i] = 0; key_off[i] = 0; key_len[i] = -1; corr_off[i] = 0; corr_len[i] = -1; }
 }
 
 // rec_bad[i]: 1 the record's batch failed a check, 2 the consumer does not deliver it (a control batch, or an aborted

@@ -95,11 +95,13 @@ static inline bool ck_txn_framed(const uint8_t* f, uint64_t flen, bool check_crc
     return !check_crc || ck_txn_crc32c(f + 21, flen - 21) == ck_txn_be32(f + 17);
 }
 
+// a zig-zag varint of at most 10 bytes whose unsigned value fits in 64 bits: a 10th byte above 1 is refused
 static inline bool ck_txn_varint(const uint8_t* p, uint64_t& pos, uint64_t end, int64_t& out) {
     uint64_t u = 0;
     for (uint32_t shift = 0;; shift += 7) {
-        if (pos >= end || shift > 63) return false;
+        if (pos >= end) return false;
         uint8_t b = p[pos++];
+        if (shift == 63 && b > 1) return false;
         u |= (uint64_t)(b & 0x7f) << shift;
         if (!(b & 0x80)) break;
     }

@@ -78,6 +78,21 @@ def test_hand_written_cases():
         assert txnmask.verdicts(buf, parts, rc) == kt.verdicts(buf, parts, rc)
 
 
+def test_control_record_length_varint_must_fit_64_bits():
+    """a control batch whose record length is a 10-byte varint with 2^64 added (a 10th byte of 2, lost by a reader that
+    keeps 64 bits) is bad; the same length padded to 10 bytes (a 10th byte of 0) is a well-formed marker"""
+    import kafka_record_cases as kc
+    from make_golden_lz4_batches import with_section
+    f = kt.control_batch(0, 7, kt.ABORT)
+    n, p = kb.get_varint(f, kb.HEADER_LEN)
+    assert p == kb.HEADER_LEN + 1 and n == len(f) - p
+    over = with_section(f, kc.overflow(n) + f[p:], 0)
+    padded = with_section(f, kc.varint(n, 10) + f[p:], 0)
+    assert txnmask.verdicts(over, [(0, [])], False) == [kt.BAD]
+    assert txnmask.verdicts(padded, [(0, [])], False) == [kt.SKIP]
+    assert kt.control_type(padded) == kt.ABORT
+
+
 def test_partitions_reset_state_and_bad_partitions_are_refused():
     """the same producer id aborted in partition 0 is not aborted in partition 1; partition starts out of order are
     refused, as is an entry naming no partition"""
